@@ -17,9 +17,10 @@ all-reduce of the timing / frame-count scalars.
 `e2e`     : the same metric through the host-buffer C-ABI call
             (fsk_b200_rx_batch_host): pinned host samples -> device -> records
             back on the host, copies inside the timed region.
-`roofline`: algorithmic bytes (4 + 20/frame_nsamples per sample, SURVEY.md 8d)
-            over the rx kernel's own CUDA-event time, against the measured HBM
-            copy bandwidth (MEASURED_PEAKS.json).
+`roofline`: algorithmic bytes (4 + 20/frame_nsamples per sample, DESIGN.md 4)
+            over the rx kernel's own CUDA-event time, against the HBM bandwidth in
+            MEASURED_PEAKS.json (hbm_gbs) when that file exists, else the H100 SXM
+            data-sheet 3.35 TB/s; `peak_source` says which.
 `configs` : the other BASELINE configurations (RTTY 45.45 @8 kHz, Bell103 300 baud with the
             reference's -f offset sweep and with AWGN, NOAA SAME per-GPU shard) and a noisy
             variant of the headline, each with its own value / kernel_ms / roofline fraction /
@@ -51,7 +52,9 @@ METRIC = "audio Msamples/s demodulated (batched streams)"
 def parse():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
-    ap.add_argument("--steps", type=int, default=5)
+    ap.add_argument("--steps", type=int, default=5,
+                    help="timed steps of the headline, of the host-buffer leg and passes of the CPU arm "
+                         "(`configs` entries use --config-steps)")
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--mode", default=os.environ.get("FSK_BENCH_MODE", "1200"))
@@ -63,7 +66,8 @@ def parse():
     ap.add_argument("--amplitude", type=float, default=1.0)
     ap.add_argument("--awgn", type=float, default=0.0, help="sigma of additive white gaussian noise on the headline")
     ap.add_argument("--offset", type=float, default=0.0, help="constant offset -f (the reference's --Xrxnoise)")
-    ap.add_argument("--e2e-streams", type=int, default=0, help="0 = the whole batch at N=1, 16384 per rank otherwise")
+    ap.add_argument("--e2e-streams", type=int, default=16384,
+                    help="streams per rank of the host-buffer leg (pinned float32 and int16 copies in host memory)")
     ap.add_argument("--cpu-streams", type=int, default=0, help="CPU sample size (0 = 64 per core, at most 8192)")
     ap.add_argument("--config-steps", type=int, default=3, help="timed steps for each entry of `configs`")
     ap.add_argument("--lanes", type=int, default=0)
@@ -73,6 +77,8 @@ def parse():
     ap.add_argument("--no-cpu", action="store_true")
     ap.add_argument("--no-configs", action="store_true")
     ap.add_argument("--only-config", default="", help="run only the `configs` entries whose key contains this")
+    ap.add_argument("--dump-outputs", default="", metavar="DIR",
+                    help="write the headline's last timed step's records to DIR/*.npy (see dump_outputs)")
     return ap.parse_args()
 
 
@@ -256,7 +262,7 @@ def peaks():
             return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "H100 SXM data sheet HBM3 bandwidth 3.35 TB/s (not measured)"
 
 
 def _code_only(text):
@@ -396,18 +402,20 @@ def time_rx(torch, dist, world, dev, eng, x, n, max_frames, frames, states, step
     barrier()
     if sampler:
         sampler.start()
-    kev = [(torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)) for _ in range(steps)]
-    t0, t1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    barrier()
-    t0.record()
-    for i in range(steps):
-        states.zero_()
-        kev[i][0].record()
-        eng.rx_batch(x, nsamples=n, max_frames=max_frames, frames=frames, states=states)
-        kev[i][1].record()
-    t1.record()
-    barrier()
-    clocks = sampler.stop() if sampler else None
+    try:
+        kev = [(torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)) for _ in range(steps)]
+        t0, t1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        barrier()
+        t0.record()
+        for i in range(steps):
+            states.zero_()
+            kev[i][0].record()
+            eng.rx_batch(x, nsamples=n, max_frames=max_frames, frames=frames, states=states)
+            kev[i][1].record()
+        t1.record()
+        barrier()
+    finally:
+        clocks = sampler.stop() if sampler else None
     ms_kernel = sum(e0.elapsed_time(e1) for e0, e1 in kev) / steps
     ms_step = t0.elapsed_time(t1) / steps
     if world > 1:
@@ -450,6 +458,28 @@ def summarize(mm, torch, dist, world, dev, wl, frames, states, ms_step, ms_kerne
         "searches_per_frame": srch_total / max(1.0, frames_total),
         "decode_check": {"streams": int(len(rows)), "fraction_exact": okfrac},
     }
+
+
+def dump_outputs(d, mm, torch, frames, states, max_bytes=64_000_000):
+    """What rx_batch returned in the last timed step, for comparing two builds output for output: the
+    stream-state records (states.npy, one column per STATE_DTYPE field) and the frame records
+    (frames.npy, one column per FRAME_DTYPE field, records past a stream's nframes zeroed) of a fixed,
+    seeded sample of streams small enough for `max_bytes` in all (rows.npy: their indices).
+    float64 keeps the 32-bit integer fields exact."""
+    S, F = frames.shape[0], frames.shape[1]
+    per_row = 8 * (F * len(mm.FRAME_DTYPE.names) + len(mm.STATE_DTYPE.names) + 1)
+    k = max(1, min(S, max_bytes // per_row))
+    rows = np.arange(S) if k == S else np.sort(np.random.default_rng(0).choice(S, k, replace=False))
+    idx = torch.from_numpy(rows).to(frames.device)
+    st = mm.states_to_numpy(states.index_select(0, idx))
+    fr = mm.frames_to_numpy(frames.index_select(0, idx))
+    st64 = np.stack([st[f].astype(np.float64) for f in mm.STATE_DTYPE.names], axis=-1)
+    fr64 = np.stack([fr[f].astype(np.float64) for f in mm.FRAME_DTYPE.names], axis=-1)
+    fr64[np.arange(F)[None, :] >= st["nframes"][:, None].astype(np.int64)] = 0.0
+    os.makedirs(d, exist_ok=True)
+    np.save(os.path.join(d, "states.npy"), st64)
+    np.save(os.path.join(d, "frames.npy"), fr64)
+    np.save(os.path.join(d, "rows.npy"), rows.astype(np.float64))
 
 
 def run_ours(a):
@@ -501,6 +531,8 @@ def run_ours(a):
     launches = mm.launch_count() - launches0 - a.warmup
     head = summarize(mm, torch, dist, world, dev, wl, frames, states, ms_step, ms_kernel,
                      clean=not (a.awgn or a.offset), peak=peak)
+    if a.dump_outputs and rank == 0:
+        dump_outputs(a.dump_outputs, mm, torch, frames, states)
     st = mm.states_to_numpy(states)
     value = head["value"]
     frame = wl.params.frame_nsamples
@@ -519,7 +551,7 @@ def run_ours(a):
     # ---- end to end through the host-buffer C ABI call
     e2e = None
     if not a.no_e2e:
-        E = min(a.e2e_streams or (S if world == 1 else 16384), S)
+        E = min(a.e2e_streams, S)
         hx = torch.empty((E, stride), dtype=torch.float32, pin_memory=True)
         hx.copy_(x[:E])
         hfr = torch.empty((E, max_frames, 5), dtype=torch.int32, pin_memory=True)
@@ -547,7 +579,7 @@ def run_ours(a):
                 dt = float(t[0])
             return dt
 
-        esteps = max(2, min(a.steps, 3))
+        esteps = a.steps
         dt = timed_host(lambda: eng.rx_batch_host(hx, nsamples=n, max_frames=max_frames, frames_out=hfr,
                                                   states_out=hst), esteps, 1)
         hs = hst.numpy().view(mm.STATE_DTYPE).reshape(-1)
@@ -584,7 +616,7 @@ def run_ours(a):
             import orc
             ncpu = cpu_sample_streams(a)
             hostx = np.ascontiguousarray(x[:min(128, S), :n].cpu().numpy())
-            cpu, both = cpu_measure(orc.Mode(a.mode, sample_rate=a.rate), hostx, n, ncpu, steps=5, warmup=1,
+            cpu, both = cpu_measure(orc.Mode(a.mode, sample_rate=a.rate), hostx, n, ncpu, steps=a.steps, warmup=1,
                                     want_port=True)
             cpu_best = both.get("port") if both.get("port") is not cpu else None
         except Exception as ex:  # the checker is optional for the number, never for the tests
@@ -593,10 +625,7 @@ def run_ours(a):
     # ---- the other BASELINE configurations
     configs = []
     if not a.no_configs:
-        del frames, states
-        if x is not wl.x:
-            del x
-        del wl
+        del frames, states, x, wl        # x may alias wl.x: both names must go for its memory to be freed
         torch.cuda.empty_cache()
         plan = [
             # key, mode, rate, streams, nsamples, amplitude, [(suffix, awgn, offset)]
@@ -648,7 +677,7 @@ def run_ours(a):
                                                  + (", AWGN sigma %.2f" % a.awgn if a.awgn else "")
                                                  + (", offset -%.2f" % a.offset if a.offset else "")),
                        "streams_per_gpu": S, "nsamples": n, "frame_nsamples": frame,
-                       "l2": "inputs (%.1f GB per GPU) far exceed the 126 MB L2; no flush needed" % (S * stride * 4 / 1e9),
+                       "l2": "inputs (%.1f GB per GPU) far exceed the 50 MB L2 of an H100; no flush needed" % (S * stride * 4 / 1e9),
                        "parallelism": "streams sharded over %d GPU(s); NCCL broadcast of the plan only" % world},
             "roofline": roofline, "cpu_baseline": cpu, "cpu_best_case": cpu_best, "e2e": e2e,
             "gpu_launches": int(launches),

@@ -1,5 +1,5 @@
 /*
- * fsk_b200.h -- C ABI of the B200-native FSK demodulation engine.
+ * fsk_b200.h -- C ABI of the H100-native (sm_90a) FSK demodulation engine.
  *
  * Part 1 is a drop-in for the reference's src/fsk.h (kamalmostafa/minimodem
  * v0.24): same type name, same public scalar fields, same five functions with
@@ -412,7 +412,7 @@ int fsk_b200_tx_batch(const fsk_b200_tx_config *cfg, const float *sin_table, uin
  * (shared-segment),fill=0> threads=64 ring=640 smem=23232 blocks=8192"; "" before the first launch). */
 const char *fsk_b200_engine_last_kernel(const fsk_b200_engine *e);
 
-/* Library / build information: "fsk_b200 <version> sm_100a". */
+/* Library / build information: "fsk_b200 <version> sm_90a". */
 const char *fsk_b200_version(void);
 /* Number of kernel launches issued by this library in this process. */
 unsigned long long fsk_b200_launch_count(void);

@@ -1,7 +1,7 @@
-"""minimodem_b200 -- B200-native batched FSK demodulation engine.
+"""minimodem_b200 -- H100-native (sm_90a) batched FSK demodulation engine.
 
 The product is the C-ABI shared library ``libfsk_b200.so`` (include/fsk_b200.h):
-C host code + hand-written CUDA kernels for sm_100a.  This package is the thin
+C host code + hand-written CUDA kernels for sm_90a.  This package is the thin
 Python binding over that ABI (ctypes; torch only provides device memory,
 streams and torch.distributed).  There is no CPU or PyTorch fallback: importing
 works anywhere, but every analysis call needs the library and a CUDA device and

@@ -112,7 +112,7 @@ ALLOW_NON_PRODUCT_LIBRARY = False
 
 
 def build(force=False):
-    """Compile libfsk_b200.so in-tree (nvcc, sm_100a; gcc for the host layer)."""
+    """Compile libfsk_b200.so in-tree (nvcc, sm_90a; gcc for the host layer)."""
     args = ["make", "-s", "-C", os.path.join(_HERE, "csrc")]
     if force:
         subprocess.check_call(args + ["clean"])
@@ -130,10 +130,10 @@ def lib():
                            "(make -C minimodem_b200/csrc); there is no CPU/PyTorch fallback" % LIB_PATH)
     L = C.CDLL(LIB_PATH)
     L.fsk_b200_version.restype = C.c_char_p
-    if b"sm_100a" not in L.fsk_b200_version() and not ALLOW_NON_PRODUCT_LIBRARY:
+    if b"sm_90a" not in L.fsk_b200_version() and not ALLOW_NON_PRODUCT_LIBRARY:
         # FSK_B200_LIB exists for tuning builds of the CUDA library; anything else (the tests' host
         # emulation of the kernels, tests/emu) must never stand in for it silently
-        raise RuntimeError("%s is not a build of the sm_100a library (%s); the binding refuses it"
+        raise RuntimeError("%s is not a build of the sm_90a library (%s); the binding refuses it"
                            % (LIB_PATH, L.fsk_b200_version().decode()))
     fp, u32p = C.POINTER(C.c_float), C.c_void_p
     L.fsk_plan_new.argtypes = [C.c_float] * 4

@@ -1,5 +1,5 @@
 /*
- * fsk_b200_device.cuh -- device functions of the B200 FSK engine.
+ * fsk_b200_device.cuh -- device functions of the FSK engine (sm_90a).
  *
  * Two basic implementations of the same arithmetic:
  *
@@ -1127,42 +1127,18 @@ __device__ __forceinline__ PfxLane pfx_lane(const fsk_b200_geom &geo, const fsk_
     return pl;
 }
 
-/* Two fp32 multiply-adds in one instruction (Blackwell FFMA2: fma.rn.f32x2 on 64-bit register pairs).  The
- * table build is bound by instruction issue, not by the FMA pipe, so halving the instruction count of its
- * inner sums is worth more than the pipe cycles. */
+/* A pair of fp32 lanes: even and odd samples summed side by side.  sm_90 has no paired fp32 FMA, so each
+ * half is one FFMA / FMUL with one rounding (round to nearest); the kernel is built with -fmad=false, so
+ * the explicit fma is the only contraction. */
 struct F2 {
     float lo, hi;
 };
-#ifndef FSK_EMU	/* inline PTX: the host emulation of the test harness brings its own */
-__device__ __forceinline__ F2 fma2(const F2 a, const F2 b, const F2 c)
-{
-    unsigned long long ua, ub, uc, ud;
-    asm("mov.b64 %0, {%1, %2};" : "=l"(ua) : "f"(a.lo), "f"(a.hi));
-    asm("mov.b64 %0, {%1, %2};" : "=l"(ub) : "f"(b.lo), "f"(b.hi));
-    asm("mov.b64 %0, {%1, %2};" : "=l"(uc) : "f"(c.lo), "f"(c.hi));
-    asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(ud) : "l"(ua), "l"(ub), "l"(uc));
-    F2 d;
-    asm("mov.b64 {%0, %1}, %2;" : "=f"(d.lo), "=f"(d.hi) : "l"(ud));
-    return d;
-}
-__device__ __forceinline__ F2 mul2(const F2 a, const F2 b)
-{
-    unsigned long long ua, ub, ud;
-    asm("mov.b64 %0, {%1, %2};" : "=l"(ua) : "f"(a.lo), "f"(a.hi));
-    asm("mov.b64 %0, {%1, %2};" : "=l"(ub) : "f"(b.lo), "f"(b.hi));
-    asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(ud) : "l"(ua), "l"(ub));
-    F2 d;
-    asm("mov.b64 {%0, %1}, %2;" : "=f"(d.lo), "=f"(d.hi) : "l"(ud));
-    return d;
-}
-#else		/* host emulation (tests/emu): the two halves one after the other, each with one rounding */
-static inline F2 fma2(const F2 a, const F2 b, const F2 c) { return F2{ fmaf(a.lo, b.lo, c.lo), fmaf(a.hi, b.hi, c.hi) }; }
-static inline F2 mul2(const F2 a, const F2 b) { return F2{ a.lo * b.lo, a.hi * b.hi }; }
-#endif
+__device__ __forceinline__ F2 fma2(const F2 a, const F2 b, const F2 c) { return F2{ fmaf(a.lo, b.lo, c.lo), fmaf(a.hi, b.hi, c.hi) }; }
+__device__ __forceinline__ F2 mul2(const F2 a, const F2 b) { return F2{ a.lo * b.lo, a.hi * b.hi }; }
 
 /* eight samples against both tones, phase counted from the first: (re, im) mark, (re, im) space.
  * loc[p][k] = the twiddles exp(-2 pi i b j / fftsize) of the sample pair j = 2p, 2p + 1, component
- * k = (re, im) mark, (re, im) space (j = 0: 1, 0, 1, 0), side by side as FFMA2 wants them.
+ * k = (re, im) mark, (re, im) space (j = 0: 1, 0, 1, 0), side by side as the paired sums (fma2) take them.
  * Even and odd samples are summed side by side and added at the end. */
 template <class LOC>
 __device__ __forceinline__ float4 pfx_local(const float4 a, const float4 b, const LOC &loc)
@@ -1222,10 +1198,10 @@ __device__ __forceinline__ void pfx_build(const float *ring, unsigned R, unsigne
     const float4 *tp = twc + pl.idx0;
     const unsigned step2 = 2u * pg.s4;
     float4 *row = pre + lane * pg.tstride;
-    /* the chunk-local twiddles in (vector) registers for the walk: as kernel parameters the compiler keeps
-     * them in uniform registers and then spends more instructions pairing those up for FFMA2 than the sums
-     * take; loaded from the block's shared copy through an address it cannot prove uniform, they are
-     * ordinary register pairs */
+    /* the chunk-local twiddles in ordinary registers for the walk, loaded from the block's shared copy
+     * through an address the compiler cannot prove uniform.  This layout was chosen for paired fp32
+     * instructions, which need register pairs; on sm_90 each half is a plain FFMA that could also read a
+     * uniform register, and whether kernel parameters would be faster here has not been measured. */
     float lc[4][4][2];
     {
 	const float4 *lp = loc_s + (lane & pg.zero);

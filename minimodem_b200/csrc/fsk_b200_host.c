@@ -1,5 +1,5 @@
 /*
- * fsk_b200_host.c -- host layer of the B200 FSK engine, plain C.
+ * fsk_b200_host.c -- host layer of the FSK engine, plain C.
  *
  *  - the drop-in for the reference's src/fsk.h (fsk_plan_new, fsk_find_frame,
  *    fsk_detect_carrier, fsk_set_tones_by_bandshift, fsk_plan_destroy),
@@ -40,7 +40,7 @@ const char *fsk_b200_last_error(void) { return last_error; }
 #ifdef FSK_EMU	/* tests/emu: the kernels' source on the host SIMT emulator; never the product */
 const char *fsk_b200_version(void) { return "fsk_b200 0.1 HOST-EMULATION (tests only)"; }
 #else
-const char *fsk_b200_version(void) { return "fsk_b200 0.1 sm_100a"; }
+const char *fsk_b200_version(void) { return "fsk_b200 0.1 sm_90a"; }
 #endif
 unsigned long long fsk_b200_launch_count(void) { return fsk_b200_cuda_launch_count(); }
 

@@ -1,5 +1,5 @@
 /*
- * fsk_b200_kernels.cu -- CUDA side of the B200 FSK engine (sm_100a): the kernels and
+ * fsk_b200_kernels.cu -- CUDA side of the FSK engine (sm_90a, H100): the kernels and
  * their host-side launch logic.  The device functions are in fsk_b200_device.cuh.
  *
  * Work decomposition (DESIGN.md has the derivation and the measurements):
@@ -22,14 +22,14 @@
  *   - MODE 2 (shared segments) correlates every sample once per batch of up to three candidates;
  *     MODE 3 (chunk-prefix table, the default for bit periods >= 128 samples) runs one stream per
  *     warp, demodulates the whole search span ONCE per loop iteration into per-chunk prefix sums
- *     (FFMA2, bank-conflict-free odd lane-runs, TMA bulk fill) and analyses every candidate of the
+ *     (paired fp32 sums, bank-conflict-free odd lane-runs, TMA bulk fill) and analyses every candidate of the
  *     coarse and the fine search from that table, two or three candidates side by side.
  *
  * k_rx<G,W,L,MODE,FILL,SRC> the whole rx loop per stream: MODE 0 per candidate (the headline kernel at
  *                         1200 baud), 1 generic (global memory, IEEE, serial order), 2 shared segments,
  *                         3 prefix table (G = 32; W codes the candidate slot); FILL 0 cp.async, 1 TMA bulk
  *                         copies; SRC 0 float32 rows, 1 int16 PCM rows widened inside the fill
- * k_rx_ws<G,W,L>          MODE 0, warp-synchronous (selectable, measured slower)
+ * k_rx_ws<G,W,L>          MODE 0, warp-synchronous (selectable)
  * k_find_frame<G,W,L,MODE> batched fsk_find_frame
  * k_tx, k_band_mags, k_detect_carrier, k_s16_to_f32, k_decode<KIND>   the "next" rows (DESIGN.md 0)
  *
@@ -234,7 +234,7 @@ k_find_frame(const __grid_constant__ fsk_b200_geom geo, const float4 *__restrict
 /* FILL 0: cp.async (LDGSTS) by all lanes of the group; FILL 1: cp.async.bulk (TMA engine)
  * issued by lane 0 with mbarrier completion.
  * EARLY_REQ (FILL 0): ask for the next iteration's samples as soon as the searches of this one
- * are over (measured +3.6 % over asking at the top of the next iteration). */
+ * are over rather than at the top of the next iteration. */
 #ifdef FSK_NO_EARLY_REQ
 #define EARLY_REQ 0
 #else
@@ -593,9 +593,9 @@ k_rx(const __grid_constant__ fsk_b200_geom geo, const __grid_constant__ fsk_b200
 			__syncwarp(gmask);	/* every read of this window precedes the copies */
 			request_at(min((npos + lookahead + need_max + 3u) & ~3u, (npos & ~AL) + R), npos);
 		    }
-		    /* (The bulk fill of MODE 3 asks at the top of the next iteration.  Asking here as well --
-		     * one more barrier phase per iteration, measured -- is 4 % slower: the state machine below
-		     * is too short to hide a copy, and the other warps of the SM do that already.) */
+		    /* (The bulk fill of MODE 3 asks at the top of the next iteration.  Asking here as well
+		     * costs one more barrier phase per iteration, and the state machine below is too short
+		     * to hide a copy; the other warps of the SM do that already.) */
 		}
 	    } else if (SRC)
 		confidence = find_frame<G, GlobalSrc16>(gsrc16, pos, geo, sel, sm.tw, sm.scr, g, gmask,
@@ -726,7 +726,7 @@ k_rx(const __grid_constant__ fsk_b200_geom geo, const __grid_constant__ fsk_b200
 
 
 /* ------------------------------------------------------------------------ */
-/* K2, warp-synchronous form (FSK_B200_FILL=3; measured 4 % slower than the     */
+/* K2, warp-synchronous form (FSK_B200_FILL=3; an alternative to the           */
 /* group-masked loop): the 32/G streams of a warp step through the loop together,*/
 /* which lets every shuffle and vote use the constant full mask                */
 /* ------------------------------------------------------------------------ */
@@ -1254,10 +1254,9 @@ extern "C" void *fsk_b200_cuda_engine_new(void)
     if ((e = getenv("FSK_B200_SPLIT"))) ce->split = atoi(e);
     ce->fill = 0;		/* see the dispatch in fsk_b200_cuda_rx_batch */
     if ((e = getenv("FSK_B200_FILL"))) ce->fill = atoi(e);
-    /* shared-segment search: -1 (default) = where it pays: modes with long bit periods, every coarse
-     * search through the shared segments (measured: Bell103 300 baud +40 %; at 40-sample periods the
-     * per-candidate kernel is faster, profiles/README.md); 0 never; 1 everywhere it fits, with the
-     * single-candidate fast path; 2 everywhere it fits, always */
+    /* shared-segment search: -1 (default) = modes with long bit periods, every coarse search through
+     * the shared segments (at short periods the per-candidate kernel is used); 0 never; 1 everywhere it
+     * fits, with the single-candidate fast path; 2 everywhere it fits, always */
     ce->multi = -1;
     if ((e = getenv("FSK_B200_MULTI"))) ce->multi = atoi(e);
     /* chunk-prefix table search: -1 (default) for bit periods of FSK_PREFIX_MIN_N samples and more, 0 never,
@@ -1269,11 +1268,10 @@ extern "C" void *fsk_b200_cuda_engine_new(void)
 #ifdef FSK_EMU
     ce->pfx_fill = 0;		/* the host emulation of the test harness does not model cp.async.bulk / mbarrier */
 #endif
-    /* 256 MiB of samples ON THE WIRE per slab, two slabs in flight: the float path runs at the PCIe
-     * rate with that (54 GB/s).  The int16 path, measured with slabs of the same stream count (128 MiB
-     * on the wire), reached 78 % of it -- about 0.7 ms per slab stayed exposed (one conversion plus
-     * one rx launch of ~350 streams; which part was not isolated) -- so its slabs now carry the same
-     * number of bytes, i.e. twice the streams. */
+    /* 256 MiB of samples ON THE WIRE per slab, two slabs in flight, so that the copies keep PCIe busy
+     * while the previous slab is demodulated.  int16 slabs carry the same number of bytes, i.e. twice
+     * the streams: with the same stream count, the fixed cost per slab (conversion and launch) is
+     * spread over half the bytes. */
     ce->slab_bytes = (size_t)256 << 20;
     if ((e = getenv("FSK_B200_SLAB_BYTES")) && atoll(e) > 0) ce->slab_bytes = (size_t)atoll(e);
     return ce;
@@ -1340,8 +1338,8 @@ extern "C" int fsk_b200_cuda_tune(void *p, int lanes, int wpb, int ring)
 #define FSK_PFX_MAX_TABLE_BYTES (16u * 1024u)
 #define FSK_PFX_TABLE_EXTRA 2056u	/* rotation-table entries past one period (a lane-run of up to 512 pieces, s4 <= 4) */
 #ifndef FSK_PREFIX_MIN_N
-#define FSK_PREFIX_MIN_N 128u	/* shortest bit period (samples) for which mode 3 is the default: measured faster than the shared
-				 * segments at 160 (Bell103) and 176 (RTTY @8 kHz), slower than the per-candidate kernel at 92 (SAME) and 40 */
+#define FSK_PREFIX_MIN_N 128u	/* shortest bit period (samples) for which mode 3 is the default: Bell103 (160) and RTTY @8 kHz
+				 * (176) take it, SAME (92) and Bell202 (40) stay on the per-candidate kernel */
 #endif
 
 /* exp(-2 pi i k n / fftsize) for k = b_mark, b_space; the argument is reduced
@@ -1546,8 +1544,8 @@ static int pick_shape(const CudaEngine *ce, const fsk_b200_geom *g, unsigned nee
     /* whole blocks; room for the widest window starting anywhere inside a block */
     const unsigned ring_min = (need_floats + 8u + 2u * RING_BLOCK - 1u) / RING_BLOCK * RING_BLOCK;
     (void)max_advance;
-    /* default: the minimum, which already leaves 1..2 blocks of look-ahead (measured: deeper
-     * rings do not pay, fewer resident streams do cost) */
+    /* default: the minimum, which already leaves 1..2 blocks of look-ahead; a deeper ring means
+     * fewer resident streams */
     unsigned ring = ce->ring ? ((unsigned)ce->ring + RING_BLOCK - 1u) / RING_BLOCK * RING_BLOCK : ring_min;
     if (ring < ring_min)
 	ring = ring_min;
@@ -1902,9 +1900,8 @@ static int rx_batch_any(CudaEngine *ce, const fsk_b200_geom *g, const fsk_b200_l
 #undef X
     } else if (sh.mode == 0) {
 	/* FSK_B200_FILL: 0 (default) cp.async fill, group-masked loop; 1 TMA bulk copies
-	 * (UBLKCP + mbarrier); 3 cp.async fill, warp-synchronous loop.  The two alternatives
-	 * pass the same tests and measured slower (profiles/README.md); they are built for the
-	 * shapes of the BASELINE configurations only. */
+	 * (cp.async.bulk + mbarrier); 3 cp.async fill, warp-synchronous loop.  The two alternatives
+	 * pass the same tests; they are built for the shapes of the BASELINE configurations only. */
 	if (ce->fill == 1) {
 #define X(GG, WW, LL) if (sh.G == GG && sh.W == WW && sh.L == LL) { e = launch_rx_t<GG, WW, LL, 0, 1>(sh, ce, lc, a, st); launched = true; }
 	    ALT_COMBOS(X)

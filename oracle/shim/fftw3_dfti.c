@@ -5,7 +5,7 @@
  * Why a second stand-in: the reference's speed on a CPU is the speed of its FFT library.  The
  * portable shim (fftw3_shim.c) is a scalar mixed-radix transform, several times slower than
  * FFTW's SIMD codelets; timing the reference with it would flatter the GPU.  MKL's DFTI is the
- * closest thing to FFTW that exists here (it is NOT FFTW; SURVEY.md 8(c),(d)), so the CPU arms of
+ * closest thing to FFTW that exists here (it is NOT FFTW), so the CPU arms of
  * bench.py time the unmodified src/fsk.c on this one when it loads (oracle/_ref/libfsk_ref_dfti.so)
  * and say so in their `sample` string.  Parity never depends on it: the golden vectors were
  * minted with the portable shim, and tests/test_oracle_vs_ref.py holds the two against each other.

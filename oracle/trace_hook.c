@@ -9,7 +9,7 @@
  * $ORACLE_TRACE_FILE: inputs, outputs, the raw complex FFT bins (b_mark,
  * b_space) of every bit window analysed, and (if $ORACLE_TRACE_SAMPLES=1) the
  * sample window itself.  tests/golden/make_golden.py turns these traces into
- * the committed golden vectors the reference's own tests lack (SURVEY.md 8c).
+ * the committed golden vectors the reference's own tests lack.
  */
 #include <stdio.h>
 #include <stdlib.h>

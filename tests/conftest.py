@@ -15,7 +15,7 @@ EMU_DEVICE = emu_mode.activate() if emu_mode.active() else None
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100)")
     config.addinivalue_line("markers", "ref: needs oracle/_ref (the reference compiled in place)")
 
 

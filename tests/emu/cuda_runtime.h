@@ -4,7 +4,7 @@
  * that the product's kernel SOURCE can be compiled by g++ and run on CPU cores under a small
  * SIMT emulator (tests/emu/Makefile -> tests/emu/libfsk_b200_emu.so).
  *
- * Why: the build container has no GPU.  With this, the parity tests that normally need a B200
+ * Why: the build container has no GPU.  With this, the parity tests that normally need an H100
  * (tests/test_gpu_parity.py) can exercise the kernels' control flow, ring bookkeeping, lane
  * exchanges and record formats on the CPU before GPU minutes are spent.  It is NOT a product
  * path: nothing in minimodem_b200/ loads it, the library it builds is only ever selected by the
@@ -323,7 +323,7 @@ static inline void *__cvta_shared_to_generic(size_t a) { return emu::blk->smem +
 
 /* the inline-PTX wrappers of fsk_b200_device.cuh (guarded there by FSK_EMU) */
 /* FSK_EMU_ULP=n: perturb the two approximate units by up to n ulp (pseudo-randomly, either way), to
- * see that no test hinges on their exact rounding -- the B200's sqrt.approx / div.approx are within
+ * see that no test hinges on their exact rounding -- the GPU's sqrt.approx / div.approx are within
  * 2 ulp of these */
 namespace emu {
 extern int approx_ulp;
@@ -375,8 +375,8 @@ static inline cudaError_t cudaGetDevice(int *d) { *d = 0; return cudaSuccess; }
 static inline cudaError_t cudaDeviceSynchronize(void) { return cudaSuccess; }
 static inline cudaError_t cudaDeviceGetAttribute(int *v, int attr, int)
 {
-    /* the B200 figures the launch-shape logic is written for */
-    *v = attr == cudaDevAttrMultiProcessorCount ? 148 : 232448;
+    /* the H100 figures the launch-shape logic is written for */
+    *v = attr == cudaDevAttrMultiProcessorCount ? 132 : 232448;
     return cudaSuccess;
 }
 template <class T>

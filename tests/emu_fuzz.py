@@ -7,7 +7,7 @@ host SIMT emulator) has to produce them -- exact bits, frame starts and acquire 
 and amplitude to the parity tolerance.  This is a logic check of the kernels over geometry the
 vectors do not reach (window counts from 7 to 44 bits, every lane split the launcher picks,
 fractional samples per bit, long windows); it runs on the emulator only, because a near-tie that
-the B200's approximate divide resolves the other way would make a random case flaky there."""
+the GPU's approximate divide resolves the other way would make a random case flaky there."""
 import numpy as np
 import pytest
 

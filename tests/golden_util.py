@@ -48,7 +48,7 @@ def close(a, b, rel=1e-4, cond=0.0):
     snr*(1-divergence) with snr = sum(sig)/sum(noise) (src/fsk.c:292,336), so a
     perturbation dn of the off-tone magnitudes (relative to the signal) moves it
     by a relative dn*confidence.  Two correct float FFTs already differ by
-    dn ~ 1e-7..1e-6 (SURVEY.md hard part 3), hence rel + cond*|confidence|."""
+    dn ~ 1e-7..1e-6, hence rel + cond*|confidence|."""
     a, b = float(a), float(b)
     if np.isinf(a) or np.isinf(b) or np.isnan(a) or np.isnan(b):
         return (np.isinf(a) and np.isinf(b) and (a > 0) == (b > 0)) or (np.isnan(a) and np.isnan(b))

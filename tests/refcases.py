@@ -137,7 +137,7 @@ def decoder_of(case, rx_mode):
 
 
 # A second batch of option runs: they pin the oracle on the CPU and the emulated kernels
-# (tests/emu_fuzz.py); not on the B200 list (that one is long enough).
+# (tests/emu_fuzz.py); not on the GPU list (that one is long enough).
 MORE = [
     _case("more-v21", _OPT_TEXT, ["V.21"], mode="V.21", audio=True),
     _case("more-6bit-3start", _OPT_TEXT, ["1200", "--startbits", "3", "--stopbits", "1.0"],

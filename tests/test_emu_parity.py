@@ -1,5 +1,5 @@
 """The kernels' SOURCE on the host SIMT emulator (tests/emu): the parity tests that normally need
-a B200 (tests/test_gpu_parity.py, marker `gpu`) run here on CPU cores against the emulation
+an H100 (tests/test_gpu_parity.py, marker `gpu`) run here on CPU cores against the emulation
 build of the very same minimodem_b200/csrc/*.cu / *.cuh files.  It checks what an emulator can
 check -- control flow, ring bookkeeping, lane exchanges, cp.async ordering (copies land as late
 as the code's own waits allow, or at once), record and state formats, every decoder -- before

@@ -1,4 +1,4 @@
-"""Parity tests proper (B200): the CUDA path, called through the C ABI, against
+"""Parity tests proper (H100): the CUDA path, called through the C ABI, against
 the oracle on the same inputs -- the reference's own test vectors (golden
 fixtures minted from the unmodified reference CLI), seeded noisy inputs, and
 size-independent properties at larger batch sizes.
@@ -1029,7 +1029,7 @@ def test_live_receiver_prints_the_reference_output_however_the_stream_is_cut(nam
 
 
 # --------------------------------------------------------------------------
-# per-bit parity gate (BASELINE.md 3, SURVEY.md 7 hard part 3): what fsk_bit_analyze saw in every
+# per-bit parity gate (BASELINE.md 3): what fsk_bit_analyze saw in every
 # bit window of the winning candidate -- signal and noise magnitudes of src/fsk.c:158-169 --
 # against the oracle's: rel 1e-4 on the signal, abs 1e-4 * (mean signal) on the noise, and the
 # noise <= FLT_EPSILON class of :278-280 (what makes `confidence=inf`) exactly

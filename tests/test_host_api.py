@@ -32,7 +32,7 @@ def test_library_exports_every_declared_symbol():
     for name in sorted(declared):
         assert hasattr(L, name), name
     assert declared == set(mm.EXPORTS)
-    assert "sm_100a" in mm.version()
+    assert "sm_90a" in mm.version()
 
 
 MODES = [("1200", {}), ("300", {}), ("rtty", {}), ("tdd", {}), ("same", {}), ("callerid", {}),
@@ -94,7 +94,7 @@ def test_presets_and_geometry_match_oracle(mode, kw):
 
 
 def test_survey_table_values():
-    """SURVEY.md 8(d): the derived integers of the BASELINE configs."""
+    """The derived integers of the BASELINE configs."""
     want = {
         ("1200", 48000): dict(fftsize=240, b=(6, 11), expect=440, frame=400, over=20, tmn=60, tmc=50, N=40, span=440),
         ("rtty", 8000): dict(fftsize=800, b=(159, 142), expect=1408, frame=1232, over=88, tmn=264, tmc=220, N=176, span=1408),

@@ -62,7 +62,7 @@ def test_rx_restatement_decodes_and_reports_like_reference(case):
         got = [orc.report_line(rx, rp) for rp in r["reports"]]
         if case["rx_one"]:
             got = got[:1]
-        # ill-conditioned confidences (noise ~ 0, SURVEY hard part 3) may differ in the
+        # ill-conditioned confidences (noise ~ 0) may differ in the
         # printed decimals; everything else must be identical text
         assert len(got) == len(want)
         for a_line, b_line in zip(got, want):
