@@ -390,7 +390,8 @@ unsigned long long fsk_b200_frame_databits(const fsk_b200_rx_params *p, const fs
  * samples through a sine table of table_len entries computed by the caller on
  * the host).  Stream s carries words[s*nwords .. +nwords) after lead_in[s]
  * samples of silence; writes exactly nsamples_out floats per stream (zero
- * padded / truncated).  All pointers are device memory. */
+ * padded / truncated).  All pointers are device memory.  -EINVAL for
+ * n_data_bits outside 1..32 or nsamples_out > stride. */
 typedef struct fsk_b200_tx_config {
     float	sample_rate, data_rate, f_mark, f_space;
     unsigned int n_data_bits;
@@ -407,6 +408,75 @@ void fsk_b200_sin_table(float *out, unsigned int len, float mag);
 int fsk_b200_tx_batch(const fsk_b200_tx_config *cfg, const float *sin_table, uint32_t table_len,
 	const uint32_t *words, uint32_t nwords, const uint32_t *lead_in,
 	float *samples_out, size_t nstreams, size_t stride, uint32_t nsamples_out, void *stream);
+
+/* ---- the batched transmitter: text in, the reference's `--tx` audio out ----------------------
+ *
+ *   fsk_b200_tx_config_from_rx(&rx_cfg, &tx_cfg);                 // or fill tx_cfg by hand
+ *   te = fsk_b200_tx_engine_new(&tx_cfg, &signal, fsk_b200_encoder_for_mode(mode, n_data_bits));
+ *   for every tick:
+ *       fsk_b200_tx_text_batch(te, d_text, n, text_stride, d_len, FSK_B200_TX_IDLE_IF_EMPTY,
+ *                              d_states, d_audio, out_stride, d_out_len, st);
+ *   at the end: one more call with FSK_B200_TX_FINAL (and zero lengths) for the trailers
+ *
+ * Per stream a call does what the reference's fsk_transmit_stdin (src/minimodem.c:114-250) does
+ * for those bytes, with every piece of state the reference keeps in static variables held in
+ * the stream's fsk_b200_tx_state, so that a text cut into any pieces gives the same audio. */
+
+/* The encoders of src/databits.h:48-65 */
+#define FSK_B200_ENCODE_ASCII8	0	/* databits_encode_ascii8, src/databits_ascii.c:28-33 */
+#define FSK_B200_ENCODE_BAUDOT	1	/* baudot_encode, src/baudot.c:258-310 */
+
+/* --volume, --lut and --float-samples (src/minimodem.c:537-538, :686-693, :749) */
+typedef struct fsk_b200_tx_signal {
+    float	amplitude;		/* tone_mag; 1.0 = full scale */
+    uint32_t	sin_table_len;		/* 0: sin() per sample (see DESIGN.md 5 on its rounding) */
+    int		float_samples;		/* 0: int16 PCM, 1: float32 */
+} fsk_b200_tx_signal;
+
+/* 16 bytes per stream, device memory; all zeros = a fresh reference process */
+typedef struct fsk_b200_tx_state {
+    float	cphase;			/* sa_tone_cphase, src/simple-tone-generator.c:98 */
+    uint32_t	baudot_charset;		/* src/baudot.c:197: 0 unknown, 1 LTRS, 2 FIGS */
+    uint32_t	transmitting;		/* tx_transmitting, src/minimodem.c:164-232: 0 idle, 1 carrier, 2 sending */
+    uint32_t	reserved;
+} fsk_b200_tx_state;
+
+#define FSK_B200_TX_IDLE_IF_EMPTY 1u	/* a stream with no bytes sends one idle tone (the reference's
+					 * select() timeout, :230-237) and drops to transmitting = 1 */
+#define FSK_B200_TX_FINAL	  2u	/* end of input: transmitting streams send the trailer (:60-74, :246) */
+
+typedef struct fsk_b200_tx_engine fsk_b200_tx_engine;
+
+/* Which encoder the reference's main() would pick (src/minimodem.c:553, :676, :821, :829): Baudot
+ * for "rtty", "tdd" and n_data_bits == 5 (the -5 option), ascii8 otherwise. */
+int fsk_b200_encoder_for_mode(const char *baudmode, unsigned int n_data_bits);
+
+/* The TX fields main() derives for a receive configuration: leader 2 bits (0 without start
+ * bits, :949-951), trailer 2 bits, 16 sync bytes for "same" and --sync-byte (:716-720, :844-845). */
+int fsk_b200_tx_config_from_rx(const fsk_b200_rx_config *rx, fsk_b200_tx_config *out);
+
+/* Creates a transmitter on the current CUDA device; it owns the device sine tables, built on the
+ * host exactly as simpleaudio_tone_init builds them (src/simple-tone-generator.c:38-72).  NULL +
+ * errno: EINVAL for n_data_bits outside 1..32 (the reference's `bits >> i` is undefined beyond),
+ * a bit of 0 samples or an unknown encoder; ENODEV without a usable CUDA device. */
+fsk_b200_tx_engine *fsk_b200_tx_engine_new(const fsk_b200_tx_config *cfg, const fsk_b200_tx_signal *sig,
+	int encoder);
+void fsk_b200_tx_engine_destroy(fsk_b200_tx_engine *te);
+
+/* Most samples a row of `nbytes` text bytes can become under `flags` (leader, preamble, Baudot's
+ * at most 2 words per byte, the idle tone, the trailer); exact for ascii8 text of nbytes bytes
+ * from a fresh state.  0 when it exceeds 2^32 - 1. */
+uint64_t fsk_b200_tx_max_samples(const fsk_b200_tx_engine *te, uint32_t nbytes, unsigned int flags);
+
+/* One tick of every stream.  text: uint8 [nstreams][text_stride], text_len[s] bytes of row s
+ * (clamped to text_stride); states: one fsk_b200_tx_state per stream, read and written back;
+ * out: int16 or float32 (as the signal says) rows [nstreams][out_stride], out_len[s] = samples
+ * written to row s (the rest of the row is not touched).  All pointers are device memory;
+ * asynchronous on `stream`.  -EINVAL (and no launch) for a NULL pointer or an out_stride below
+ * fsk_b200_tx_max_samples(te, text_stride, flags). */
+int fsk_b200_tx_text_batch(fsk_b200_tx_engine *te, const uint8_t *text, size_t nstreams, size_t text_stride,
+	const uint32_t *text_len, unsigned int flags, fsk_b200_tx_state *states, void *out, size_t out_stride,
+	uint32_t *out_len, void *stream);
 
 /* Diagnostics: which rx kernel the engine's latest fsk_b200_rx_batch launched ("k_rx<G=8,W=3,L=2,mode=2
  * (shared-segment),fill=0> threads=64 ring=640 smem=23232 blocks=8192"; "" before the first launch). */

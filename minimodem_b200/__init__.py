@@ -14,5 +14,7 @@ from .api import (  # noqa: F401
     FRAME_DTYPE, STATE_DTYPE, STATE_WORDS, FRAME_ACQUIRED, FRAME_REPORT, EXPORTS,
     DECODE_ASCII, DECODE_BINARY, DECODE_BAUDOT, DECODE_CALLERID, DECODE_UIC_GROUND, DECODE_UIC_TRAIN,
     DECODER_STATE_BYTES, DecoderState, decoder_for_mode, decode_max_bytes_per_frame, decode_max_bytes, detect_carrier_batch, stream_push, wav_locate,
+    TxEngine, TxSignal, TxState, TX_STATE_BYTES, TX_IDLE_IF_EMPTY, TX_FINAL, ENCODE_ASCII8, ENCODE_BAUDOT,
+    encoder_for_mode, tx_max_samples,
 )
-from .serving import LiveReceiver  # noqa: F401,E402
+from .serving import LiveReceiver, LiveTransmitter  # noqa: F401,E402

@@ -84,6 +84,22 @@ class TxConfig(C.Structure):
                 ("leader_bits", C.c_int), ("trailer_bits", C.c_int)]
 
 
+class TxSignal(C.Structure):
+    """fsk_b200_tx_signal: --volume, --lut, --float-samples."""
+    _fields_ = [("amplitude", C.c_float), ("sin_table_len", C.c_uint32), ("float_samples", C.c_int)]
+
+
+class TxState(C.Structure):
+    """fsk_b200_tx_state, 16 bytes per stream; all zeros = a fresh reference process."""
+    _fields_ = [("cphase", C.c_float), ("baudot_charset", C.c_uint32), ("transmitting", C.c_uint32),
+                ("reserved", C.c_uint32)]
+
+
+TX_STATE_BYTES = 16
+TX_IDLE_IF_EMPTY, TX_FINAL = 1, 2
+ENCODE_ASCII8, ENCODE_BAUDOT = 0, 1
+
+
 class FskPlanStruct(C.Structure):
     """struct fsk_plan, include/fsk_b200.h (layout of src/fsk.h:30-46)."""
     _fields_ = [("sample_rate", C.c_float), ("f_mark", C.c_float), ("f_space", C.c_float),
@@ -104,6 +120,8 @@ EXPORTS = [
     "fsk_b200_decode_max_bytes", "fsk_b200_detect_carrier_batch",
     "fsk_b200_stream_window", "fsk_b200_engine_set_holdback", "fsk_b200_stream_push", "fsk_b200_wav_locate",
     "fsk_b200_version", "fsk_b200_launch_count", "fsk_b200_last_error", "fsk_b200_engine_last_kernel",
+    "fsk_b200_encoder_for_mode", "fsk_b200_tx_config_from_rx", "fsk_b200_tx_engine_new", "fsk_b200_tx_engine_destroy",
+    "fsk_b200_tx_max_samples", "fsk_b200_tx_text_batch",
 ]
 
 _lib = None
@@ -214,6 +232,19 @@ def lib():
     L.fsk_b200_wav_locate.argtypes = [C.c_char_p, C.c_size_t, C.POINTER(C.c_size_t), C.POINTER(C.c_size_t),
                                       C.POINTER(C.c_uint32), C.POINTER(C.c_int)]
     L.fsk_b200_wav_locate.restype = C.c_int
+    L.fsk_b200_encoder_for_mode.argtypes = [C.c_char_p, C.c_uint]
+    L.fsk_b200_encoder_for_mode.restype = C.c_int
+    L.fsk_b200_tx_config_from_rx.argtypes = [C.POINTER(RxConfig), C.POINTER(TxConfig)]
+    L.fsk_b200_tx_config_from_rx.restype = C.c_int
+    L.fsk_b200_tx_engine_new.argtypes = [C.POINTER(TxConfig), C.POINTER(TxSignal), C.c_int]
+    L.fsk_b200_tx_engine_new.restype = C.c_void_p
+    L.fsk_b200_tx_engine_destroy.argtypes = [C.c_void_p]
+    L.fsk_b200_tx_engine_destroy.restype = None
+    L.fsk_b200_tx_max_samples.argtypes = [C.c_void_p, C.c_uint32, C.c_uint]
+    L.fsk_b200_tx_max_samples.restype = C.c_uint64
+    L.fsk_b200_tx_text_batch.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t, C.c_void_p, C.c_uint,
+                                         C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p]
+    L.fsk_b200_tx_text_batch.restype = C.c_int
     L.fsk_b200_sin_table.argtypes = [C.POINTER(C.c_float), C.c_uint, C.c_float]
     L.fsk_b200_sin_table.restype = None
     L.fsk_b200_version.restype = C.c_char_p
@@ -645,15 +676,90 @@ def s16_to_f32(src, out=None, stream=None):
 
 
 def tx_config_from(cfg, leader_bits=None, trailer_bits=2, do_tx_sync_bytes=None):
-    """TxConfig matching an RxConfig (src/minimodem.c:995-1007 passes the same fields)."""
+    """TxConfig matching an RxConfig (fsk_b200_tx_config_from_rx: what src/minimodem.c:716-720, :844-845,
+    :949-951 derive); the keywords override its fields."""
     t = TxConfig()
-    t.sample_rate, t.data_rate = cfg.sample_rate, cfg.data_rate
-    t.f_mark, t.f_space = cfg.f_mark, cfg.f_space
-    t.n_data_bits = cfg.n_data_bits
-    t.nstartbits, t.nstopbits = float(cfg.nstartbits), cfg.nstopbits
-    t.invert_start_stop, t.msb_first = cfg.invert_start_stop, cfg.msb_first
-    t.do_tx_sync_bytes = (16 if cfg.do_rx_sync else 0) if do_tx_sync_bytes is None else do_tx_sync_bytes
-    t.sync_byte = cfg.sync_byte & 0xFFFFFFFF if cfg.do_rx_sync else 0
-    t.leader_bits = (0 if cfg.nstartbits == 0 else 2) if leader_bits is None else leader_bits   # :950-951
+    if lib().fsk_b200_tx_config_from_rx(C.byref(cfg), C.byref(t)) != 0:
+        _err("fsk_b200_tx_config_from_rx")
+    if do_tx_sync_bytes is not None:
+        t.do_tx_sync_bytes = do_tx_sync_bytes
+    if leader_bits is not None:
+        t.leader_bits = leader_bits
     t.trailer_bits = trailer_bits
     return t
+
+
+def encoder_for_mode(baudmode, n_data_bits=8):
+    """Which databits encoder the reference's main() would use (ENCODE_ASCII8 / ENCODE_BAUDOT)."""
+    k = lib().fsk_b200_encoder_for_mode(str(baudmode).encode(), int(n_data_bits))
+    if k < 0:
+        _err("fsk_b200_encoder_for_mode", k)
+    return k
+
+
+class TxEngine:
+    """The batched transmitter (fsk_b200_tx_engine): text rows in, the reference's `--tx` samples out,
+    all on the device.  cfg: TxConfig; the signal options are --volume, --lut and --float-samples."""
+
+    def __init__(self, cfg, encoder=ENCODE_ASCII8, amplitude=1.0, lut=4096, float_samples=False):
+        self.cfg = cfg
+        self.encoder = int(encoder)
+        self.float_samples = bool(float_samples)
+        sig = TxSignal(float(amplitude), int(lut), int(self.float_samples))
+        self._te = lib().fsk_b200_tx_engine_new(C.byref(cfg), C.byref(sig), self.encoder)
+        if not self._te:
+            _err("fsk_b200_tx_engine_new")
+
+    @classmethod
+    def for_mode(cls, baudmode, sample_rate=48000, amplitude=1.0, lut=4096, float_samples=False, **overrides):
+        rx = rx_config_for_mode(baudmode, sample_rate, **overrides)
+        return cls(tx_config_from(rx), encoder_for_mode(baudmode, rx.n_data_bits), amplitude, lut, float_samples)
+
+    def max_samples(self, nbytes, flags=0):
+        """fsk_b200_tx_max_samples: the out_stride a row of nbytes text bytes never exceeds."""
+        return int(lib().fsk_b200_tx_max_samples(self._te, int(nbytes), int(flags)))
+
+    def new_states(self, nstreams, device=None):
+        """Fresh per-stream states: uint8 CUDA tensor [nstreams, TX_STATE_BYTES] of zeros."""
+        torch = _torch()
+        return torch.zeros((int(nstreams), TX_STATE_BYTES), dtype=torch.uint8,
+                           device=device if device is not None else torch.device("cuda:0"))
+
+    def text_batch(self, text, lengths, states, flags=0, out=None, out_len=None, stream=None):
+        """fsk_b200_tx_text_batch.  text: uint8 CUDA tensor [nstreams, text_stride]; lengths: int32
+        [nstreams]; states: uint8 [nstreams, TX_STATE_BYTES] (updated in place).  Returns (samples
+        [nstreams, out_stride] int16 or float32, counts [nstreams] int32)."""
+        torch = _torch()
+        assert text.dtype == torch.uint8 and text.is_contiguous() and text.dim() == 2
+        nstreams, text_stride = text.shape
+        assert lengths.dtype == torch.int32 and lengths.is_contiguous() and lengths.numel() == nstreams
+        assert states.dtype == torch.uint8 and states.is_contiguous() and tuple(states.shape) == (nstreams, TX_STATE_BYTES)
+        if out is None:
+            stride = (self.max_samples(text_stride, flags) + 7) & ~7
+            out = torch.empty((nstreams, stride), dtype=torch.float32 if self.float_samples else torch.int16,
+                              device=text.device)
+        assert out.is_contiguous() and out.dtype == (torch.float32 if self.float_samples else torch.int16)
+        if out_len is None:
+            out_len = torch.empty((nstreams,), dtype=torch.int32, device=text.device)
+        rc = lib().fsk_b200_tx_text_batch(self._te, _ptr(text), nstreams, text_stride, _ptr(lengths), int(flags),
+                                          _ptr(states), _ptr(out), out.shape[1], _ptr(out_len),
+                                          _stream_handle(stream))
+        if rc:
+            _err("fsk_b200_tx_text_batch", rc)
+        return out, out_len
+
+    def destroy(self):
+        if self._te:
+            lib().fsk_b200_tx_engine_destroy(self._te)
+            self._te = None
+
+    def __del__(self):
+        try:
+            self.destroy()
+        except Exception:
+            pass
+
+
+def tx_max_samples(engine, nbytes, flags=0):
+    """fsk_b200_tx_max_samples of a TxEngine."""
+    return engine.max_samples(nbytes, flags)

@@ -17,6 +17,12 @@
  *           :185-186), that the 256-byte message buffer is never cleared, and that a bad
  *           MDMF field discards the fields printed before it (:62-71)
  *   uic     src/databits_uic.c:29-74, src/uic_codes.c:23-68   one text line per 39-bit word
+ *
+ * and the transmitter's two encoders (bytes -> data words), compiled into the tx kernel and, for the
+ * tests, by gcc into oracle/tx_oracle.c:
+ *   ascii8  src/databits_ascii.c:28-33        the byte, sign-extended as a char
+ *   baudot  src/baudot.c:258-310              ITA2 from the decoder's columns, shift codes,
+ *           unshift-on-space, non-encodable characters skipped
  */
 #ifndef FSK_B200_DECODE_CORE_H
 #define FSK_B200_DECODE_CORE_H
@@ -366,6 +372,94 @@ FSK_HD void fsk_dec_record(int kind, unsigned int shift, unsigned int n_data_bit
     if (do_rx_sync && bits == sync_byte)		/* :1436-1439 */
 	return;
     fsk_dec_word(kind, n_data_bits, st, bits, k);
+}
+
+/* ------------------------------------------------------------------------ */
+/* the databits encoders of the transmitter (src/databits.h:48-65)          */
+/* ------------------------------------------------------------------------ */
+
+/* databits_encode_ascii8, src/databits_ascii.c:28-33: the byte as a (signed) char, so that
+ * bytes >= 0x80 are sign-extended into the word */
+FSK_HD uint32_t fsk_enc_ascii8(unsigned int byte)
+{
+    return (uint32_t)(int32_t)(int8_t)(uint8_t)byte;
+}
+
+/* toupper() of the C locale on a char value (-128..127) */
+FSK_HD int fsk_enc_toupper(int c)
+{
+    return c >= 'a' && c <= 'z' ? c - ('a' - 'A') : c;
+}
+
+/* Which charsets hold ASCII character c (0 <= c < 0x60) and under which code, read off the
+ * decoder's columns (fsk_dec_baudot_char): (mask << 8) | code, mask bit 0 = LTRS, bit 1 = U.S.
+ * FIGS, 0 = not encodable.  Code 0 is NUL in both columns (the decoder prints '_' / '^' for it),
+ * the two shift codes carry no character.  One deviation from the plain inversion is the
+ * reference's own: its encoder sends '+' as 0x12 in FIGS (')' in the U.S. column; '+' is the
+ * CCITT No. 2 figure of 0x11), src/baudot.c baudot_encode_table. */
+FSK_HD unsigned int fsk_enc_baudot_entry(int c)
+{
+    if (c == '+')
+	return (2u << 8) | 0x12u;
+    unsigned int mask = 0, code = 0;
+    for (unsigned int k = 0; k < 32u; k++) {
+	if (k == 0x1bu || k == 0x1fu)
+	    continue;
+	const int l = k ? (int)fsk_dec_baudot_char(k, 0) : 0;
+	const int f = k ? (int)fsk_dec_baudot_char(k, 1) : 0;
+	if (c == l) {
+	    mask |= 1u;
+	    code = k;
+	}
+	if (c == f) {
+	    mask |= 2u;
+	    code = k;
+	}
+    }
+    return (mask << 8) | code;
+}
+
+/* baudot_encode, src/baudot.c:258-310 (baudot_usos = 1), with the file-static baudot_charset
+ * held in *charset (0 unknown, 1 LTRS, 2 FIGS).  c: toupper() of the char value, entry:
+ * fsk_enc_baudot_entry(c) when 0 <= c < 0x60 (anything, otherwise).  Returns the number of
+ * words stored (0, 1 or 2): a shift code first when the character is not in the current
+ * charset, then the character's code. */
+FSK_HD unsigned int fsk_enc_baudot_with(uint32_t *charset, int c, unsigned int entry, uint32_t *words)
+{
+    if (c >= 0x60 || c < 0)				/* :263-267 */
+	return 0;
+    const unsigned int mask = entry >> 8;
+    unsigned int shift = 0;
+    if ((*charset & mask) == 0) {			/* :277-294 */
+	if (mask == 0)
+	    return 0;
+	if (*charset == 0)
+	    *charset = 1;
+	if (mask != 3u)
+	    *charset = mask;
+	shift = *charset == 1u ? 0x1Fu : 0x1Bu;
+    }
+    if (c == ' ')					/* :305-306 */
+	*charset = 1;
+    if (!shift) {
+	words[0] = entry & 0x1fu;			/* :302 */
+	return 1;
+    }
+    words[0] = shift;
+    words[1] = entry & 0x1fu;
+    return 2;
+}
+
+/* the whole encoder call for one input byte: encoder kind FSK_B200_ENCODE_*; returns the words
+ * stored (at most 2) */
+FSK_HD unsigned int fsk_enc_byte(int kind, uint32_t *charset, unsigned int byte, uint32_t *words)
+{
+    if (kind != FSK_B200_ENCODE_BAUDOT) {
+	words[0] = fsk_enc_ascii8(byte);
+	return 1;
+    }
+    const int c = fsk_enc_toupper((int)(int8_t)(uint8_t)byte);
+    return fsk_enc_baudot_with(charset, c, c >= 0 && c < 0x60 ? fsk_enc_baudot_entry(c) : 0u, words);
 }
 
 #endif

@@ -909,6 +909,54 @@ void fsk_b200_sin_table(float *out, unsigned int len, float mag)
 	out[i] = mag * sinf((float)M_PI * 2 * i / len);
 }
 
+/* ------------------------------------------------------------------------ */
+/* transmitter                                                              */
+/* ------------------------------------------------------------------------ */
+
+/* the integers fsk_transmit_stdin derives (src/minimodem.c:131-132, :96-97, :110-111, :155, :236) */
+static int tx_plan_from(const fsk_b200_tx_config *c, int encoder, fsk_b200_tx_plan *p)
+{
+    memset(p, 0, sizeof(*p));
+    if (c->n_data_bits < 1 || c->n_data_bits > 32) {
+	fsk_b200_set_error("tx: n_data_bits must be 1..32 (got %u)", c->n_data_bits);
+	return -EINVAL;
+    }
+    if (encoder != FSK_B200_ENCODE_ASCII8 && encoder != FSK_B200_ENCODE_BAUDOT && encoder != FSK_B200_ENCODE_WORDS) {
+	fsk_b200_set_error("tx: unknown encoder %d", encoder);
+	return -EINVAL;
+    }
+    if (!(c->sample_rate >= 1.0f && c->sample_rate < 16777216.0f) || !(c->data_rate > 0.0f)
+	    || !(c->f_mark > 0.0f) || !(c->f_space > 0.0f) || c->leader_bits < 0 || c->trailer_bits < 0) {
+	fsk_b200_set_error("tx: bad sample rate, data rate, tone or leader/trailer length");
+	return -EINVAL;
+    }
+    const size_t sample_rate = (size_t)c->sample_rate;
+    const size_t bit = sample_rate / c->data_rate + 0.5f;
+    if (bit == 0 || bit > 0xffffffffu) {
+	fsk_b200_set_error("tx: a bit of %zu samples", bit);
+	return -EINVAL;
+    }
+    p->rate = (uint32_t)sample_rate;
+    p->f_mark = c->f_mark;
+    p->f_space = c->f_space;
+    p->bit = (uint32_t)bit;
+    p->has_start = c->nstartbits > 0;
+    p->has_stop = c->nstopbits > 0;
+    p->start = p->has_start ? (uint32_t)(size_t)(bit * c->nstartbits) : 0;
+    p->stop = p->has_stop ? (uint32_t)(size_t)(bit * c->nstopbits) : 0;
+    p->idle = (uint32_t)((1000000u / 25) * sample_rate / 1000000);
+    p->n_data_bits = c->n_data_bits;
+    p->tones_per_frame = (uint32_t)p->has_start + c->n_data_bits + (uint32_t)p->has_stop;
+    p->invert_start_stop = c->invert_start_stop;
+    p->msb_first = c->msb_first;
+    p->nsync = c->do_tx_sync_bytes;
+    p->sync_byte = c->sync_byte;
+    p->leader = (uint32_t)c->leader_bits;
+    p->trailer = (uint32_t)c->trailer_bits;
+    p->encoder = encoder;
+    return 0;
+}
+
 int fsk_b200_tx_batch(const fsk_b200_tx_config *cfg, const float *sin_table, uint32_t table_len,
 	const uint32_t *words, uint32_t nwords, const uint32_t *lead_in, float *samples_out,
 	size_t nstreams, size_t stride, uint32_t nsamples_out, void *stream)
@@ -917,8 +965,183 @@ int fsk_b200_tx_batch(const fsk_b200_tx_config *cfg, const float *sin_table, uin
 	fsk_b200_set_error("tx_batch: NULL argument");
 	return -EINVAL;
     }
-    return fsk_b200_cuda_tx_batch(cfg, sin_table, table_len, words, nwords, lead_in, samples_out,
-	    nstreams, stride, nsamples_out, stream);
+    if (nsamples_out > stride) {
+	fsk_b200_set_error("tx_batch: nsamples_out %u exceeds the stride %zu", nsamples_out, stride);
+	return -EINVAL;
+    }
+    fsk_b200_tx_plan p;
+    int rc = tx_plan_from(cfg, FSK_B200_ENCODE_WORDS, &p);
+    if (rc)
+	return rc;
+    p.lut_len = table_len;
+    p.float_samples = 1;
+    if (nsamples_out == 0)
+	return 0;
+    fsk_b200_tx_io io;
+    memset(&io, 0, sizeof(io));
+    io.words = words;
+    io.nwords = nwords;
+    io.lead_in = lead_in;
+    io.out = samples_out;
+    io.out_stride = stride;
+    io.cap = nsamples_out;
+    io.nstreams = nstreams;
+    return fsk_b200_cuda_tx_synth(&p, sin_table, &io, stream);
+}
+
+struct fsk_b200_tx_engine {
+    fsk_b200_tx_plan plan;
+    void *d_lut;		/* the sine table of the output format, device memory */
+};
+
+int fsk_b200_encoder_for_mode(const char *baudmode, unsigned int n_data_bits)
+{
+    if (!baudmode)
+	return -EINVAL;
+    if (n_data_bits == 5 || strncasecmp(baudmode, "rtty", 5) == 0 || strncasecmp(baudmode, "tdd", 4) == 0)
+	return FSK_B200_ENCODE_BAUDOT;				/* :676, :821, :829 */
+    return FSK_B200_ENCODE_ASCII8;				/* :553 */
+}
+
+int fsk_b200_tx_config_from_rx(const fsk_b200_rx_config *rx, fsk_b200_tx_config *out)
+{
+    if (!rx || !out)
+	return -EINVAL;
+    memset(out, 0, sizeof(*out));
+    out->sample_rate = rx->sample_rate;
+    out->data_rate = rx->data_rate;
+    out->f_mark = rx->f_mark;
+    out->f_space = rx->f_space;
+    out->n_data_bits = rx->n_data_bits;
+    out->nstartbits = (float)rx->nstartbits;
+    out->nstopbits = rx->nstopbits;
+    out->invert_start_stop = rx->invert_start_stop;
+    out->msb_first = rx->msb_first;
+    out->do_tx_sync_bytes = rx->do_rx_sync ? 16u : 0u;			/* :716-720, :844-845 */
+    out->sync_byte = rx->do_rx_sync ? (unsigned int)rx->sync_byte : 0u;
+    out->leader_bits = rx->nstartbits == 0 ? 0 : 2;			/* :51, :949-951 */
+    out->trailer_bits = 2;						/* :52 */
+    return 0;
+}
+
+fsk_b200_tx_engine *fsk_b200_tx_engine_new(const fsk_b200_tx_config *cfg, const fsk_b200_tx_signal *sig,
+	int encoder)
+{
+    if (!cfg || !sig || !(sig->amplitude > 0.0f) || (encoder != FSK_B200_ENCODE_ASCII8
+		&& encoder != FSK_B200_ENCODE_BAUDOT)) {
+	fsk_b200_set_error("tx_engine_new: bad argument");
+	errno = EINVAL;
+	return NULL;
+    }
+    fsk_b200_tx_engine *te = calloc(1, sizeof(*te));
+    if (!te) {
+	errno = ENOMEM;
+	return NULL;
+    }
+    if (tx_plan_from(cfg, encoder, &te->plan)) {
+	free(te);
+	errno = EINVAL;
+	return NULL;
+    }
+    if (!fsk_b200_cuda_device_ok()) {
+	fsk_b200_set_error("tx_engine_new: no usable CUDA device");
+	free(te);
+	errno = ENODEV;
+	return NULL;
+    }
+    /* simpleaudio_tone_init, src/simple-tone-generator.c:38-72, and the mag_s of :145-150 */
+    const float mag = sig->amplitude;
+    unsigned short mag_s = 32767.0f * mag + 0.5f;
+    if (mag > 1.0f)
+	mag_s = 32767;
+    if (mag_s < 1)
+	mag_s = 1;
+    te->plan.lut_len = sig->sin_table_len;
+    te->plan.mag = mag;
+    te->plan.mag_s = (float)mag_s;
+    te->plan.float_samples = sig->float_samples != 0;
+    const unsigned len = sig->sin_table_len;
+    if (len) {
+	const size_t bytes = (size_t)len * (te->plan.float_samples ? sizeof(float) : sizeof(short));
+	void *t = malloc(bytes);
+	if (!t) {
+	    free(te);
+	    errno = ENOMEM;
+	    return NULL;
+	}
+	if (te->plan.float_samples)
+	    fsk_b200_sin_table((float *)t, len, mag);
+	else
+	    for (unsigned i = 0; i < len; i++)
+		((short *)t)[i] = lroundf(mag_s * sinf((float)M_PI * 2 * i / len));
+	te->d_lut = fsk_b200_cuda_upload(t, bytes);
+	free(t);
+	if (!te->d_lut) {
+	    free(te);
+	    errno = ENODEV;
+	    return NULL;
+	}
+    }
+    return te;
+}
+
+void fsk_b200_tx_engine_destroy(fsk_b200_tx_engine *te)
+{
+    if (!te)
+	return;
+    if (te->d_lut)
+	fsk_b200_cuda_free(te->d_lut);
+    free(te);
+}
+
+uint64_t fsk_b200_tx_max_samples(const fsk_b200_tx_engine *te, uint32_t nbytes, unsigned int flags)
+{
+    if (!te)
+	return 0;
+    const fsk_b200_tx_plan *p = &te->plan;
+    const uint64_t frame = (uint64_t)p->start + (uint64_t)p->n_data_bits * p->bit + p->stop;
+    const uint64_t words = (uint64_t)nbytes * (p->encoder == FSK_B200_ENCODE_BAUDOT ? 2u : 1u);
+    uint64_t n = 0;
+    if (nbytes)					/* leader, preamble and the frames (:202-228) */
+	n = (uint64_t)p->leader * p->bit + (p->nsync + words) * frame;
+    if ((flags & FSK_B200_TX_IDLE_IF_EMPTY) && n < p->idle)	/* or the idle tone of an empty row */
+	n = p->idle;
+    if (flags & FSK_B200_TX_FINAL)
+	n += (uint64_t)p->trailer * p->bit;
+    return n > 0xffffffffu ? 0 : n;
+}
+
+int fsk_b200_tx_text_batch(fsk_b200_tx_engine *te, const uint8_t *text, size_t nstreams, size_t text_stride,
+	const uint32_t *text_len, unsigned int flags, fsk_b200_tx_state *states, void *out, size_t out_stride,
+	uint32_t *out_len, void *stream)
+{
+    if (!te || !text || !text_len || !states || !out || !out_len) {
+	fsk_b200_set_error("tx_text_batch: NULL argument");
+	return -EINVAL;
+    }
+    if (flags & ~(FSK_B200_TX_IDLE_IF_EMPTY | FSK_B200_TX_FINAL)) {
+	fsk_b200_set_error("tx_text_batch: unknown flags 0x%x", flags);
+	return -EINVAL;
+    }
+    const uint64_t need = fsk_b200_tx_max_samples(te, text_stride > 0xffffffffu ? 0xffffffffu : (uint32_t)text_stride,
+	    flags);
+    if (text_stride > 0xffffffffu || (need == 0 && text_stride > 0) || out_stride < need) {
+	fsk_b200_set_error("tx_text_batch: out_stride %zu is below the %llu samples a row of %zu bytes can need",
+		out_stride, (unsigned long long)need, text_stride);
+	return -EINVAL;
+    }
+    fsk_b200_tx_io io;
+    memset(&io, 0, sizeof(io));
+    io.text = text;
+    io.text_stride = text_stride;
+    io.text_len = text_len;
+    io.states = states;
+    io.out = out;
+    io.out_stride = out_stride;
+    io.out_len = out_len;
+    io.flags = flags;
+    io.nstreams = nstreams;
+    return fsk_b200_cuda_tx_synth(&te->plan, te->d_lut, &io, stream);
 }
 
 /* ------------------------------------------------------------------------ */

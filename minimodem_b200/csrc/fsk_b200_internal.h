@@ -108,6 +108,44 @@ typedef struct fsk_b200_pfx {
     uint32_t	zero;		/* 0 (an operand the compiler cannot see through) */
 } fsk_b200_pfx;
 
+/* ---- transmitter ------------------------------------------------------------------------------
+ * Everything the synthesis kernel needs, in the integers and floats fsk_transmit_stdin
+ * (src/minimodem.c:114-250) and the tone generator compute them (passed by value). */
+#define FSK_B200_ENCODE_WORDS 2		/* pre-encoded data words (fsk_b200_tx_batch) */
+typedef struct fsk_b200_tx_plan {
+    uint32_t	rate;			/* simpleaudio_get_rate(): the tone's wave length is (float)rate / freq */
+    float	f_mark, f_space;
+    uint32_t	bit, start, stop;	/* samples of a data bit, the start and the stop tone (0 = none), :96-97, :110-111, :132 */
+    uint32_t	idle;			/* samples of the idle tone, idle_carrier_usec * rate / 1000000, :236 */
+    uint32_t	n_data_bits;		/* 1..32 */
+    uint32_t	tones_per_frame;	/* (start > 0) + n_data_bits + (stop > 0) */
+    int		has_start, has_stop;	/* nstartbits > 0, nstopbits > 0 (:95, :109) */
+    int		invert_start_stop, msb_first;
+    uint32_t	nsync, sync_byte, leader, trailer;
+    int		encoder;		/* FSK_B200_ENCODE_* */
+    uint32_t	lut_len;		/* 0: sin() per sample */
+    float	mag;			/* tone_mag (float output without a table) */
+    float	mag_s;			/* (float)mag_s (int16 output without a table), src/simple-tone-generator.c:146-150 */
+    int		float_samples;
+} fsk_b200_tx_plan;
+
+/* one launch: text rows (or pre-encoded words) in, sample rows out */
+typedef struct fsk_b200_tx_io {
+    const uint8_t *text;		/* encoder ASCII8 / BAUDOT: [nstreams][text_stride], text_len[s] bytes */
+    size_t	text_stride;
+    const uint32_t *text_len;
+    const uint32_t *words;		/* encoder WORDS: [nstreams][nwords] */
+    uint32_t	nwords;
+    const uint32_t *lead_in;		/* WORDS: samples of silence before the signal (may be NULL) */
+    fsk_b200_tx_state *states;		/* NULL: every stream fresh, and FINAL */
+    void	*out;
+    size_t	out_stride;
+    uint32_t	*out_len;		/* samples written per stream (may be NULL when cap != 0) */
+    uint32_t	cap;			/* 0: a row ends with its signal; else exactly cap samples, zero padded / truncated */
+    uint32_t	flags;			/* FSK_B200_TX_* */
+    size_t	nstreams;
+} fsk_b200_tx_io;
+
 void fsk_b200_set_error(const char *fmt, ...);
 
 /* host-side pure derivations (fsk_b200_host.c) */
@@ -149,9 +187,12 @@ int  fsk_b200_cuda_detect_carrier_batch(int fftsize, const float *samples, size_
 int  fsk_b200_cuda_stream_push(float *samples, size_t nstreams, size_t stride, uint32_t *fill,
 	fsk_b200_stream_state *states, const float *chunk, size_t chunk_stride, const uint32_t *chunk_len,
 	uint32_t chunk_len_all, uint32_t *dropped, void *stream);
-int  fsk_b200_cuda_tx_batch(const fsk_b200_tx_config *cfg, const float *sin_table,
-	uint32_t table_len, const uint32_t *words, uint32_t nwords, const uint32_t *lead_in,
-	float *samples_out, size_t nstreams, size_t stride, uint32_t nsamples_out, void *stream);
+/* the synthesis kernel; lut: device table of plan->lut_len float or int16 entries */
+int  fsk_b200_cuda_tx_synth(const fsk_b200_tx_plan *plan, const void *lut, const fsk_b200_tx_io *io,
+	void *stream);
+/* device copy of `bytes` host bytes (NULL on failure), and its release */
+void *fsk_b200_cuda_upload(const void *host, size_t bytes);
+void fsk_b200_cuda_free(void *dev);
 int  fsk_b200_cuda_s16_to_f32(const int16_t *src, float *dst, size_t nstreams, size_t stride, void *stream);
 int  fsk_b200_cuda_rx_batch_host_s16(void *ce, const fsk_b200_geom *g, const fsk_b200_loopc *lc,
 	const int16_t *host_samples, size_t nstreams, size_t stride, uint32_t nsamples_all,

@@ -31,7 +31,8 @@
  *                         copies; SRC 0 float32 rows, 1 int16 PCM rows widened inside the fill
  * k_rx_ws<G,W,L>          MODE 0, warp-synchronous (selectable)
  * k_find_frame<G,W,L,MODE> batched fsk_find_frame
- * k_tx, k_band_mags, k_detect_carrier, k_s16_to_f32, k_decode<KIND>   the "next" rows (DESIGN.md 0)
+ * k_tx_synth<T,VEC,LUT>   the transmitter: text (or data words) -> int16 / float32 samples
+ * k_band_mags, k_detect_carrier, k_s16_to_f32, k_decode<KIND>   the "next" rows (DESIGN.md 0)
  *
  * Compiled with -fmad=false: every a*b+c below is either an explicit fmaf() (the
  * correlation sums) or two separately rounded operations, as in the reference's
@@ -1006,74 +1007,346 @@ __global__ void k_detect_carrier(const float *__restrict__ samples, unsigned nst
 }
 
 /* ------------------------------------------------------------------------ */
-/* transmitter signal model, one warp per stream                            */
+/* transmitter: bytes -> data words -> tones -> samples, one warp per stream */
 /* (src/minimodem.c:81-250, src/simple-tone-generator.c:107-175)            */
 /* ------------------------------------------------------------------------ */
+/* A stream's signal is a sequence of TONES (frequency, duration): optional silence (the lead-in of
+ * fsk_b200_tx_batch), leader, sync-byte preamble, the frames of the data words, the idle tone,
+ * the trailer.  The warp makes them 32 at a time, lane j tone j of the batch: its duration, the
+ * start sample (a warp scan of the durations) and its starting phase (the reference's serial
+ * cphase chain, one add and one fractional part per tone) go into a ring of the last 64 tones in
+ * shared memory.  Then the lanes write the samples up to the end of the batch, lane j the VEC
+ * consecutive samples of vector j, j + 32, ... whatever tone they fall in: a bit of 40 samples
+ * does not leave lanes idle, and each lane stores 16 bytes at a time when the row alignment
+ * allows it.  The words come from the stream's bytes 32 at a time, encoded by the lanes side by
+ * side; Baudot's charset (the only state an encoder has) is carried across the lanes by a warp
+ * scan of the three-state transition maps. */
 
-struct TxLens { unsigned bit, start, stop, rate; };
+#define TX_WARPS 4			/* warps (streams) per block */
+#define TX_RING 64			/* tones kept per warp: the batch being written and the one before */
+#define TX_WRING 128			/* data words kept per warp */
 
-__device__ __forceinline__ void tx_tone(float *o, unsigned &pos, unsigned cap, float &cphase,
-	unsigned rate, float freq, unsigned dur, const float *__restrict__ lut, unsigned len,
-	unsigned lane)
+/* fmodf(x, 1.0f) for x >= 0, exactly: the fractional part of a float is representable, so
+ * x - trunc(x) is computed without rounding -- the same value the reference's fmodf returns
+ * (src/simple-tone-generator.c:162-163), for a third of the instructions on the serial chain */
+__device__ __forceinline__ float tx_frac(float x)
 {
-    const float wave = (float)rate / freq;			/* :116 */
-    for (unsigned i = lane; i < dur; i += 32) {
-	const float turns = (float)i / wave + cphase;		/* :121 */
-	int t = (int)((float)len * turns + 0.5f);		/* :91 */
-	t %= (int)len;
-	if (pos + i < cap)
-	    o[pos + i] = lut[t];
-    }
-    pos += dur;
-    cphase = fmodf(cphase + (float)dur / wave, 1.0f);		/* :163 */
+    return x - truncf(x);
 }
 
-__device__ __forceinline__ void tx_frame(float *o, unsigned &pos, unsigned cap, float &cphase,
-	const fsk_b200_tx_config &c, const TxLens &L, unsigned bits, int msb_first,
-	const float *__restrict__ lut, unsigned len, unsigned lane)
+/* sin(x) in double precision for 0 <= x < 2^22 (x = 2 pi turns; a tone of up to ~667 000 cycles):
+ * a two-constant reduction by pi/2 with exact fma products, then the Taylor series of sin or cos
+ * on |r| <= pi/4 (truncation below 1e-19).  Rounded to float it equals (float)sin((double)x) of
+ * glibc on every float of that range (checked exhaustively on the CPU); unlike CUDA's sin() it
+ * has no slow-path call, whose register saves spill in this kernel. */
+__device__ __forceinline__ double tx_sin(float xf)
 {
-    if (c.nstartbits > 0)
-	tx_tone(o, pos, cap, cphase, L.rate, c.invert_start_stop ? c.f_mark : c.f_space, L.start,
-		lut, len, lane);
-    for (unsigned i = 0; i < c.n_data_bits; i++) {
-	const unsigned bit = msb_first ? (bits >> (c.n_data_bits - i - 1)) & 1u : (bits >> i) & 1u;
-	tx_tone(o, pos, cap, cphase, L.rate, bit ? c.f_mark : c.f_space, L.bit, lut, len, lane);
-    }
-    if (c.nstopbits > 0)
-	tx_tone(o, pos, cap, cphase, L.rate, c.invert_start_stop ? c.f_space : c.f_mark, L.stop,
-		lut, len, lane);
+    const double x = (double)xf;
+    const double q = rint(x * 0.63661977236758134308);
+    double r = fma(-q, 0x1.921fb54442d18p0, x);
+    r = fma(-q, 0x1.1a62633145c07p-54, r);
+    const double z = r * r;
+    const double sn = r + r * z * (-1.0 / 6 + z * (1.0 / 120 + z * (-1.0 / 5040 + z * (1.0 / 362880
+	    + z * (-1.0 / 39916800 + z * (1.0 / 6227020800.0 + z * (-1.0 / 1307674368000.0
+	    + z * (1.0 / 355687428096000.0))))))));
+    const double cs = 1.0 + z * (-0.5 + z * (1.0 / 24 + z * (-1.0 / 720 + z * (1.0 / 40320
+	    + z * (-1.0 / 3628800 + z * (1.0 / 479001600.0 + z * (-1.0 / 87178291200.0
+	    + z * (1.0 / 20922789888000.0 + z * (-1.0 / 6402373705728000.0)))))))));
+    const int k = (int)q & 3;
+    return k == 0 ? sn : k == 1 ? cs : k == 2 ? -sn : -cs;
 }
 
-__global__ void k_tx(const __grid_constant__ fsk_b200_tx_config c, TxLens L,
-	const float *__restrict__ lut, unsigned len, const uint32_t *__restrict__ words,
-	unsigned nwords, const uint32_t *__restrict__ lead_in, float *__restrict__ out,
-	unsigned nstreams, size_t stride, unsigned cap)
+/* warp-inclusive sum */
+__device__ __forceinline__ unsigned tx_scan_add(unsigned v, unsigned lane)
 {
-    const unsigned lane = threadIdx.x & 31;
-    const unsigned s = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-    if (s >= nstreams)
-	return;
-    float *o = out + (size_t)s * stride;
-    unsigned pos = lead_in ? min(lead_in[s], cap) : 0u;
-    for (unsigned i = lane; i < pos; i += 32)
-	o[i] = 0.f;
-    float cphase = 0.f;
-    const uint32_t *w = words + (size_t)s * nwords;
-    if (nwords) {
-	for (int j = 0; j < c.leader_bits; j++)
-	    tx_tone(o, pos, cap, cphase, L.rate, c.invert_start_stop ? c.f_space : c.f_mark, L.bit,
-		    lut, len, lane);
-	for (unsigned j = 0; j < c.do_tx_sync_bytes; j++)
-	    tx_frame(o, pos, cap, cphase, c, L, c.sync_byte, 0, lut, len, lane);
-	for (unsigned j = 0; j < nwords; j++)
-	    tx_frame(o, pos, cap, cphase, c, L, w[j], c.msb_first, lut, len, lane);
-	for (int j = 0; j < c.trailer_bits; j++)
-	    tx_tone(o, pos, cap, cphase, L.rate, c.f_mark, L.bit, lut, len, lane);
+    for (unsigned o = 1; o < 32; o <<= 1) {
+	const unsigned u = __shfl_sync(0xffffffffu, v, lane >= o ? lane - o : lane);
+	if (lane >= o)
+	    v += u;
     }
-    for (unsigned i = min(pos, cap) + lane; i < cap; i += 32)
-	o[i] = 0.f;
+    return v;
 }
 
+/* Baudot charset transition maps: 2 bits per incoming charset (0, 1, 2) */
+#define TX_MAP_ID (0u | 1u << 2 | 2u << 4)
+__device__ __forceinline__ unsigned tx_map_apply(unsigned m, unsigned cs) { return (m >> (2 * cs)) & 3u; }
+__device__ __forceinline__ unsigned tx_map_then(unsigned first, unsigned second)
+{
+    unsigned r = 0;
+    for (unsigned cs = 0; cs < 3; cs++)
+	r |= tx_map_apply(second, tx_map_apply(first, cs)) << (2 * cs);
+    return r;
+}
+
+/* the sample at i samples into a tone (wave == 0: silence) */
+template <typename T, bool LUT>
+__device__ __forceinline__ T tx_sample(const fsk_b200_tx_plan &P, const T *lut, unsigned i, float wave,
+	float cph)
+{
+    if (wave == 0.0f)
+	return (T)0;
+    const float turns = (float)i / wave + cph;				/* :121 */
+    if constexpr (LUT) {
+	int t = (int)((float)P.lut_len * turns + 0.5f);			/* :77-84, :89-96 */
+	t = (P.lut_len & (P.lut_len - 1u)) ? t % (int)P.lut_len : t & (int)(P.lut_len - 1u);
+	return lut[t];
+    }
+    /* :133-134, :151-152, with the sine in double precision for glibc's sinf (DESIGN.md 5) */
+    const float s = (float)tx_sin((float)M_PI * 2 * turns);
+    if constexpr (sizeof(T) == 4)
+	return (T)(P.mag * s);
+    else
+	return (T)lroundf(P.mag_s * s);
+}
+
+template <typename T, int VEC>
+__device__ __forceinline__ void tx_store(T *row, unsigned q0, unsigned end, const T (&v)[VEC])
+{
+    if constexpr (VEC > 1) {
+	if (q0 + VEC <= end) {
+	    if constexpr (sizeof(T) == 4) {
+		*reinterpret_cast<float4 *>(row + q0) = make_float4(v[0], v[1], v[2], v[3]);
+	    } else {
+		int4 w;
+		w.x = (int)((uint16_t)v[0] | (unsigned)(uint16_t)v[1] << 16);
+		w.y = (int)((uint16_t)v[2] | (unsigned)(uint16_t)v[3] << 16);
+		w.z = (int)((uint16_t)v[4] | (unsigned)(uint16_t)v[5] << 16);
+		w.w = (int)((uint16_t)v[6] | (unsigned)(uint16_t)v[7] << 16);
+		*reinterpret_cast<int4 *>(row + q0) = w;
+	    }
+	    return;
+	}
+    }
+    for (int e = 0; e < VEC; e++)
+	if (q0 + e < end)
+	    row[q0 + e] = v[e];
+}
+
+/* samples [from, to) of the row (from a multiple of VEC): the tones [lo, hi) are in the ring,
+ * tones end at sample `sig_end`, zeros follow */
+template <typename T, int VEC, bool LUT>
+__device__ __forceinline__ void tx_write(const fsk_b200_tx_plan &P, const T *lut, const float4 *ring,
+	unsigned lo, unsigned hi, unsigned sig_end, T *row, unsigned from, unsigned to, unsigned lane)
+{
+    for (unsigned q0 = from + lane * VEC; q0 < to; q0 += 32 * VEC) {
+	T v[VEC];
+	unsigned idx = lo, next = 0xffffffffu;
+	float wave = 0.0f, cph = 0.0f;
+	unsigned start = 0;
+	if (q0 < sig_end) {
+	    unsigned a = lo, b = hi;				/* the last tone that starts at or before q0 */
+	    while (b - a > 1) {
+		const unsigned m = (a + b) >> 1;
+		if (__float_as_uint(ring[m % TX_RING].x) <= q0)
+		    a = m;
+		else
+		    b = m;
+	    }
+	    idx = a;
+	    const float4 r = ring[idx % TX_RING];
+	    start = __float_as_uint(r.x), wave = r.y, cph = r.z;
+	    next = idx + 1 < hi ? __float_as_uint(ring[(idx + 1) % TX_RING].x) : 0xffffffffu;
+	}
+#pragma unroll
+	for (int e = 0; e < VEC; e++) {
+	    const unsigned q = q0 + e;
+	    if (q >= sig_end) {
+		v[e] = (T)0;
+		continue;
+	    }
+	    while (q >= next) {					/* the next tone(s) begin inside this vector */
+		idx++;
+		const float4 r = ring[idx % TX_RING];
+		start = __float_as_uint(r.x), wave = r.y, cph = r.z;
+		next = idx + 1 < hi ? __float_as_uint(ring[(idx + 1) % TX_RING].x) : 0xffffffffu;
+	    }
+	    v[e] = tx_sample<T, LUT>(P, lut, q - start, wave, cph);
+	}
+	tx_store<T, VEC>(row, q0, to, v);
+    }
+}
+
+template <typename T, int VEC, bool LUT>
+__global__ void __launch_bounds__(TX_WARPS * 32, 8) k_tx_synth(const __grid_constant__ fsk_b200_tx_plan P,
+	const __grid_constant__ fsk_b200_tx_io io, const T *__restrict__ lut_global, unsigned lut_in_smem)
+{
+    FSK_DYN_SMEM(smem);
+    T *lut_s = reinterpret_cast<T *>(smem);
+    const unsigned lut_bytes = lut_in_smem ? ((P.lut_len * (unsigned)sizeof(T) + 15u) & ~15u) : 0u;
+    unsigned *btab = reinterpret_cast<unsigned *>(reinterpret_cast<unsigned char *>(smem) + lut_bytes);
+    float4 *rings = reinterpret_cast<float4 *>(btab + 96);
+    unsigned *wrings = reinterpret_cast<unsigned *>(rings + TX_WARPS * TX_RING);
+    if (lut_in_smem)
+	for (unsigned i = threadIdx.x; i < P.lut_len; i += blockDim.x)
+	    lut_s[i] = lut_global[i];
+    if (P.encoder == FSK_B200_ENCODE_BAUDOT)
+	for (unsigned i = threadIdx.x; i < 96; i += blockDim.x)
+	    btab[i] = fsk_enc_baudot_entry((int)i);
+    __syncthreads();
+    const T *lut = lut_in_smem ? lut_s : lut_global;
+
+    const unsigned lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const size_t s = (size_t)blockIdx.x * TX_WARPS + warp;
+    if (s >= io.nstreams)
+	return;						/* whole warps leave together */
+    float4 *ring = rings + warp * TX_RING;
+    unsigned *wring = wrings + warp * TX_WRING;
+    T *row = reinterpret_cast<T *>(io.out) + s * io.out_stride;
+
+    fsk_b200_tx_state st = { 0.0f, 0u, 0u, 0u };
+    if (io.states)
+	st = io.states[s];
+    const unsigned flags = io.states ? io.flags : FSK_B200_TX_FINAL;
+    const unsigned tpf = P.tones_per_frame;
+    const unsigned n_in = P.encoder == FSK_B200_ENCODE_WORDS ? io.nwords
+	    : io.text_len[s] < io.text_stride ? io.text_len[s] : (unsigned)io.text_stride;
+    const unsigned lead = io.lead_in ? min(io.lead_in[s], io.cap) : 0u;
+
+    /* the tone sequence, src/minimodem.c:202-237, :246-247, :60-66 */
+    const unsigned nS = lead ? 1u : 0u;
+    const unsigned nL = n_in && st.transmitting == 0 ? P.leader : 0u;
+    const unsigned nP = n_in && st.transmitting < 2 ? P.nsync * tpf : 0u;
+    const unsigned nI = !n_in && (flags & FSK_B200_TX_IDLE_IF_EMPTY) ? 1u : 0u;
+    const unsigned tx_after = n_in ? 2u : nI ? 1u : st.transmitting;
+    const unsigned nT = (flags & FSK_B200_TX_FINAL) && tx_after ? P.trailer : 0u;
+    const unsigned d0 = nS + nL + nP;			/* the first tone of the data frames */
+    const float mark_idle = P.invert_start_stop ? P.f_space : P.f_mark;
+
+    unsigned nread = 0, nenc = 0, charset = st.baudot_charset;
+    float cphase = st.cphase;
+    unsigned sig_end = 0, written = 0, G = 0, nb = 0;
+    const unsigned cap = io.cap;
+    for (;; G += 32) {
+	/* encode until the words of this batch's data tones are there */
+	if (G + 31 >= d0) {
+	    const unsigned w_hi = (G + 31 - d0) / tpf;
+	    while (nread < n_in && nenc <= w_hi) {
+		const unsigned take = min(32u, n_in - nread);
+		unsigned w0 = 0, w1 = 0, cnt = 0;
+		if (P.encoder == FSK_B200_ENCODE_WORDS) {
+		    if (lane < take) {
+			w0 = io.words[s * io.nwords + nread + lane];
+			cnt = 1;
+		    }
+		} else {
+		    const unsigned byte = lane < take ? io.text[s * io.text_stride + nread + lane] : 0u;
+		    if (P.encoder == FSK_B200_ENCODE_ASCII8) {
+			w0 = fsk_enc_ascii8(byte);
+			cnt = lane < take ? 1u : 0u;
+		    } else {
+			const int c = fsk_enc_toupper((int)(int8_t)(uint8_t)byte);
+			const unsigned entry = c >= 0 && c < 0x60 ? btab[c] : 0u;
+			uint32_t w[2];
+			unsigned map = TX_MAP_ID;
+			if (lane < take) {
+			    map = 0;
+			    for (unsigned cs = 0; cs < 3; cs++) {
+				uint32_t t = cs;
+				fsk_enc_baudot_with(&t, c, entry, w);
+				map |= t << (2 * cs);
+			    }
+			}
+			unsigned incl = map;			/* charset map of bytes 0..lane */
+			for (unsigned o = 1; o < 32; o <<= 1) {
+			    const unsigned u = __shfl_sync(0xffffffffu, incl, lane >= o ? lane - o : lane);
+			    if (lane >= o)
+				incl = tx_map_then(u, incl);
+			}
+			const unsigned excl = __shfl_sync(0xffffffffu, incl, lane ? lane - 1 : 0);
+			uint32_t cs_in = tx_map_apply(lane ? excl : TX_MAP_ID, charset);
+			if (lane < take) {
+			    cnt = fsk_enc_baudot_with(&cs_in, c, entry, w);
+			    w0 = w[0];
+			    w1 = w[1];
+			}
+			charset = tx_map_apply(__shfl_sync(0xffffffffu, incl, 31), charset);
+		    }
+		}
+		const unsigned end = tx_scan_add(cnt, lane);
+		const unsigned at = nenc + end - cnt;
+		if (cnt > 0)
+		    wring[at % TX_WRING] = w0;
+		if (cnt > 1)
+		    wring[(at + 1) % TX_WRING] = w1;
+		nenc += __shfl_sync(0xffffffffu, end, 31);
+		nread += take;
+		__syncwarp();
+	    }
+	}
+	const unsigned nD = nread == n_in ? nenc * tpf : 0xffffffffu;
+	const unsigned total = nread == n_in ? d0 + nD + nI + nT : 0xffffffffu;
+	if (G >= total)
+	    break;
+	nb = min(32u, total - G);
+
+	/* lane j: tone G + j */
+	float freq = 0.0f;
+	unsigned dur = 0;
+	if (lane < nb) {
+	    unsigned k = G + lane;
+	    if (k < nS) {
+		dur = lead;					/* silence */
+	    } else if ((k -= nS) < nL) {
+		freq = mark_idle, dur = P.bit;			/* leader, :211-212 */
+	    } else if ((k -= nL) < nP || k - nP < nD) {
+		/* a frame, fsk_transmit_frame :81-112: the sync byte (LSB first, :218-221) or a data word */
+		const bool sync = k < nP;
+		unsigned b = (sync ? k : k - nP) % tpf;
+		const unsigned word = sync ? P.sync_byte : wring[((k - nP) / tpf) % TX_WRING];
+		const int msb = sync ? 0 : P.msb_first;
+		if (P.has_start && b-- == 0) {
+		    freq = P.invert_start_stop ? P.f_mark : P.f_space, dur = P.start;
+		} else if (b < P.n_data_bits) {
+		    const unsigned bit = msb ? (word >> (P.n_data_bits - b - 1)) & 1u : (word >> b) & 1u;
+		    freq = bit ? P.f_mark : P.f_space, dur = P.bit;
+		} else {
+		    freq = P.invert_start_stop ? P.f_space : P.f_mark, dur = P.stop;
+		}
+	    } else if ((k -= nP + nD) < nI) {
+		freq = mark_idle, dur = P.idle;			/* idle tone, :233-236 */
+	    } else {
+		freq = P.f_mark, dur = P.bit;			/* trailer, :65-66 */
+	    }
+	}
+	const unsigned end = tx_scan_add(dur, lane);
+	const unsigned start = sig_end + end - dur;
+	sig_end += __shfl_sync(0xffffffffu, end, 31);
+	/* the phase chain (src/simple-tone-generator.c:116, :162-163; a tone of frequency 0 is
+	 * silence and restarts the phase, :166-169) */
+	const float wave = freq != 0.0f ? (float)P.rate / freq : 0.0f;
+	const float step = freq != 0.0f ? (float)dur / wave : 0.0f;
+	float my_cph = 0.0f;
+	for (unsigned i = 0; i < nb; i++) {
+	    const float si = __shfl_sync(0xffffffffu, step, i);
+	    const float wi = __shfl_sync(0xffffffffu, wave, i);
+	    if (lane == i)
+		my_cph = cphase;
+	    cphase = wi != 0.0f ? tx_frac(cphase + si) : 0.0f;
+	}
+	if (lane < nb)
+	    ring[(G + lane) % TX_RING] = make_float4(__uint_as_float(start), wave, my_cph, 0.0f);
+	__syncwarp();
+	const bool last = G + nb >= total;
+	unsigned to = last ? (cap ? cap : sig_end) : sig_end / VEC * VEC;
+	if (cap)
+	    to = min(to, cap);
+	const unsigned hi = G + nb;
+	tx_write<T, VEC, LUT>(P, lut, ring, hi > TX_RING ? hi - TX_RING : 0u, hi, sig_end, row, written, to, lane);
+	written = max(written, to);
+	__syncwarp();
+	if (last || (cap && written >= cap))
+	    break;
+    }
+    if (cap && written < cap)				/* no tones at all: a silent row */
+	tx_write<T, VEC, LUT>(P, lut, ring, 0u, 0u, 0u, row, written, cap, lane);
+    if (io.states && lane == 0) {
+	st.cphase = cphase;
+	st.baudot_charset = charset;
+	st.transmitting = flags & FSK_B200_TX_FINAL ? 0u : tx_after;	/* :71 */
+	io.states[s] = st;
+	io.out_len[s] = sig_end;
+    }
+}
 /* ------------------------------------------------------------------------ */
 /* N2: int16 PCM -> float32 (x / 32768, exact), 8 samples per thread        */
 /* ------------------------------------------------------------------------ */
@@ -2253,26 +2526,61 @@ extern "C" int fsk_b200_cuda_detect_carrier_batch(int fftsize, const float *samp
     return 0;
 }
 
-extern "C" int fsk_b200_cuda_tx_batch(const fsk_b200_tx_config *cfg, const float *sin_table,
-	uint32_t table_len, const uint32_t *words, uint32_t nwords, const uint32_t *lead_in,
-	float *samples_out, size_t nstreams, size_t stride, uint32_t nsamples_out, void *stream)
+extern "C" void *fsk_b200_cuda_upload(const void *host, size_t bytes)
 {
-    TxLens L;
-    /* src/minimodem.c:131-132, :96-97, :110-111: size_t * float -> size_t */
-    const size_t sample_rate = (size_t)cfg->sample_rate;
-    const size_t bit = sample_rate / cfg->data_rate + 0.5f;
-    L.bit = (unsigned)bit;
-    L.start = (unsigned)(size_t)(bit * cfg->nstartbits);
-    L.stop = (unsigned)(size_t)(bit * cfg->nstopbits);
-    L.rate = (unsigned)sample_rate;
-    const unsigned threads = 128;
-    const size_t blocks = (nstreams * 32 + threads - 1) / threads;
-    FSK_LAUNCH(k_tx, (unsigned)blocks, threads, 0, (cudaStream_t)stream, *cfg, L, sin_table, table_len, words,
-	    nwords, lead_in, samples_out, (unsigned)nstreams, stride, nsamples_out);
+    void *d = NULL;
+    if (cudaMalloc(&d, bytes ? bytes : 16) != cudaSuccess) {
+	fsk_b200_set_error("cudaMalloc(%zu): %s", bytes, cudaGetErrorString(cudaGetLastError()));
+	return NULL;
+    }
+    if (bytes && cudaMemcpy(d, host, bytes, cudaMemcpyHostToDevice) != cudaSuccess) {
+	fsk_b200_set_error("cudaMemcpy: %s", cudaGetErrorString(cudaGetLastError()));
+	cudaFree(d);
+	return NULL;
+    }
+    return d;
+}
+
+extern "C" void fsk_b200_cuda_free(void *d)
+{
+    cudaFree(d);
+}
+
+template <typename T>
+static void tx_launch(const fsk_b200_tx_plan *p, const void *lut, const fsk_b200_tx_io *io, cudaStream_t st)
+{
+    const unsigned blocks = (unsigned)((io->nstreams + TX_WARPS - 1) / TX_WARPS);
+    /* the sine table goes to shared memory when it is small (16 KB at the default --lut=4096) */
+    const unsigned lut_bytes = p->lut_len * (unsigned)sizeof(T);
+    const unsigned in_smem = p->lut_len && lut_bytes <= 32768u;
+    const size_t smem = (in_smem ? ((lut_bytes + 15u) & ~15u) : 0u) + 96 * sizeof(unsigned)
+	    + TX_WARPS * (TX_RING * sizeof(float4) + TX_WRING * sizeof(unsigned));
+    /* 16-byte stores when every row starts 16-byte aligned */
+    const bool wide = ((uintptr_t)io->out & 15u) == 0 && (io->out_stride * sizeof(T)) % 16u == 0;
+    const T *l = (const T *)lut;
+    if (wide && p->lut_len)
+	FSK_LAUNCH((k_tx_synth<T, 16 / sizeof(T), true>), blocks, TX_WARPS * 32, smem, st, *p, *io, l, in_smem);
+    else if (wide)
+	FSK_LAUNCH((k_tx_synth<T, 16 / sizeof(T), false>), blocks, TX_WARPS * 32, smem, st, *p, *io, l, in_smem);
+    else if (p->lut_len)
+	FSK_LAUNCH((k_tx_synth<T, 1, true>), blocks, TX_WARPS * 32, smem, st, *p, *io, l, in_smem);
+    else
+	FSK_LAUNCH((k_tx_synth<T, 1, false>), blocks, TX_WARPS * 32, smem, st, *p, *io, l, in_smem);
+}
+
+extern "C" int fsk_b200_cuda_tx_synth(const fsk_b200_tx_plan *p, const void *lut, const fsk_b200_tx_io *io,
+	void *stream)
+{
+    if (io->nstreams == 0)
+	return 0;
+    if (p->float_samples)
+	tx_launch<float>(p, lut, io, (cudaStream_t)stream);
+    else
+	tx_launch<int16_t>(p, lut, io, (cudaStream_t)stream);
     g_launches++;
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) {
-	fsk_b200_set_error("tx_batch launch: %s", cudaGetErrorString(e));
+	fsk_b200_set_error("tx launch: %s", cudaGetErrorString(e));
 	return -EIO;
     }
     return 0;
