@@ -478,8 +478,10 @@ int fsk_b200_tx_text_batch(fsk_b200_tx_engine *te, const uint8_t *text, size_t n
 	const uint32_t *text_len, unsigned int flags, fsk_b200_tx_state *states, void *out, size_t out_stride,
 	uint32_t *out_len, void *stream);
 
-/* Diagnostics: which rx kernel the engine's latest fsk_b200_rx_batch launched ("k_rx<G=8,W=3,L=2,mode=2
- * (shared-segment),fill=0> threads=64 ring=640 smem=23232 blocks=8192"; "" before the first launch). */
+/* Diagnostics: which kernel instance the engine's latest fsk_b200_rx_batch or fsk_b200_find_frame_batch
+ * launched ("k_rx<G=8,W=3,L=2,mode=2(shared-segment),fill=0,src=f32> threads=64 ring=640 smem=23232
+ * blocks=8192", "k_find_frame<G=8,W=2,L=1,mode=0(per-candidate)> ..."; "" before the first launch).  `fill`
+ * is that of the kernel that ran: FSK_B200_FILL asks for an alternative that is built for a few shapes only. */
 const char *fsk_b200_engine_last_kernel(const fsk_b200_engine *e);
 
 /* Library / build information: "fsk_b200 <version> sm_90a". */

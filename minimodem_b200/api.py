@@ -393,7 +393,7 @@ class RxEngine:
             _err("fsk_b200_engine_tune", rc)
 
     def last_kernel(self):
-        """Which rx kernel the latest rx_batch launched (diagnostics)."""
+        """Which kernel instance the latest rx_batch or find_frame_batch launched (diagnostics)."""
         return lib().fsk_b200_engine_last_kernel(self._e).decode()
 
     def max_frames(self, nsamples):

@@ -3,7 +3,7 @@
  *
  * Two basic implementations of the same arithmetic:
  *
- *  FAST   frame_analyze_fast<G,W,L> / find_frame_fast: the stream's samples are in a
+ *  FAST   frame_analyze_fast<G,W,L> / find_frame_fast_body: the stream's samples are in a
  *         per-stream shared-memory ring of R floats (R % 4 == 0) whose first
  *         window-length is mirrored behind its end, so a bit window is always one
  *         linear run; each lane owns W windows (and 1/L of their samples) and
@@ -148,7 +148,7 @@ __device__ __forceinline__ void resum_fp64(const Src &src, unsigned base, unsign
 template <int G, class Src>
 __device__ __noinline__ float frame_analyze(const Src &src, unsigned t0,
 	const fsk_b200_geom &geo, int sel, const float4 *__restrict__ tw, float2 *scr,
-	unsigned g, unsigned gmask, unsigned long long &bits_out, float &ampl_out)
+	unsigned g, unsigned gmask, unsigned long long &bits_out, float &ampl_out, float2 *mags_out = nullptr)
 {
     const unsigned N = geo.bit_nsamples, nb = geo.n_bits, L = geo.lanes_per_window;
     const unsigned wpp = G / L;			/* windows analysed per pass */
@@ -191,6 +191,8 @@ __device__ __noinline__ float frame_analyze(const Src &src, unsigned t0,
 	    if (needs_resum(mag_mark, mag_space))
 		resum_fp64(src, t0 + geo.bit_begin[w], N, tw, geo.mag_scalar, mag_mark, mag_space);
 	    mismatch |= decide_bit(mag_mark, mag_space, geo.expect[sel][w], scr + w);
+	    if (mags_out)		/* (signal, noise) per bit: the statistic below reuses the scratch */
+		mags_out[w] = make_float2(scr[w].x, fabsf(scr[w].y));
 	}
     }
     __syncwarp(gmask);
@@ -789,18 +791,6 @@ __device__ __forceinline__ Found find_frame_slide(const Ring rg, unsigned pos_of
 	    p[j] = ring + ring_wrap(ring_wrap(pos_off + t, R) + lw.beg[j], R);	/* window starts (fp64 re-sum) */
     }
     return best;
-}
-
-/* the same, as a call: the kernels with more than one search site keep one copy of the code */
-template <int G, int W, int L>
-__device__ __noinline__ Found find_frame_fast(const Ring rg, unsigned pos_off,
-	const fsk_b200_geom &geo, const LaneWin<W> lw, int sel, unsigned tw_s,
-	unsigned g, unsigned gmask, unsigned try_first, unsigned try_max, unsigned try_step, float limit,
-	int ready = 0, bool pending = false)
-{
-    unsigned ncand = 0;
-    return find_frame_fast_body<G, W, L>(rg, pos_off, geo, lw, sel, tw_s, g, gmask, try_first, try_max,
-	    try_step, limit, ready, pending, ncand);
 }
 
 /* ======================================================================== */

@@ -193,8 +193,12 @@ k_find_frame(const __grid_constant__ fsk_b200_geom geo, const float4 *__restrict
 		cp_async_commit();
 		cp_async_wait<0>();
 		__syncwarp(gmask);
-		const Found f = find_frame_fast<G, W, L>(rg, off & 3u, geo, lw, sel, tw_s, g, gmask,
-			a.try_first[s], tmax, tstep, a.limit[s]);
+		/* the search inlined, as k_rx has it: built as a separate __noinline__ call taking the LaneWin by
+		 * value, the sm_90a code returned wrong bits for the first window of every lane at W = 4, L = 1
+		 * (magnitudes, decisions and confidence right; tests/test_gpu_instantiations.py) */
+		unsigned ncand = 0;
+		const Found f = find_frame_fast_body<G, W, L>(rg, off & 3u, geo, lw, sel, tw_s, g, gmask,
+			a.try_first[s], tmax, tstep, a.limit[s], 0, false, ncand);
 		conf = f.confidence;
 		ampl = f.amplitude;
 		start = f.start;
@@ -214,12 +218,8 @@ k_find_frame(const __grid_constant__ fsk_b200_geom geo, const float4 *__restrict
 		if (a.bit_mags) {
 		    unsigned long long b2;
 		    float am;
-		    (void)frame_analyze<G, GlobalSrc>(src, off + start, geo, sel, sm.tw, sm.scr, g, gmask, b2, am);
-		    __syncwarp(gmask);
-		    /* the scratch holds (signal, +-noise) per bit unless pass 1 rejected the candidate midway */
-		    for (unsigned w = g; w < geo.n_bits; w += G)
-			a.bit_mags[(size_t)s * geo.n_bits + w] = make_float2(sm.scr[w].x, fabsf(sm.scr[w].y));
-		    __syncwarp(gmask);
+		    (void)frame_analyze<G, GlobalSrc>(src, off + start, geo, sel, sm.tw, sm.scr, g, gmask, b2, am,
+			    a.bit_mags + (size_t)s * geo.n_bits);
 		}
 	    }
 	}
@@ -2072,6 +2072,9 @@ extern "C" int fsk_b200_cuda_find_frame_batch(void *p, const fsk_b200_geom *g, c
     } else {
 	e = launch_find_t<32, 1, 1, 1>(sh, ce, a, st);
     }
+    snprintf(ce->last_kernel, sizeof(ce->last_kernel),
+	    "k_find_frame<G=%d,W=%d,L=%d,mode=%d(%s)> threads=%d ring=%u smem=%zu blocks=%d", sh.G, sh.W, sh.L, sh.mode,
+	    sh.mode == 0 ? "per-candidate" : "generic", sh.wpb * 32, sh.ring, sh.smem, sh.blocks);
     if (e != cudaSuccess) {
 	fsk_b200_set_error("find_frame_batch launch (G=%d W=%d L=%d mode=%d smem=%zu): %s", sh.G, sh.W,
 		sh.L, sh.mode, sh.smem, cudaGetErrorString(e));
@@ -2134,6 +2137,7 @@ static int rx_batch_any(CudaEngine *ce, const fsk_b200_geom *g, const fsk_b200_l
     cudaStream_t st = (cudaStream_t)stream;
     cudaError_t e = cudaErrorInvalidValue;
     bool launched = false;
+    int fill = ce->fill;	/* mode 0: the fill of the kernel that actually ran (last_kernel) */
     if (elem == 2) {
 	if (ce->fill != 0)
 	    return -ENOTSUP;
@@ -2185,6 +2189,7 @@ static int rx_batch_any(CudaEngine *ce, const fsk_b200_geom *g, const fsk_b200_l
 #undef X
 	}
 	if (!launched) {
+	    fill = 0;		/* the alternatives are not built for this shape: the default kernel runs */
 #define X(GG, WW, LL) if (sh.G == GG && sh.W == WW && sh.L == LL) e = launch_rx_t<GG, WW, LL, 0, 0>(sh, ce, lc, a, st);
 	    FAST_COMBOS(X)
 #undef X
@@ -2195,7 +2200,7 @@ static int rx_batch_any(CudaEngine *ce, const fsk_b200_geom *g, const fsk_b200_l
     snprintf(ce->last_kernel, sizeof(ce->last_kernel),
 	    "k_rx<G=%d,W=%d,L=%d,mode=%d(%s),fill=%d,src=%s> threads=%d ring=%u smem=%zu blocks=%d", sh.G, sh.W, sh.L,
 	    sh.mode, sh.mode == 3 ? "prefix-table" : sh.mode == 2 ? "shared-segment" : sh.mode == 0 ? "per-candidate" : "generic",
-	    sh.mode == 0 ? ce->fill : (sh.mode == 3 && elem == 4) ? ce->pfx_fill : 0, elem == 2 ? (sh.slide ? "s16,slide" : "s16") : (sh.slide ? "f32,slide" : "f32"),
+	    sh.mode == 0 ? fill : (sh.mode == 3 && elem == 4) ? ce->pfx_fill : 0, elem == 2 ? (sh.slide ? "s16,slide" : "s16") : (sh.slide ? "f32,slide" : "f32"),
 	    sh.wpb * 32, sh.ring, sh.smem, sh.blocks);
     if (e != cudaSuccess) {
 	fsk_b200_set_error("rx_batch launch (G=%d W=%d L=%d mode=%d ring=%u smem=%zu): %s", sh.G, sh.W,

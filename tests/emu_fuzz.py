@@ -6,8 +6,11 @@ makes the stream, the oracle's rx loop says what the records must be, the kernel
 host SIMT emulator) has to produce them -- exact bits, frame starts and acquire flags, confidence
 and amplitude to the parity tolerance.  This is a logic check of the kernels over geometry the
 vectors do not reach (window counts from 7 to 44 bits, every lane split the launcher picks,
-fractional samples per bit, long windows); it runs on the emulator only, because a near-tie that
-the GPU's approximate divide resolves the other way would make a random case flaky there."""
+fractional samples per bit, long windows), run on the emulator.  Random framings reach the hardware
+through tests/test_gpu_instantiations.py instead: there every stream first goes through a
+deterministic near-tie screen (tests/tie_screen.py), so that a stream whose records a knife-edge
+decision could flip under the device's approximate units is known in advance rather than being a
+flaky case, and all other streams are compared exactly."""
 import numpy as np
 import pytest
 

@@ -14,8 +14,8 @@ import pytest
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
-def run_emulated(select, async_mode, timeout, module="test_gpu_parity.py"):
-    env = dict(os.environ, FSK_B200_EMU="1", FSK_EMU_ASYNC=async_mode)
+def run_emulated(select, async_mode, timeout, module="test_gpu_parity.py", extra_env=None):
+    env = dict(os.environ, FSK_B200_EMU="1", FSK_EMU_ASYNC=async_mode, **(extra_env or {}))
     env.pop("FSK_B200_LIB", None)
     r = subprocess.run([sys.executable, "-m", "pytest", os.path.join(ROOT, "tests", module),
                         "-m", "gpu", "-q", "-x", "-p", "no:cacheprovider", "-k", select],
@@ -46,6 +46,17 @@ def test_random_modes_and_dropouts_on_the_emulated_kernels():
     tail = run_emulated("random_mode or dropouts or second_batch or batched_kernels_print", "late", 1200,
                         module="emu_fuzz.py")
     assert "failed" not in tail and ("137 passed" in tail or "138 passed" in tail)     # one seed is ring-limited
+
+
+def test_every_instantiation_on_the_emulated_kernels_with_perturbed_units():
+    """tests/test_gpu_instantiations.py at the device's sizes (under a minute): every rx, find-frame and
+    transmitter instance the launchers can dispatch (the TMA bulk fills excepted: not emulated), on random
+    framings, with the approximate sqrt and divide perturbed by up to 64 ulp (FSK_EMU_ULP=64).  Every stream the near-tie
+    screen calls robust must still give the oracle's records: the screen's margin covers arithmetic that
+    differs from the oracle's, which is what makes the random cases exact on the GPU."""
+    tail = run_emulated("instantiation or screen or odd_stride", "late", 900, module="test_gpu_instantiations.py",
+                        extra_env={"FSK_EMU_ULP": "64"})
+    assert " passed" in tail and "failed" not in tail
 
 
 def test_the_emulator_itself():
