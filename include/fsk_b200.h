@@ -294,6 +294,47 @@ int fsk_b200_stream_push(float *samples, size_t nstreams, size_t stride, uint32_
 int fsk_b200_detect_carrier_batch(int fftsize, const float *samples, size_t nstreams, size_t stride,
 	const uint32_t *offset, uint32_t nsamples, float min_mag_threshold, int32_t *out_band, void *stream);
 
+/* --auto-carrier (-a, src/minimodem.c:1179-1220) inside the batched rx loop: every stream finds its own
+ * tone pair, and finds it again after each carrier loss.  While a stream has no band it scans windows of
+ * min(nsamples_per_bit, fftsize) samples with fsk_detect_carrier's rule; a band b is accepted when its
+ * space band b + b_shift lies in [1, nbands), and the same iteration searches a frame on (b, b + b_shift).
+ * More than 20 iterations without confidence drop the band (:1295-1297).  The scan covers what the
+ * reference's sample ring would hold, so the scan grid is the reference CLI's on the same audio; DESIGN.md
+ * section 5, item 10, says where the records can still differ from the CLI's.
+ *
+ * fsk_b200_auto_state: 16 bytes per stream, all zeros for a fresh stream, kept with the
+ * fsk_b200_stream_state to continue a stream.
+ * fsk_b200_rx_config_autodetect_shift: the autodetect_shift the reference derives from the data rate
+ * (:900-934).
+ * fsk_b200_engine_set_auto_carrier: enables the calls below; threshold 0.001 is the CLI's -a, inverted its
+ * --inverted.  The band shift is b_shift = (int)(-(float)(autodetect_shift + band_width/2) / band_width),
+ * negated when inverted.  -EINVAL (and the calls below disabled) for a threshold that is not positive
+ * and finite, for b_shift == 0 (the reference asserts there, src/fsk.c:587), and for a scan window
+ * min(nsamples_per_bit, fftsize) under one sample, i.e. a data rate above the sample rate (the
+ * reference's scan never advances there).
+ * fsk_b200_rx_batch_auto / _s16: fsk_b200_rx_batch / _s16 with the scan; auto_states (device, one per
+ * stream) as above; rec_band (device, optional, [nstreams][max_frames]) receives the mark band of every
+ * record, the band of the session that ended for a REPORT record.  -ENOTSUP, with nothing launched, where
+ * the per-candidate rx kernel cannot take the mode (e.g. 0.5 baud).
+ * fsk_b200_auto_stream_window: the holdback for live streams with auto-carrier, max(stream window,
+ * samplebuf_size): with it the records do not depend on how a stream is cut into chunks. */
+typedef struct fsk_b200_auto_state {
+    uint32_t	carrier_band;	/* accepted mark band; 0 = none (bands start at 1) */
+    uint32_t	v;		/* virtual ring count: the samples from pos on the reference's ring would hold */
+    uint32_t	reserved[2];
+} fsk_b200_auto_state;
+int fsk_b200_rx_config_autodetect_shift(const fsk_b200_rx_config *cfg);
+int fsk_b200_engine_set_auto_carrier(fsk_b200_engine *e, float threshold, int autodetect_shift, int inverted);
+int fsk_b200_rx_batch_auto(fsk_b200_engine *e, const float *samples, size_t nstreams,
+	size_t stride, const uint32_t *nsamples, uint32_t nsamples_all,
+	fsk_b200_frame *frames, uint32_t max_frames, fsk_b200_stream_state *states,
+	fsk_b200_auto_state *auto_states, uint32_t *rec_band, void *stream);
+int fsk_b200_rx_batch_auto_s16(fsk_b200_engine *e, const int16_t *samples, size_t nstreams,
+	size_t stride, const uint32_t *nsamples, uint32_t nsamples_all,
+	fsk_b200_frame *frames, uint32_t max_frames, fsk_b200_stream_state *states,
+	fsk_b200_auto_state *auto_states, uint32_t *rec_band, void *stream);
+uint32_t fsk_b200_auto_stream_window(const fsk_b200_rx_params *p);
+
 /* N2 -- 16-bit PCM ingest (the reference transmitter's default sample format, read back by
  * its rx as float = short / 32768: src/simpleaudio-sndfile.c:43-57, src/minimodem.c:786-788).
  * fsk_b200_s16_to_f32: device conversion (exact: a power-of-two scale), asynchronous on `stream`.

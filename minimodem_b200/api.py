@@ -96,6 +96,7 @@ class TxState(C.Structure):
 
 
 TX_STATE_BYTES = 16
+AUTO_STATE_BYTES = 16           # fsk_b200_auto_state
 TX_IDLE_IF_EMPTY, TX_FINAL = 1, 2
 ENCODE_ASCII8, ENCODE_BAUDOT = 0, 1
 
@@ -122,6 +123,8 @@ EXPORTS = [
     "fsk_b200_version", "fsk_b200_launch_count", "fsk_b200_last_error", "fsk_b200_engine_last_kernel",
     "fsk_b200_encoder_for_mode", "fsk_b200_tx_config_from_rx", "fsk_b200_tx_engine_new", "fsk_b200_tx_engine_destroy",
     "fsk_b200_tx_max_samples", "fsk_b200_tx_text_batch",
+    "fsk_b200_rx_config_autodetect_shift", "fsk_b200_engine_set_auto_carrier", "fsk_b200_rx_batch_auto",
+    "fsk_b200_rx_batch_auto_s16", "fsk_b200_auto_stream_window",
 ]
 
 _lib = None
@@ -247,6 +250,16 @@ def lib():
     L.fsk_b200_tx_text_batch.restype = C.c_int
     L.fsk_b200_sin_table.argtypes = [C.POINTER(C.c_float), C.c_uint, C.c_float]
     L.fsk_b200_sin_table.restype = None
+    L.fsk_b200_rx_config_autodetect_shift.argtypes = [C.POINTER(RxConfig)]
+    L.fsk_b200_rx_config_autodetect_shift.restype = C.c_int
+    L.fsk_b200_engine_set_auto_carrier.argtypes = [C.c_void_p, C.c_float, C.c_int, C.c_int]
+    L.fsk_b200_engine_set_auto_carrier.restype = C.c_int
+    L.fsk_b200_rx_batch_auto.argtypes = L.fsk_b200_rx_batch.argtypes + [C.c_void_p, C.c_void_p]
+    L.fsk_b200_rx_batch_auto.restype = C.c_int
+    L.fsk_b200_rx_batch_auto_s16.argtypes = list(L.fsk_b200_rx_batch_auto.argtypes)
+    L.fsk_b200_rx_batch_auto_s16.restype = C.c_int
+    L.fsk_b200_auto_stream_window.argtypes = [C.POINTER(RxParams)]
+    L.fsk_b200_auto_stream_window.restype = C.c_uint32
     L.fsk_b200_version.restype = C.c_char_p
     L.fsk_b200_launch_count.restype = C.c_ulonglong
     L.fsk_b200_last_error.restype = C.c_char_p
@@ -377,15 +390,17 @@ class FskPlan:
 class RxEngine:
     """Batched engine over device-resident streams (Part 2 of include/fsk_b200.h)."""
 
-    def __init__(self, params):
+    def __init__(self, params, autodetect_shift=None):
         self.params = params
+        self._autodetect_shift = autodetect_shift
         self._e = lib().fsk_b200_engine_new(C.byref(params))
         if not self._e:
             _err("fsk_b200_engine_new")
 
     @classmethod
     def for_mode(cls, baudmode, sample_rate=48000, **overrides):
-        return cls(rx_params(rx_config_for_mode(baudmode, sample_rate, **overrides)))
+        cfg = rx_config_for_mode(baudmode, sample_rate, **overrides)
+        return cls(rx_params(cfg), lib().fsk_b200_rx_config_autodetect_shift(C.byref(cfg)))
 
     def tune(self, lanes_per_stream=0, warps_per_block=0, ring_floats=0):
         rc = lib().fsk_b200_engine_tune(self._e, lanes_per_stream, warps_per_block, ring_floats)
@@ -509,6 +524,56 @@ class RxEngine:
     def stream_window(self):
         """fsk_b200_stream_window: the farthest sample a search can touch from its start."""
         return int(lib().fsk_b200_stream_window(C.byref(self.params)))
+
+    def set_auto_carrier(self, threshold=0.001, autodetect_shift=None, inverted=False):
+        """fsk_b200_engine_set_auto_carrier: the reference's --auto-carrier (-a is threshold 0.001) for
+        rx_batch_auto.  autodetect_shift defaults to the one the reference derives from this engine's
+        data rate (fsk_b200_rx_config_autodetect_shift); inverted is the CLI's --inverted."""
+        if autodetect_shift is None:
+            autodetect_shift = self._autodetect_shift
+        if autodetect_shift is None:
+            raise ValueError("set_auto_carrier: pass autodetect_shift (fsk_b200_rx_config_autodetect_shift)")
+        rc = lib().fsk_b200_engine_set_auto_carrier(self._e, float(threshold), int(autodetect_shift), int(inverted))
+        if rc:
+            _err("fsk_b200_engine_set_auto_carrier", rc)
+
+    def rx_batch_auto(self, samples, nsamples=None, max_frames=None, frames=None, states=None,
+                      auto_states=None, rec_band=False, nsamples_each=None, stream=None):
+        """rx_batch with --auto-carrier (set_auto_carrier first): every stream finds its own tone pair.
+        samples: [nstreams, stride] float32 or int16 CUDA tensor.  auto_states: uint8 CUDA tensor
+        [nstreams, AUTO_STATE_BYTES], zeros for fresh streams, carried with `states` to continue them.
+        Returns (frames, states, auto_states), and with rec_band=True (or a [nstreams, max_frames] int32
+        CUDA tensor) also the mark band of every record."""
+        torch = _torch()
+        assert samples.is_cuda and samples.dtype in (torch.float32, torch.int16) and samples.is_contiguous()
+        nstreams, stride = samples.shape
+        n_all = int(nsamples if nsamples is not None else stride)
+        if max_frames is None:
+            max_frames = self.max_frames(n_all)
+        if frames is None:
+            frames = torch.empty((nstreams, max_frames, 5), dtype=torch.int32, device=samples.device)
+        if states is None:
+            states = torch.zeros((nstreams, STATE_WORDS), dtype=torch.int32, device=samples.device)
+        if auto_states is None:
+            auto_states = torch.zeros((nstreams, AUTO_STATE_BYTES), dtype=torch.uint8, device=samples.device)
+        assert auto_states.dtype == torch.uint8 and tuple(auto_states.shape) == (nstreams, AUTO_STATE_BYTES)
+        bands = None
+        if rec_band is True:
+            bands = torch.zeros((nstreams, max_frames), dtype=torch.int32, device=samples.device)
+        elif rec_band is not False and rec_band is not None:
+            bands = rec_band
+        fn = lib().fsk_b200_rx_batch_auto if samples.dtype == torch.float32 else lib().fsk_b200_rx_batch_auto_s16
+        rc = fn(self._e, _ptr(samples), nstreams, stride, _ptr(nsamples_each), n_all, _ptr(frames), max_frames,
+                _ptr(states), _ptr(auto_states), _ptr(bands), _stream_handle(stream))
+        if rc:
+            _err("fsk_b200_rx_batch_auto", rc)
+        if bands is None:
+            return frames, states, auto_states
+        return frames, states, auto_states, bands
+
+    def auto_stream_window(self):
+        """fsk_b200_auto_stream_window: the live-stream holdback with auto-carrier."""
+        return int(lib().fsk_b200_auto_stream_window(C.byref(self.params)))
 
     def set_holdback(self, nsamples):
         """fsk_b200_engine_set_holdback: searches start only with this many samples left (0 = the

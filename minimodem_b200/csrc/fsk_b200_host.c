@@ -512,6 +512,8 @@ struct fsk_b200_engine {
     fsk_b200_geom geom;
     fsk_b200_loopc loopc;
     void *ce;			/* CUDA-side state */
+    fsk_b200_auto_args autoc;	/* --auto-carrier (fsk_b200_engine_set_auto_carrier) */
+    int auto_on;
 };
 
 fsk_b200_engine *fsk_b200_engine_new(const fsk_b200_rx_params *params)
@@ -691,6 +693,131 @@ int fsk_b200_rx_batch_s16(fsk_b200_engine *e, const int16_t *samples, size_t nst
 	fsk_b200_set_error("rx_batch_s16: this mode's launch shape has no int16 build; widen with fsk_b200_s16_to_f32 "
 		"and call fsk_b200_rx_batch (fsk_b200_rx_batch_host_s16 does that by itself)");
     return rc;
+}
+
+/* ---- --auto-carrier ------------------------------------------------------------ */
+
+int fsk_b200_rx_config_autodetect_shift(const fsk_b200_rx_config *cfg)
+{
+    if (!cfg)
+	return 0;
+    if (cfg->data_rate >= 400)				/* src/minimodem.c:900-910 */
+	return -(cfg->data_rate * 5 / 6);
+    if (cfg->data_rate >= 100)				/* :911-921 */
+	return 200;
+    return 170;						/* :922-934 */
+}
+
+/* samplebuf_size of src/minimodem.c:1056-1069 */
+static size_t auto_samplebuf_size(const fsk_b200_rx_params *p)
+{
+    const unsigned int sample_rate = (unsigned int)p->sample_rate;
+    const unsigned nbits = 1 + p->nstartbits + p->n_data_bits + 1;
+    size_t sz = ceilf(p->nsamples_per_bit) * (nbits + 1);
+    sz *= 2;
+    if (sz < sample_rate / 12)
+	sz = sample_rate / 12;
+    return sz;
+}
+
+uint32_t fsk_b200_auto_stream_window(const fsk_b200_rx_params *p)
+{
+    if (!p)
+	return 0u;
+    const uint32_t w = fsk_b200_stream_window(p);
+    const size_t sb = auto_samplebuf_size(p);
+    return sb > w ? (uint32_t)sb : w;
+}
+
+int fsk_b200_engine_set_auto_carrier(fsk_b200_engine *e, float threshold, int autodetect_shift, int inverted)
+{
+    if (!e) {
+	fsk_b200_set_error("set_auto_carrier: NULL engine");
+	return -EINVAL;
+    }
+    e->auto_on = 0;
+    if (!(threshold > 0.0f) || !isfinite(threshold)) {
+	fsk_b200_set_error("set_auto_carrier: the threshold must be positive and finite");
+	return -EINVAL;
+    }
+    const fsk_b200_rx_params *p = &e->params;
+    int b_shift = -(float)(autodetect_shift + p->band_width / 2.0f) / p->band_width;	/* :1200-1203 */
+    if (inverted)
+	b_shift *= -1;
+    if (b_shift == 0) {
+	fsk_b200_set_error("set_auto_carrier: band shift 0 (autodetect_shift %d, band width %g)", autodetect_shift,
+		(double)p->band_width);
+	return -EINVAL;
+    }
+    int rc = fsk_b200_cuda_set_unit_table(e->ce, p->fftsize);
+    if (rc)
+	return rc;
+    float scan_n = p->nsamples_per_bit;			/* :1183-1185 */
+    if (scan_n > p->fftsize)
+	scan_n = p->fftsize;
+    /* The scan steps i = (unsigned)(i + scan_n) while i + scan_n <= the ring count, in float.  A window
+     * under one sample (data rate above the sample rate) never moves i: the reference spins there for
+     * ever.  And the step must stay exact in float, which holds while the ring count is below 2^24. */
+    const size_t half_ring = auto_samplebuf_size(p) / 2;
+    if (!(scan_n >= 1.0f) || half_ring >= (1u << 24)) {
+	fsk_b200_set_error("set_auto_carrier: scan window of %g samples (data rate above the sample rate), or a sample "
+		"ring of %zu", (double)scan_n, 2 * half_ring);
+	return -EINVAL;
+    }
+    e->autoc.threshold = threshold;
+    e->autoc.scan_n = scan_n;
+    e->autoc.b_shift = b_shift;
+    e->autoc.fftsize = p->fftsize;
+    e->autoc.nbands = p->nbands;
+    e->autoc.half_ring = (unsigned)half_ring;
+    e->autoc.expect_nsamples = p->expect_nsamples;
+    e->auto_on = 1;
+    return 0;
+}
+
+static int rx_batch_auto_any(fsk_b200_engine *e, const void *samples, int elem, size_t nstreams, size_t stride,
+	const uint32_t *nsamples, uint32_t nsamples_all, fsk_b200_frame *frames, uint32_t max_frames,
+	fsk_b200_stream_state *states, fsk_b200_auto_state *auto_states, uint32_t *rec_band, void *stream)
+{
+    if (!e || !e->auto_on) {
+	fsk_b200_set_error("rx_batch_auto: call fsk_b200_engine_set_auto_carrier first");
+	return -EINVAL;
+    }
+    if (nstreams == 0)
+	return 0;
+    const size_t align = elem == 2 ? 7 : 3;
+    if (!samples || ((uintptr_t)samples & 15) || (stride & align)) {
+	fsk_b200_set_error("rx_batch_auto: samples must be 16-byte aligned and the stride a multiple of %zu samples",
+		align + 1);
+	return -EINVAL;
+    }
+    if (!frames || !states || !auto_states || max_frames == 0) {
+	fsk_b200_set_error("rx_batch_auto: NULL argument");
+	return -EINVAL;
+    }
+    if ((!nsamples && (size_t)nsamples_all > stride) || nstreams > 0x7fffffffu) {
+	fsk_b200_set_error("rx_batch_auto: nsamples_all (%u) exceeds the row stride (%zu), or too many streams",
+		nsamples_all, stride);
+	return -EINVAL;
+    }
+    return fsk_b200_cuda_rx_batch_auto(e->ce, &e->geom, &e->loopc, &e->autoc, samples, elem, nstreams, stride,
+	    nsamples, nsamples_all, frames, max_frames, states, auto_states, rec_band, stream);
+}
+
+int fsk_b200_rx_batch_auto(fsk_b200_engine *e, const float *samples, size_t nstreams, size_t stride,
+	const uint32_t *nsamples, uint32_t nsamples_all, fsk_b200_frame *frames, uint32_t max_frames,
+	fsk_b200_stream_state *states, fsk_b200_auto_state *auto_states, uint32_t *rec_band, void *stream)
+{
+    return rx_batch_auto_any(e, samples, 4, nstreams, stride, nsamples, nsamples_all, frames, max_frames, states,
+	    auto_states, rec_band, stream);
+}
+
+int fsk_b200_rx_batch_auto_s16(fsk_b200_engine *e, const int16_t *samples, size_t nstreams, size_t stride,
+	const uint32_t *nsamples, uint32_t nsamples_all, fsk_b200_frame *frames, uint32_t max_frames,
+	fsk_b200_stream_state *states, fsk_b200_auto_state *auto_states, uint32_t *rec_band, void *stream)
+{
+    return rx_batch_auto_any(e, samples, 2, nstreams, stride, nsamples, nsamples_all, frames, max_frames, states,
+	    auto_states, rec_band, stream);
 }
 
 /* ---- live streams ------------------------------------------------------------ */

@@ -184,6 +184,22 @@ int  fsk_b200_cuda_band_mags(void *ce, int fftsize, const float *host_samples,
 	unsigned int nsamples, unsigned int nbands, float *host_mags);
 int  fsk_b200_cuda_detect_carrier_batch(int fftsize, const float *samples, size_t nstreams, size_t stride,
 	const uint32_t *offset, uint32_t nsamples, float min_mag_threshold, int32_t *out_band, void *stream);
+
+/* --auto-carrier constants of an engine (fsk_b200_engine_set_auto_carrier) */
+typedef struct fsk_b200_auto_args {
+    float	threshold;		/* carrier_autodetect_threshold, > 0 */
+    float	scan_n;			/* min(nsamples_per_bit, fftsize), src/minimodem.c:1183-1185 */
+    int		b_shift;		/* :1200-1203 */
+    int		fftsize;
+    unsigned int nbands;
+    unsigned int half_ring;		/* samplebuf_size / 2 */
+    unsigned int expect_nsamples;	/* the loop's own stop rule (:1229), below any holdback */
+} fsk_b200_auto_args;
+int  fsk_b200_cuda_set_unit_table(void *ce, int fftsize);
+int  fsk_b200_cuda_rx_batch_auto(void *ce, const fsk_b200_geom *g, const fsk_b200_loopc *lc,
+	const fsk_b200_auto_args *aa, const void *samples, int elem, size_t nstreams, size_t stride,
+	const uint32_t *nsamples, uint32_t nsamples_all, fsk_b200_frame *frames, uint32_t max_frames,
+	fsk_b200_stream_state *states, fsk_b200_auto_state *auto_states, uint32_t *rec_band, void *stream);
 int  fsk_b200_cuda_stream_push(float *samples, size_t nstreams, size_t stride, uint32_t *fill,
 	fsk_b200_stream_state *states, const float *chunk, size_t chunk_stride, const uint32_t *chunk_len,
 	uint32_t chunk_len_all, uint32_t *dropped, void *stream);

@@ -154,6 +154,76 @@ struct RxArgs {
     fsk_b200_stream_state *states;
 };
 
+__device__ __forceinline__ float sample_at(const float *__restrict__ x, unsigned n) { return x[n]; }
+/* int16 PCM rows: the reference's float = short / 32768 (exact) */
+__device__ __forceinline__ float sample_at(const int16_t *__restrict__ x, unsigned n)
+{
+    return (float)x[n] * (1.0f / 32768.0f);
+}
+
+/* magnitude of band k over the first nsamples of x, zero-padded to fftsize (src/fsk.c:549-553) */
+template <class T>
+__device__ __forceinline__ float band_mag(const T *__restrict__ x, unsigned nsamples, unsigned F, unsigned k)
+{
+    double re = 0., im = 0.;
+    unsigned r = 0;				/* (k*n) mod F, kept exact in integers */
+    for (unsigned n = 0; n < nsamples; n++) {
+	float sn, cs;
+	sincospif(2.0f * (float)r / (float)F, &sn, &cs);
+	const float xn = sample_at(x, n);
+	re += (double)(xn * cs);
+	im += (double)(xn * sn);
+	r += k;
+	if (r >= F)
+	    r -= F;
+    }
+    const float magscalar = 1.0f / ((float)nsamples / 2.0f);	/* src/fsk.c:553 */
+    const float fr = (float)re, fi = (float)im;
+    return sqrtf(fr * fr + fi * fi) * magscalar;
+}
+
+/* --auto-carrier (src/minimodem.c:1179-1220) in the per-candidate rx kernel (AUTO = 1) */
+struct AutoArgs {
+    fsk_b200_auto_state *states;
+    uint32_t *rec_band;		/* optional: [nstreams][max_frames], the mark band of every record */
+    const float2 *unit;		/* (cos, -sin)(2 pi r / fftsize), r = 0 .. fftsize-1, as fsk_b200_cuda_set_table rounds them */
+    float threshold;		/* carrier_autodetect_threshold */
+    float scan_n;		/* nsamples_per_scan = min(nsamples_per_bit, fftsize), a float as in the reference */
+    int b_shift;		/* :1200-1203, negated under --inverted */
+    unsigned fftsize, nbands;
+    unsigned half_ring;		/* samplebuf_size / 2: the refill of the virtual ring count */
+    unsigned expect_nsamples;	/* the loop's own stop rule; lc.expect_nsamples above it is a live stream's holdback */
+};
+
+/* fsk_detect_carrier (src/fsk.c:543-581) on one window, by the G lanes of a group: lane g takes the
+ * bands 1 + g, 1 + g + G, ...; the rule of k_detect_carrier picks the first strictly largest
+ * magnitude at or above the threshold.  Returns the band or -1. */
+template <int G, class T>
+__device__ __forceinline__ int detect_group(const T *__restrict__ x, unsigned nsamples, const AutoArgs &au,
+	unsigned g, unsigned gmask)
+{
+    float max_mag = 0.0f;
+    int best = -1;
+    for (unsigned k = 1 + g; k < au.nbands; k += G) {
+	const float m = band_mag(x, nsamples, au.fftsize, k);
+	if (m < au.threshold)
+	    continue;
+	if (max_mag < m) {
+	    max_mag = m;
+	    best = (int)k;
+	}
+    }
+    for (int o = G / 2; o; o >>= 1) {
+	const float om = __shfl_xor_sync(gmask, max_mag, o);
+	const int ob = __shfl_xor_sync(gmask, best, o);
+	if (ob >= 0 && (best < 0 || max_mag < om || (max_mag == om && ob < best))) {
+	    max_mag = om;
+	    best = ob;
+	}
+    }
+    return best;
+}
+
 /* ------------------------------------------------------------------------ */
 /* K1: batched fsk_find_frame (src/fsk.c:449-538), one search per stream     */
 /* ------------------------------------------------------------------------ */
@@ -255,15 +325,20 @@ k_find_frame(const __grid_constant__ fsk_b200_geom geo, const float4 *__restrict
 #define FSK_PFX_MAXTHREADS 512
 #endif
 /* SRC 0: float32 rows; SRC 1: int16 PCM rows (N2, src/simpleaudio-sndfile.c:43-57), widened to the
- * reference's float = short / 32768 inside the ring fill: 2 bytes per sample of HBM traffic */
-template <int G, int W, int L, int MODE, int FILL, int SRC = 0>
+ * reference's float = short / 32768 inside the ring fill: 2 bytes per sample of HBM traffic.
+ * AUTO 1 (MODE 0, FILL 0 only): --auto-carrier.  Each stream has its own tone table in shared memory
+ * behind the mbarriers (geo.tw_entries float4 per slot, filled from au.unit when a band is accepted),
+ * and scans for a carrier band over its virtual ring count while it has none (DESIGN.md 5). */
+template <int G, int W, int L, int MODE, int FILL, int SRC = 0, int AUTO = 0>
 __global__ void __launch_bounds__(MODE == 3 ? FSK_PFX_MAXTHREADS : FSK_MAXTHREADS,
 	MODE == 3 ? 1 : (MODE == 2 && G >= 16) ? 3 : FSK_MINBLOCKS)
 k_rx(const __grid_constant__ fsk_b200_geom geo, const __grid_constant__ fsk_b200_loopc lc,
 	const float4 *__restrict__ tw_global, unsigned tw_in_smem, unsigned ring_floats,
 	unsigned lookahead, const __grid_constant__ RxArgs a, const __grid_constant__ fsk_b200_mplan mp,
-	const float4 *__restrict__ tw_sample, const __grid_constant__ fsk_b200_pfx pg)
+	const float4 *__restrict__ tw_sample, const __grid_constant__ fsk_b200_pfx pg,
+	const __grid_constant__ AutoArgs au)
 {
+    static_assert(!AUTO || (MODE == 0 && FILL == 0), "auto-carrier: per-candidate kernel, cp.async fill");
     FSK_DYN_SMEM(smem4);
     /* MODE 3 (chunk-prefix table): the ring's mirror covers one lane-run of the table build (not a bit window);
      * the staged table (tw_global) is the chunk-rotation table, the per-sample one stays in global memory
@@ -274,7 +349,10 @@ k_rx(const __grid_constant__ fsk_b200_geom geo, const __grid_constant__ fsk_b200
 	    &pg.loc[0][0][0], (MODE == 3 && LB == 0) ? 32u : 0u);
     GROUP_VARS;
     const Ring rg = { smem_u32(sm.ring), ring_floats, ring_pad };
-    const unsigned tw_s = tw_in_smem ? smem_u32(sm.tw) : 0u;	/* the fast path requires the table in shared memory */
+    /* the fast path requires the table in shared memory; AUTO: this slot's own table */
+    float4 *const tw_auto = AUTO ? reinterpret_cast<float4 *>(sm.bars - 2u * (warp * spw + sidx) + 2u * wpb * spw)
+	    + (size_t)(warp * spw + sidx) * geo.tw_entries : nullptr;
+    const unsigned tw_s = AUTO ? smem_u32(tw_auto) : tw_in_smem ? smem_u32(sm.tw) : 0u;
     /* MODE 2 (shared-segment search) owns CONSECUTIVE bit periods per lane, MODE 0 interleaved windows */
     const LaneWin<W> lw = lane_windows<G, W, L>(geo, g);
     const LaneWinM<W> lwm = lane_windows_multi<G, W, L>(geo, g);
@@ -305,6 +383,22 @@ k_rx(const __grid_constant__ fsk_b200_geom geo, const __grid_constant__ fsk_b200
 	unsigned done = 0;
 	unsigned ncand = 0, nsearch = 0;	/* statistics: candidates analysed, searches run */
 	bool mhint = st.reserved != 0u;		/* MODE 2: the latest coarse search needed more than its first candidate */
+	/* AUTO: the accepted mark band (0: none, :1180) and the virtual ring count */
+	unsigned band = AUTO ? au.states[s].carrier_band : 0u, vring = AUTO ? au.states[s].v : 0u;
+	/* fsk_set_tones_by_bandshift (src/fsk.c:585-598) for this stream's table: entry e of the tone b is
+	 * the unit-circle entry (b * e) mod fftsize, the value fsk_b200_cuda_set_table computes for it */
+	auto set_tones = [&](unsigned bm) {
+	    const unsigned bsp = (unsigned)((int)bm + au.b_shift);
+	    __syncwarp(gmask);
+	    for (unsigned e = g; e < geo.tw_entries; e += G) {
+		const float2 um = au.unit[(unsigned)(((unsigned long long)bm * e) % au.fftsize)];
+		const float2 us = au.unit[(unsigned)(((unsigned long long)bsp * e) % au.fftsize)];
+		tw_auto[e] = make_float4(um.x, um.y, us.x, us.y);
+	    }
+	    __syncwarp(gmask);
+	};
+	if (AUTO && band)
+	    set_tones(band);
 
 	/* ring bookkeeping (MODE 0): ring offset of `pos`, and the absolute index up to
 	 * which the ring content has been REQUESTED (copies issued or zeros stored) */
@@ -422,6 +516,49 @@ k_rx(const __grid_constant__ fsk_b200_geom geo, const __grid_constant__ fsk_b200
 	for (;;) {
 	    if (pos >= n) { done = 1; break; }			/* :1176 */
 	    const unsigned remaining = n - pos;
+	    if (AUTO) {
+		/* a live stream's holdback (lc.expect_nsamples raised above the loop's own rule) stops the
+		 * loop before the scan: the refill below must not see where the stream was cut */
+		if (lc.expect_nsamples > au.expect_nsamples && remaining < lc.expect_nsamples) { done = 1; break; }
+		if (vring > remaining)				/* (a state that does not fit this row) */
+		    vring = remaining;
+		if (vring < au.half_ring)			/* :1158-1174, the refill */
+		    vring += min(remaining - vring, au.half_ring);
+		if (band == 0) {				/* :1181-1220 */
+		    const float sf = au.scan_n;
+		    const unsigned sn = (unsigned)sf;
+		    unsigned i = 0;
+		    int found = -1;
+		    for (; (float)i + sf <= (float)vring; i = (unsigned)((float)i + sf)) {
+			if (SRC)
+			    found = detect_group<G>(x16 + pos + i, sn, au, g, gmask);
+			else
+			    found = detect_group<G>(x + pos + i, sn, au, g, gmask);
+			if (found >= 0)
+			    break;
+		    }
+		    const int b_space = found + au.b_shift;
+		    if (found >= 0 && b_space >= 1 && b_space < (int)au.nbands) {
+			band = (unsigned)found;
+			set_tones(band);			/* and search at the ring start */
+		    } else {
+			const unsigned adv = min((unsigned)((float)i + sf), vring);
+			pos += adv;
+			vring -= adv;
+			/* restart the ring at the new position, as a resumed stream starts it */
+			drain();
+			filled = pos & ~AL;
+			landed = filled;
+			pos_off = pos & AL;
+			fdst = dst0;
+			fsrc = SRC ? x : x + filled + 4u * g;
+			conv = filled;
+			coff = 0;
+			__syncwarp(gmask);
+			continue;
+		    }
+		}
+	    }
 	    if (remaining < lc.expect_nsamples) { done = 1; break; }	/* :1229 */
 	    if (nframes >= a.max_frames)
 		break;						/* output full: resumable */
@@ -623,6 +760,8 @@ k_rx(const __grid_constant__ fsk_b200_geom geo, const __grid_constant__ fsk_b200
 			if (g == 0)
 			    store_frame(out + nframes, carrier_nsamples, confidence_total,
 				    amplitude_total, FSK_B200_FRAME_REPORT);
+			if (AUTO && g == 0 && au.rec_band)
+			    au.rec_band[(size_t)s * a.max_frames + nframes] = band;
 			nframes++;
 			carrier = 0;				/* :1303-1308 */
 			carrier_nsamples = 0;
@@ -631,6 +770,8 @@ k_rx(const __grid_constant__ fsk_b200_geom geo, const __grid_constant__ fsk_b200
 			nframes_decoded = 0;
 			track_amplitude = 0.f;
 		    }
+		    if (AUTO)
+			band = 0;				/* :1297 */
 		}
 		advance = try_max;				/* :1318 */
 	    } else {
@@ -680,11 +821,15 @@ k_rx(const __grid_constant__ fsk_b200_geom geo, const __grid_constant__ fsk_b200
 		noconfidence = 0;
 		if (g == 0)
 		    store_frame(out + nframes, bits, confidence, amplitude, frame_start | acquired);
+		if (AUTO && g == 0 && au.rec_band)
+		    au.rec_band[(size_t)s * a.max_frames + nframes] = band;
 		nframes++;
 		advance = frame_start + lc.frame_nsamples - lc.nsamples_overscan;	/* :1407 */
 	    }
 	    if (advance > remaining) { done = 1; break; }	/* :1151 */
 	    pos += advance;
+	    if (AUTO)
+		vring = advance >= vring ? 0u : vring - advance;
 	    if (MODE != 1) {
 		pos_off = ring_wrap(pos_off + advance, R);	/* advance < R by construction */
 		if (filled < (pos & ~AL)) {
@@ -720,6 +865,10 @@ k_rx(const __grid_constant__ fsk_b200_geom geo, const __grid_constant__ fsk_b200
 	    st.stat_searches += nsearch;
 	    st.reserved = mhint ? 1u : 0u;
 	    a.states[s] = st;
+	    if (AUTO) {
+		au.states[s].carrier_band = band;
+		au.states[s].v = vring;
+	    }
 	}
 	__syncwarp(gmask);
     }
@@ -941,25 +1090,6 @@ k_rx_ws(const __grid_constant__ fsk_b200_geom geo, const __grid_constant__ fsk_b
 /* ------------------------------------------------------------------------ */
 /* full-spectrum magnitudes for fsk_detect_carrier (src/fsk.c:543-581)      */
 /* ------------------------------------------------------------------------ */
-
-/* magnitude of band k over the first nsamples of x, zero-padded to fftsize (src/fsk.c:549-553) */
-__device__ __forceinline__ float band_mag(const float *__restrict__ x, unsigned nsamples, unsigned F, unsigned k)
-{
-    double re = 0., im = 0.;
-    unsigned r = 0;				/* (k*n) mod F, kept exact in integers */
-    for (unsigned n = 0; n < nsamples; n++) {
-	float sn, cs;
-	sincospif(2.0f * (float)r / (float)F, &sn, &cs);
-	re += (double)(x[n] * cs);
-	im += (double)(x[n] * sn);
-	r += k;
-	if (r >= F)
-	    r -= F;
-    }
-    const float magscalar = 1.0f / ((float)nsamples / 2.0f);	/* src/fsk.c:553 */
-    const float fr = (float)re, fi = (float)im;
-    return sqrtf(fr * fr + fi * fi) * magscalar;
-}
 
 __global__ void k_band_mags(const float *__restrict__ x, unsigned nsamples, int fftsize,
 	unsigned nbands, float *__restrict__ mags)
@@ -1494,6 +1624,8 @@ struct CudaEngine {
     size_t slab_streams, slab_stride, slab_max_frames;
     size_t slab_bytes;			/* host-buffer path: sample bytes per slab (FSK_B200_SLAB_BYTES) */
     cudaStream_t st[2];
+    float2 *d_unit;			/* --auto-carrier: unit-circle table of unit_f entries (AutoArgs.unit) */
+    int unit_f;
 };
 
 extern "C" unsigned long long fsk_b200_cuda_launch_count(void) { return g_launches; }
@@ -1570,6 +1702,7 @@ extern "C" void fsk_b200_cuda_engine_destroy(void *p)
 	return;
     cudaFree(ce->d_tw);
     cudaFree(ce->d_twc);
+    cudaFree(ce->d_unit);
     cudaFree(ce->d_one);
     cudaFree(ce->d_args);
     cudaFree(ce->d_frame);
@@ -1801,17 +1934,20 @@ static bool split_for(int G, unsigned n_bits, int force_L, int *W, int *L)
     return best > 0.0;
 }
 
+/* per_stream_tw (--auto-carrier): the per-candidate kernel only, with a tone table per stream instead of
+ * one per block */
 static int pick_shape(const CudaEngine *ce, const fsk_b200_geom *g, unsigned need_floats,
-	unsigned max_advance, size_t nstreams, Shape *sh, const fsk_b200_loopc *lc = NULL)
+	unsigned max_advance, size_t nstreams, Shape *sh, const fsk_b200_loopc *lc = NULL, bool per_stream_tw = false)
 {
     sh->geo = *g;
     memset(&sh->mplan, 0, sizeof(sh->mplan));
     const size_t smem_max = (size_t)ce->smem_optin;
     const size_t tw_bytes = (size_t)g->bit_nsamples * sizeof(float4);	/* the sliding search's extension is added at the end */
     sh->tw_in_smem = tw_bytes <= 24 * 1024;
-    const size_t fixed = sh->tw_in_smem ? tw_bytes : 0;
+    const size_t fixed = sh->tw_in_smem && !per_stream_tw ? tw_bytes : 0;
     const size_t pad_bytes = (size_t)((g->bit_nsamples + 3u) & ~3u) * 4;
-    const size_t scr_bytes = (size_t)g->n_bits * sizeof(float2) + pad_bytes + 16;	/* per stream, besides the ring: scratch, mirror, 2 mbarriers */
+    /* per stream, besides the ring: scratch, mirror, 2 mbarriers (and its tone table) */
+    const size_t scr_bytes = (size_t)g->n_bits * sizeof(float2) + pad_bytes + 16 + (per_stream_tw ? tw_bytes : 0);
 
     /* ring: the widest search window plus (ideally) one full advance of look-ahead */
     /* whole blocks; room for the widest window starting anywhere inside a block */
@@ -1884,7 +2020,7 @@ static int pick_shape(const CudaEngine *ce, const fsk_b200_geom *g, unsigned nee
 	}
     }
     sh->mode = fast ? 0 : 1;
-    if (fast && lc && ce->multi && ce->fill == 0 && (ce->multi > 0 || g->bit_nsamples >= FSK_MULTI_MIN_N)) {
+    if (fast && lc && !per_stream_tw && ce->multi && ce->fill == 0 && (ce->multi > 0 || g->bit_nsamples >= FSK_MULTI_MIN_N)) {
 	/* the rx loop's searches from shared segment sums, if this mode's windows tile and all of its
 	 * searches fit the period slots of a (W, L) split of this group size */
 	int W2 = 0, L2 = 0;
@@ -1897,7 +2033,7 @@ static int pick_shape(const CudaEngine *ce, const fsk_b200_geom *g, unsigned nee
 	}
     }
     memset(&sh->pfx, 0, sizeof(sh->pfx));
-    if (lc && ce->prefix && ce->fill == 0 && ce->twc_n && ring_min >= 128u
+    if (lc && !per_stream_tw && ce->prefix && ce->fill == 0 && ce->twc_n && ring_min >= 128u
 	    && (ce->prefix > 0 || g->bit_nsamples >= FSK_PREFIX_MIN_N)) {
 	/* the rx loop's searches from a chunk-prefix table (mode 3): one stream per warp, one lane per
 	 * window boundary of a candidate, the ring without its mirror plus the table per stream */
@@ -2005,7 +2141,8 @@ static int pick_shape(const CudaEngine *ce, const fsk_b200_geom *g, unsigned nee
     sh->geo.tw_entries = sh->mode == 3 ? sh->pfx_tw_stage : g->bit_nsamples;
     sh->slide = 0;
     if (sh->mode == 0 && lc && lc->slide && g->tw_entries > g->bit_nsamples && sh->tw_in_smem) {
-	const size_t extra = (size_t)(g->tw_entries - g->bit_nsamples) * sizeof(float4);
+	const size_t extra = (size_t)(g->tw_entries - g->bit_nsamples) * sizeof(float4)
+	    * (per_stream_tw ? (size_t)wpb * (32 / G) : 1u);
 	if (sh->smem + extra <= smem_max) {
 	    sh->smem += extra;
 	    sh->geo.tw_entries = g->tw_entries;
@@ -2097,16 +2234,18 @@ static cudaError_t launch_rx_ws_t(const Shape &sh, const CudaEngine *ce, const f
     return cudaGetLastError();
 }
 
-template <int G, int W, int L, int MODE, int FILL, int SRC = 0>
+template <int G, int W, int L, int MODE, int FILL, int SRC = 0, int AUTO = 0>
 static cudaError_t launch_rx_t(const Shape &sh, const CudaEngine *ce, const fsk_b200_loopc *lc,
-	const RxArgs &a, cudaStream_t st)
+	const RxArgs &a, cudaStream_t st, const AutoArgs &au = AutoArgs())
 {
-    cudaError_t e = cudaFuncSetAttribute(k_rx<G, W, L, MODE, FILL, SRC>,
+    cudaError_t e = cudaFuncSetAttribute(k_rx<G, W, L, MODE, FILL, SRC, AUTO>,
 	    cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sh.smem);
     if (e != cudaSuccess)
 	return e;
-    FSK_LAUNCH((k_rx<G, W, L, MODE, FILL, SRC>), sh.blocks, sh.wpb * 32, sh.smem, st, sh.geo, *lc,
-	    MODE == 3 ? ce->d_twc : ce->d_tw, sh.tw_in_smem, sh.ring, sh.lookahead, a, sh.mplan, ce->d_tw, sh.pfx);
+    /* AUTO: no block-wide table is staged (tw_in_smem 0); every stream fills its own */
+    FSK_LAUNCH((k_rx<G, W, L, MODE, FILL, SRC, AUTO>), sh.blocks, sh.wpb * 32, sh.smem, st, sh.geo, *lc,
+	    MODE == 3 ? ce->d_twc : ce->d_tw, AUTO ? 0u : sh.tw_in_smem, sh.ring, sh.lookahead, a, sh.mplan, ce->d_tw, sh.pfx,
+	    au);
     g_launches++;
     return cudaGetLastError();
 }
@@ -2226,6 +2365,101 @@ extern "C" int fsk_b200_cuda_rx_batch_s16(void *p, const fsk_b200_geom *g, const
 {
     return rx_batch_any((CudaEngine *)p, g, lc, samples, 2, nstreams, stride, nsamples, nsamples_all, frames,
 	    max_frames, states, stream);
+}
+
+/* --auto-carrier: the shapes of the per-candidate kernel with a tone table per stream (AUTO 1), in float
+ * and int16 builds -- what pick_shape chooses for the presets of fsk_b200_rx_config_for_mode at 8 and 48 kHz */
+#define AUTO_COMBOS(X) \
+    X(8, 3, 2) X(16, 2, 4) X(16, 3, 4) X(16, 3, 1) X(32, 1, 4) X(32, 2, 4) X(32, 3, 2)
+
+/* (cos, -sin)(2 pi r / fftsize): the expression of fsk_b200_cuda_set_table with r = (b * n) mod fftsize, so
+ * every per-stream table entry is bit-identical to the one a fixed-tone engine builds */
+extern "C" int fsk_b200_cuda_set_unit_table(void *p, int fftsize)
+{
+    CudaEngine *ce = (CudaEngine *)p;
+    if (ce->d_unit && ce->unit_f == fftsize)
+	return 0;
+    if (fftsize <= 0)
+	return -EINVAL;
+    float2 *h = (float2 *)malloc(sizeof(float2) * (size_t)fftsize);
+    if (!h)
+	return -ENOMEM;
+    const double F = (double)fftsize;
+    for (int r = 0; r < fftsize; r++) {
+	const double a = 2.0 * M_PI * (double)r / F;
+	h[r].x = (float)cos(a);
+	h[r].y = (float)-sin(a);
+    }
+    cudaFree(ce->d_unit);
+    ce->d_unit = NULL;
+    ce->unit_f = 0;
+    cudaError_t err = cudaMalloc(&ce->d_unit, sizeof(float2) * (size_t)fftsize);
+    if (err == cudaSuccess)
+	err = cudaMemcpy(ce->d_unit, h, sizeof(float2) * (size_t)fftsize, cudaMemcpyHostToDevice);
+    if (err == cudaSuccess)
+	err = cudaDeviceSynchronize();
+    free(h);
+    if (err != cudaSuccess) {
+	fsk_b200_set_error("set_unit_table: %s", cudaGetErrorString(err));
+	return -EIO;
+    }
+    ce->unit_f = fftsize;
+    return 0;
+}
+
+/* elem 4: float32 rows, elem 2: int16 rows.  -ENOTSUP (nothing launched) where the per-candidate kernel
+ * cannot take the mode or the shape has no auto build. */
+extern "C" int fsk_b200_cuda_rx_batch_auto(void *p, const fsk_b200_geom *g, const fsk_b200_loopc *lc,
+	const fsk_b200_auto_args *aa, const void *samples, int elem, size_t nstreams, size_t stride,
+	const uint32_t *nsamples, uint32_t nsamples_all, fsk_b200_frame *frames, uint32_t max_frames,
+	fsk_b200_stream_state *states, fsk_b200_auto_state *auto_states, uint32_t *rec_band, void *stream)
+{
+    CudaEngine *ce = (CudaEngine *)p;
+    if (!ce->d_unit || ce->unit_f != aa->fftsize) {
+	fsk_b200_set_error("rx_batch_auto: auto-carrier not set");
+	return -EINVAL;
+    }
+    if (engine_device_check(ce, "rx_batch_auto"))
+	return -EINVAL;
+    Shape sh;
+    const unsigned tmax = lc->try_max_nocarrier > lc->try_max_carrier ? lc->try_max_nocarrier : lc->try_max_carrier;
+    const unsigned max_advance = tmax - 1u + lc->frame_nsamples;
+    pick_shape(ce, g, tmax - 1u + g->span, max_advance, nstreams, &sh, lc, true);
+    fsk_b200_loopc lc_launch = *lc;
+    lc_launch.slide = sh.slide;
+    bool launched = false;
+    cudaError_t e = cudaErrorInvalidValue;
+    if (sh.mode == 0) {
+	const RxArgs a = { elem == 4 ? (const float *)samples : NULL, elem == 2 ? (const int16_t *)samples : NULL,
+	    (unsigned)nstreams, stride, nsamples, nsamples_all, frames, max_frames, states };
+	const AutoArgs au = { auto_states, rec_band, ce->d_unit, aa->threshold, aa->scan_n, aa->b_shift,
+	    (unsigned)aa->fftsize, aa->nbands, aa->half_ring, aa->expect_nsamples };
+	cudaStream_t st = (cudaStream_t)stream;
+	if (elem == 2) {
+#define X(GG, WW, LL) if (sh.G == GG && sh.W == WW && sh.L == LL) { e = launch_rx_t<GG, WW, LL, 0, 0, 1, 1>(sh, ce, &lc_launch, a, st, au); launched = true; }
+	    AUTO_COMBOS(X)
+#undef X
+	} else {
+#define X(GG, WW, LL) if (sh.G == GG && sh.W == WW && sh.L == LL) { e = launch_rx_t<GG, WW, LL, 0, 0, 0, 1>(sh, ce, &lc_launch, a, st, au); launched = true; }
+	    AUTO_COMBOS(X)
+#undef X
+	}
+    }
+    if (!launched) {
+	fsk_b200_set_error("rx_batch_auto: no auto-carrier build of the per-candidate kernel for this mode "
+		"(launch shape G=%d W=%d L=%d mode=%d)", sh.G, sh.W, sh.L, sh.mode);
+	return -ENOTSUP;
+    }
+    snprintf(ce->last_kernel, sizeof(ce->last_kernel),
+	    "k_rx_auto<G=%d,W=%d,L=%d,mode=0(per-candidate),fill=0,src=%s> threads=%d ring=%u smem=%zu blocks=%d",
+	    sh.G, sh.W, sh.L, elem == 2 ? (sh.slide ? "s16,slide" : "s16") : (sh.slide ? "f32,slide" : "f32"),
+	    sh.wpb * 32, sh.ring, sh.smem, sh.blocks);
+    if (e != cudaSuccess) {
+	fsk_b200_set_error("rx_batch_auto launch (G=%d W=%d L=%d ring=%u smem=%zu): %s", sh.G, sh.W, sh.L, sh.ring,
+		sh.smem, cudaGetErrorString(e));
+	return -EIO;
+    }
+    return 0;
 }
 
 /* host buffers in, host results out: slabs of streams, copy/compute overlap on two streams.

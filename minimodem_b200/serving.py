@@ -11,7 +11,9 @@ Per call: fsk_b200_stream_push (carry the unconsumed tail, append the chunk) -> 
 decoder for the mode, with its per-stream state carried along).  The holdback is set so that a
 search only starts when every sample it can touch has arrived: the text does not depend on how
 the stream was cut into chunks (tests/test_gpu_parity.py::test_live_receiver_*).  Everything
-stays on the device; there is no per-stream work on the host.
+stays on the device; there is no per-stream work on the host.  With auto_carrier=threshold (0.001 is
+the CLI's -a) every stream finds its own tone pair: fsk_b200_rx_batch_auto with the per-stream
+auto states and the auto holdback (fsk_b200_auto_stream_window) in place of fsk_b200_rx_batch.
 
     tx = LiveTransmitter("rtty", sample_rate=8000, nstreams=4096, max_text=64)
     for text, lengths in source:                  # uint8 CUDA tensor [nstreams, <= max_text], int32 [nstreams]
@@ -29,12 +31,14 @@ from . import api
 
 class LiveReceiver:
     def __init__(self, baudmode, sample_rate=48000, nstreams=1, max_chunk=4800, device=None,
-                 binary_output=False, **overrides):
+                 binary_output=False, auto_carrier=None, **overrides):
         torch = api._torch()
-        cfg = api.rx_config_for_mode(baudmode, sample_rate, **overrides)
-        self.engine = api.RxEngine(api.rx_params(cfg))
+        self.engine = api.RxEngine.for_mode(baudmode, sample_rate, **overrides)
         self.kind = api.decoder_for_mode(baudmode, self.engine.params.n_data_bits, binary_output)
-        self.window = self.engine.stream_window()
+        self.auto = auto_carrier is not None
+        if self.auto:
+            self.engine.set_auto_carrier(auto_carrier, inverted=bool(overrides.get("inverted", False)))
+        self.window = self.engine.auto_stream_window() if self.auto else self.engine.stream_window()
         self.engine.set_holdback(self.window)
         self.nstreams, self.max_chunk = int(nstreams), int(max_chunk)
         # a row holds the longest tail the loop can leave behind plus one chunk
@@ -50,11 +54,17 @@ class LiveReceiver:
         self.dstates = z((self.nstreams, api.DECODER_STATE_BYTES), torch.uint8)
         self.dropped = z((self.nstreams,), torch.int32)
         self._empty = z((self.nstreams, 4), torch.float32)
+        self.auto_states = z((self.nstreams, api.AUTO_STATE_BYTES), torch.uint8) if self.auto else None
 
     def _step(self, chunk, lengths):
         api.stream_push(self.rows, self.fill, self.states, chunk, lengths, dropped=self.dropped)
-        frames, self.states = self.engine.rx_batch(self.rows, nsamples=self.stride, nsamples_each=self.fill,
-                                                   max_frames=self.max_frames, states=self.states)
+        if self.auto:
+            frames, self.states, self.auto_states = self.engine.rx_batch_auto(
+                self.rows, nsamples=self.stride, nsamples_each=self.fill, max_frames=self.max_frames,
+                states=self.states, auto_states=self.auto_states)
+        else:
+            frames, self.states = self.engine.rx_batch(self.rows, nsamples=self.stride, nsamples_each=self.fill,
+                                                       max_frames=self.max_frames, states=self.states)
         return self.engine.decode_batch(self.kind, frames, self.states, dstates=self.dstates,
                                         out_stride=self.row_bytes)
 
