@@ -327,19 +327,7 @@ struct LaneWin {
     unsigned beg[W];	/* bit_begin of window j (0 for a slot past n_bits) */
     unsigned own;	/* bit j: this lane decides window j */
     unsigned exp;	/* 2 bits per (sel, j): expect value 0, 1 or 2 */
-    unsigned a_end;	/* samples of a candidate that the first stage (windows j < STAGE_J) reads */
 };
-
-/* The correlation of a candidate can run in two stages: the windows j < FSK_STAGE_J of every
- * lane (the first FSK_STAGE_J*G/L bits of the frame), then the rest.  The rx loop asks for the
- * tail of a frame's samples only when it gets there, so a first stage could work on samples
- * already in the ring while the copies of the rest are in flight.  Measured: the second
- * twiddle pass costs more than the hidden latency buys (-4.5 % at stage 1, -6 % at stage 2),
- * so the default is one stage (any value >= W); the wait still sits inside the search, right
- * before the first candidate's correlation. */
-#ifndef FSK_STAGE_J
-#define FSK_STAGE_J 99
-#endif
 
 template <int G, int W, int L>
 __device__ __forceinline__ LaneWin<W> lane_windows(const fsk_b200_geom &geo, unsigned g)
@@ -349,10 +337,6 @@ __device__ __forceinline__ LaneWin<W> lane_windows(const fsk_b200_geom &geo, uns
     LaneWin<W> lw;
     lw.own = 0;
     lw.exp = 0;
-    {
-	const unsigned na = min((unsigned)FSK_STAGE_J * WPP, geo.n_bits);
-	lw.a_end = geo.bit_begin[na - 1u] + geo.bit_nsamples;
-    }
 #pragma unroll
     for (int j = 0; j < W; j++) {
 	const unsigned w = j * WPP + wslot;
@@ -366,22 +350,16 @@ __device__ __forceinline__ LaneWin<W> lane_windows(const fsk_b200_geom &geo, uns
     return lw;
 }
 
-/* windows J0..J1-1 of this lane against both tones, its share n = part, part+L, ... of the samples */
-template <int J0, int J1, int W, int L>
+/* the W windows of this lane against both tones, its share n = part, part+L, ... of the samples */
+template <int W, int L>
 __device__ __forceinline__ void corr_pass(float (&acc)[W][4], const float *const (&p)[W],
 	const float4 *tw, unsigned part, unsigned N)
 {
-#if defined(FSK_UNROLL) && FSK_UNROLL == 8
-    _Pragma("unroll 8")
-#elif defined(FSK_UNROLL) && FSK_UNROLL == 2
-    _Pragma("unroll 2")
-#else
-    _Pragma("unroll 4")
-#endif
+#pragma unroll 4
     for (unsigned n = part; n < N; n += L) {
 	const float4 c = tw[n];
 #pragma unroll
-	for (int j = J0; j < J1; j++) {
+	for (int j = 0; j < W; j++) {
 	    const float x = p[j][n];
 	    acc[j][0] = fmaf(x, c.x, acc[j][0]);
 	    acc[j][1] = fmaf(x, c.y, acc[j][1]);
@@ -401,22 +379,17 @@ struct Found {
  * between the L lanes of a window, the per-window decision (src/fsk.c:158-169, :211), the sums
  * and the confidence (:271-336).  CONSEC: window j of the lane is bit wslot*W + j (MULTI) instead
  * of j*(G/L) + wslot.  p[j] = first sample of window j (for the fp64 re-sum). */
-template <int G, int W, int L, bool WS, bool CONSEC>
+template <int G, int W, int L, bool CONSEC>
 __device__ __forceinline__ float frame_finish(float (&acc)[W][4], const float *const (&p)[W],
 	const unsigned own_mask, const unsigned exp_bits, const fsk_b200_geom &geo, const float4 *tw, int sel,
-	unsigned g, unsigned gmask_in, unsigned &bits_lo_out, unsigned &bits_hi_out, float &ampl_out,
+	unsigned g, unsigned gmask, unsigned &bits_lo_out, unsigned &bits_hi_out, float &ampl_out,
 	float2 *bit_mags = nullptr)
 {
-    const unsigned gmask = WS ? 0xffffffffu : gmask_in;
     constexpr unsigned WPP = G / L;
     const unsigned N = geo.bit_nsamples, nb = geo.n_bits;
     const unsigned part = g % L, wslot = g / L;
     constexpr int KW = (W + L - 1) / L;
-#ifdef FSK_NO_XCHG
-    constexpr bool XCHG = false;
-#else
     constexpr bool XCHG = (L == 2);
-#endif
     /* XCHG (L == 2): instead of an all-reduce that leaves every sum on both lanes of a window, the
      * two lanes swap the partial sums of the window the OTHER one post-processes (same two
      * addends, so the same sums): 4 shuffles per round instead of 8 */
@@ -519,12 +492,11 @@ __device__ __forceinline__ float frame_finish(float (&acc)[W][4], const float *c
 	    }
 	}
     }
-    /* pass 1 reject, src/fsk.c:211-212.  The group-masked form does not vote: a lane that saw a
-     * mismatch poisons the noise sum with +inf, and the verdict is read off the reduced sum
-     * (one convergence point fewer per candidate; a noise sum that overflowed by itself would
-     * give confidence 0, which never wins either). */
-    const bool rejected_ws = WS ? (__ballot_sync(0xffffffffu, mismatch) & gmask_in) != 0u : false;
-    if (!WS && mismatch)
+    /* pass 1 reject, src/fsk.c:211-212.  No vote: a lane that saw a mismatch poisons the noise sum
+     * with +inf, and the verdict is read off the reduced sum (one convergence point fewer per
+     * candidate; a noise sum that overflowed by itself would give confidence 0, which never wins
+     * either). */
+    if (mismatch)
 	tn = INFINITY;
     /* total_sig = sum over marks + sum over spaces; the mark count rides above the bits when
      * the frame is short enough (disjoint bit positions: OR == ADD) */
@@ -537,8 +509,7 @@ __device__ __forceinline__ float frame_finish(float (&acc)[W][4], const float *c
 	as += __shfl_xor_sync(gmask, as, o);
 	packed += __shfl_xor_sync(gmask, packed, o);
     }
-    const bool rejected = WS ? rejected_ws : tn == INFINITY;
-    if (!WS && rejected) {
+    if (tn == INFINITY) {
 	bits_lo_out = bits_hi_out = 0;
 	ampl_out = 0.f;
 	return 0.f;
@@ -573,11 +544,6 @@ __device__ __forceinline__ float frame_finish(float (&acc)[W][4], const float *c
     divergence *= 2.f;						/* :312-313 */
     divergence = divergence * geo.inv_n_bits;
 
-    if (WS && rejected) {
-	bits_lo_out = bits_hi_out = 0;
-	ampl_out = 0.f;
-	return 0.f;
-    }
     bits_lo_out = blo;
     bits_hi_out = bhi;
     ampl_out = avg_bit_sig;					/* :342 */
@@ -590,27 +556,20 @@ __device__ __forceinline__ float frame_finish(float (&acc)[W][4], const float *c
  * to memory, and the frame statistics of src/fsk.c:271-336 are formed by
  * butterfly reductions over the group instead of a serial loop over the bits
  * (same terms, different but fixed summation order). */
-template <int G, int W, int L, bool WS = false, bool CONSEC = false, class LW = LaneWin<W> >
+template <int G, int W, int L, bool CONSEC = false, class LW = LaneWin<W> >
 __device__ __forceinline__ float frame_analyze_fast(const Ring rg, unsigned cand_off,
 	const fsk_b200_geom &geo, const LW &lw, int sel, unsigned tw_s,
-	unsigned g, unsigned gmask_in, unsigned &bits_lo_out, unsigned &bits_hi_out, float &ampl_out,
-	int avail, bool &pending, float2 *bit_mags = nullptr)
+	unsigned g, unsigned gmask, unsigned &bits_lo_out, unsigned &bits_hi_out, float &ampl_out,
+	bool &pending, float2 *bit_mags = nullptr)
 {
-    /* WS ("warp-synchronous"): the caller guarantees that all 32 lanes are here together, so
-     * shuffles and votes use the constant full mask (the shuffle distances stay inside a
-     * group); with a run-time group mask the compiler has to guard every shuffle with a
-     * MATCH/VOTE sequence.  A rejected candidate is then zeroed at the end instead of
-     * returning early. */
-    const unsigned gmask = WS ? 0xffffffffu : gmask_in;
     /* ring and twiddles are handed over as shared-window addresses and turned back into
      * pointers here, so that the compiler keeps them in the shared address space (LDS with
      * 32-bit addresses and immediate offsets) even though this code is not inlined */
     const float *ring = static_cast<const float *>(__cvta_shared_to_generic(rg.ring_s));
     const float4 *tw = static_cast<const float4 *>(__cvta_shared_to_generic(tw_s));
     /* cand_off: ring offset (< R) of the candidate's first sample */
-    constexpr unsigned WPP = G / L;		/* windows per pass */
-    const unsigned N = geo.bit_nsamples, nb = geo.n_bits, R = rg.R;
-    const unsigned part = g % L, wslot = g / L;
+    const unsigned N = geo.bit_nsamples, R = rg.R;
+    const unsigned part = g % L;
 
     /* slots past n_bits read window 0: harmless, their results are dropped */
     const float *p[W];
@@ -623,55 +582,15 @@ __device__ __forceinline__ float frame_analyze_fast(const Ring rg, unsigned cand
     for (int j = 0; j < W; j++)
 	acc[j][0] = acc[j][1] = acc[j][2] = acc[j][3] = 0.f;
 
-    /* `pending`: copies into this ring may still be in flight; `avail` samples from the
-     * candidate's first one are known to have landed */
-    constexpr int SJ = (FSK_STAGE_J < W) ? FSK_STAGE_J : 0;
-    if (SJ > 0) {
-	if (pending && (int)lw.a_end > avail) {
-	    cp_async_wait<0>();
-	    __syncwarp(gmask);
-	    pending = false;
-	}
-	corr_pass<0, SJ, W, L>(acc, p, tw, part, N);
-    }
+    /* `pending`: copies into this ring may still be in flight */
     if (pending) {
 	cp_async_wait<0>();
 	__syncwarp(gmask);
 	pending = false;
     }
-    corr_pass<SJ, W, W, L>(acc, p, tw, part, N);
-    return frame_finish<G, W, L, WS, CONSEC>(acc, p, lw.own, lw.exp, geo, tw, sel, g, gmask_in, bits_lo_out,
+    corr_pass<W, L>(acc, p, tw, part, N);
+    return frame_finish<G, W, L, CONSEC>(acc, p, lw.own, lw.exp, geo, tw, sel, g, gmask, bits_lo_out,
 	    bits_hi_out, ampl_out, bit_mags);
-}
-
-/* The zig-zag search of src/fsk.c:477-502 run warp-synchronously: every lane of the warp
- * takes every trip of the loop; a group whose search is over (or that has no stream, `on`
- * false) rides along on candidate 0 and drops the result.  SIMT would spend those trips
- * waiting anyway; in exchange all shuffles inside use the constant full mask. */
-template <int G, int W, int L>
-__device__ __noinline__ Found find_frame_ws(const Ring rg, unsigned pos_off,
-	const fsk_b200_geom &geo, const LaneWin<W> lw, int sel, unsigned tw_s, unsigned g,
-	unsigned gmask, bool on, unsigned try_first, unsigned try_max, unsigned try_step, float limit)
-{
-    Found best = { 0.f, 0.f, 0u, 0u, 0u };
-    bool searching = on, nopend = false;
-    for (int j = 0; __any_sync(0xffffffffu, searching); j++) {
-	const int up = (j & 1) ? 1 : -1;
-	const int t = (int)try_first + up * ((j + 1) / 2) * (int)try_step;
-	if (t >= (int)try_max)
-	    searching = false;					/* :481 */
-	const bool eval = searching && t >= 0;			/* :483 */
-	unsigned lo, hi;
-	float a;
-	const float c = frame_analyze_fast<G, W, L, true>(rg, eval ? ring_wrap(pos_off + (unsigned)t, rg.R) : 0u,
-		geo, lw, sel, tw_s, g, gmask, lo, hi, a, 0, nopend);
-	if (eval && best.confidence < c) {			/* :492: NaN and negatives never win */
-	    best = Found{ c, a, (unsigned)t, lo, hi };
-	    if (c >= limit)
-		searching = false;				/* :499 first to reach the limit wins */
-	}
-    }
-    return best;
 }
 
 /* frame search, src/fsk.c:449-538 */
@@ -679,10 +598,10 @@ template <int G, int W, int L>
 __device__ __forceinline__ Found find_frame_fast_body(const Ring rg, unsigned pos_off,
 	const fsk_b200_geom &geo, const LaneWin<W> lw, int sel, unsigned tw_s,
 	unsigned g, unsigned gmask, unsigned try_first, unsigned try_max, unsigned try_step, float limit,
-	int ready, bool pending, unsigned &ncand)
+	bool pending, unsigned &ncand)
 {
-    /* pending: the caller's latest copies into the ring are still in flight, and `ready` samples
-     * from pos_off on are known to have landed; the first candidate waits as late as it can */
+    /* pending: the caller's latest copies into the ring are still in flight; the first candidate
+     * waits as late as it can */
     Found best = { 0.f, 0.f, 0u, 0u, 0u };
     for (int j = 0;; j++) {					/* :477-502 */
 	const int up = (j & 1) ? 1 : -1;
@@ -695,7 +614,7 @@ __device__ __forceinline__ Found find_frame_fast_body(const Ring rg, unsigned po
 	float a;
 	ncand++;
 	const float c = frame_analyze_fast<G, W, L>(rg, ring_wrap(pos_off + (unsigned)t, rg.R), geo, lw, sel,
-		tw_s, g, gmask, lo, hi, a, ready - t, pending);
+		tw_s, g, gmask, lo, hi, a, pending);
 	if (best.confidence < c) {			/* NaN and negatives never win */
 	    best = Found{ c, a, (unsigned)t, lo, hi };
 	    if (c >= limit)
@@ -738,7 +657,7 @@ __device__ __forceinline__ Found find_frame_slide(const Ring rg, unsigned pos_of
 	p[j] = ring + ring_wrap(ring_wrap(pos_off + t, R) + lw.beg[j], R);
 	acc[j][0] = acc[j][1] = acc[j][2] = acc[j][3] = 0.f;
     }
-    corr_pass<0, W, W, L>(acc, p, tw + t, part, N);	/* the lowest candidate: a full correlation, phase index t + n */
+    corr_pass<W, L>(acc, p, tw + t, part, N);	/* the lowest candidate: a full correlation, phase index t + n */
 
     Found best = { 0.f, 0.f, 0u, 0u, 0u };
     unsigned best_order = 0;
@@ -753,7 +672,7 @@ __device__ __forceinline__ Found find_frame_slide(const Ring rg, unsigned pos_of
 		wsum[j][k] = acc[j][k];			/* frame_finish may reduce in place */
 	unsigned lo, hi;
 	float a;
-	const float c = frame_finish<G, W, L, false, false>(wsum, p, lw.own, lw.exp, geo, tw, sel, g, gmask, lo, hi, a);
+	const float c = frame_finish<G, W, L, false>(wsum, p, lw.own, lw.exp, geo, tw, sel, g, gmask, lo, hi, a);
 	/* place in the reference's visiting order: first, +1, -1, +2, -2, ... */
 	const unsigned order = t >= try_first ? (t == try_first ? 0u : 2u * ((t - try_first) / step) - 1u)
 	    : 2u * ((try_first - t) / step);
@@ -818,7 +737,6 @@ struct LaneWinM {
     unsigned own;	/* bit j: this lane decides window j (one of the L lanes of the slot, round-robin) */
     unsigned exp;	/* 2 bits per (sel, j): expect value 0, 1 or 2 */
     unsigned wrapj;	/* the j whose slot is the wrap-around slot (period -1), W if it is not this lane's */
-    unsigned a_end;	/* unused (interface of LaneWin) */
     unsigned rot0;	/* this slot starts its walk over every segment rot0 iterations in, and wraps: periods are
 			 * a multiple of the bank count apart in slow modes, so slots walking in step would
 			 * hit the same shared-memory banks (0: the periods spread the slots by themselves) */
@@ -833,7 +751,6 @@ __device__ __forceinline__ LaneWinM<W> lane_windows_multi(const fsk_b200_geom &g
     lw.own = 0;
     lw.exp = 0;
     lw.wrapj = W;
-    lw.a_end = 0;
 #pragma unroll
     for (int j = 0; j < W; j++) {
 	const unsigned m = slot * W + j;
@@ -1058,7 +975,7 @@ __device__ __forceinline__ FoundN find_frame_multi(const Ring rg, unsigned pos_o
 		q[j] = ring + ring_wrap(cand_off + lw.beg[j], R);
 	    unsigned lo, hi;
 	    float a;
-	    const float c = frame_finish<G, W, L, false, true>(wp, q, lw.own, lw.exp, geo, tw, sel, g, gmask,
+	    const float c = frame_finish<G, W, L, true>(wp, q, lw.own, lw.exp, geo, tw, sel, g, gmask,
 		    lo, hi, a);
 	    /* src/fsk.c:492-501 visits the candidates in `order`; a later batch may hold an earlier
 	     * candidate, so among equals the earlier one is kept (what `best_c < c` does there) */
@@ -1550,32 +1467,14 @@ __device__ __forceinline__ void ring_issue(const Ring rg, const float *__restric
 #define RING_BLOCK 128u
 #endif
 
-/* one whole block, all of it valid: foff = ring offset of the block, src = its first sample */
-template <int G>
-__device__ __forceinline__ void ring_block(const Ring rg, unsigned ring_s, unsigned foff,
-	const float *__restrict__ src, unsigned g)
-{
-    constexpr int CPL = (int)(RING_BLOCK / 4u) / G;	/* copies per lane */
-    const unsigned d = ring_s + (foff + 4u * g) * 4u;
-    const float *sp = src + 4u * g;
-#pragma unroll
-    for (int k = 0; k < CPL; k++)
-	ldgsts16(d + (unsigned)k * 16u * G, sp + k * 4 * G);
-    if (foff < rg.pad) {			/* the head of the ring is mirrored behind its end */
-#pragma unroll
-	for (int k = 0; k < CPL; k++)
-	    if (foff + 4u * (g + (unsigned)k * G) < rg.pad)
-		ldgsts16(d + rg.R * 4u + (unsigned)k * 16u * G, sp + k * 4 * G);
-    }
-}
-
-/* the same with the lane's addresses carried by the caller: dst/src = this lane's first chunk
- * of the block, mlim = shared address below which a chunk belongs to the mirrored head */
+/* one whole block, all of it valid, with the lane's addresses carried by the caller: dst/src = this
+ * lane's first chunk of the block, mlim = shared address below which a chunk belongs to the mirrored
+ * head of the ring (copied behind its end as well) */
 template <int G>
 __device__ __forceinline__ void ring_block_at(unsigned dst, const float *__restrict__ src,
 	unsigned mlim, unsigned R)
 {
-    constexpr int CPL = (int)(RING_BLOCK / 4u) / G;
+    constexpr int CPL = (int)(RING_BLOCK / 4u) / G;	/* copies per lane */
 #pragma unroll
     for (int k = 0; k < CPL; k++)
 	ldgsts16(dst + (unsigned)k * 16u * G, src + k * 4 * G);

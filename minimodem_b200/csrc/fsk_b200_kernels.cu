@@ -8,7 +8,7 @@
  *     hands out, so streams of different length or difficulty balance by themselves;
  *   - the stream's samples live in a per-stream shared-memory RING (whole 128-float
  *     blocks, the first bit-window length mirrored behind its end); every input sample
- *     is fetched from HBM exactly once with 16-byte cp.async copies (or, selectably,
+ *     is fetched from HBM exactly once with 16-byte cp.async copies (MODE 3: by default
  *     cp.async.bulk through the TMA engine) issued one loop iteration ahead of its use;
  *   - inside a frame candidate the lanes of a group split the bit windows and, L lanes
  *     per window, the samples of a window, and correlate each window against the mark
@@ -28,8 +28,7 @@
  * k_rx<G,W,L,MODE,FILL,SRC> the whole rx loop per stream: MODE 0 per candidate (the headline kernel at
  *                         1200 baud), 1 generic (global memory, IEEE, serial order), 2 shared segments,
  *                         3 prefix table (G = 32; W codes the candidate slot); FILL 0 cp.async, 1 TMA bulk
- *                         copies; SRC 0 float32 rows, 1 int16 PCM rows widened inside the fill
- * k_rx_ws<G,W,L>          MODE 0, warp-synchronous (selectable)
+ *                         copies (MODE 3 only); SRC 0 float32 rows, 1 int16 PCM rows widened inside the fill
  * k_find_frame<G,W,L,MODE> batched fsk_find_frame
  * k_tx_synth<T,VEC,LUT>   the transmitter: text (or data words) -> int16 / float32 samples
  * k_band_mags, k_detect_carrier, k_s16_to_f32, k_decode<KIND>   the "next" rows (DESIGN.md 0)
@@ -268,7 +267,7 @@ k_find_frame(const __grid_constant__ fsk_b200_geom geo, const float4 *__restrict
 		 * (magnitudes, decisions and confidence right; tests/test_gpu_instantiations.py) */
 		unsigned ncand = 0;
 		const Found f = find_frame_fast_body<G, W, L>(rg, off & 3u, geo, lw, sel, tw_s, g, gmask,
-			a.try_first[s], tmax, tstep, a.limit[s], 0, false, ncand);
+			a.try_first[s], tmax, tstep, a.limit[s], false, ncand);
 		conf = f.confidence;
 		ampl = f.amplitude;
 		start = f.start;
@@ -279,7 +278,7 @@ k_find_frame(const __grid_constant__ fsk_b200_geom geo, const float4 *__restrict
 		    bool nopend = false;
 		    __syncwarp(gmask);
 		    (void)frame_analyze_fast<G, W, L>(rg, ring_wrap((off & 3u) + f.start, rg.R), geo, lw, sel, tw_s,
-			    g, gmask, lo, hi, am, 0, nopend, a.bit_mags + (size_t)s * geo.n_bits);
+			    g, gmask, lo, hi, am, nopend, a.bit_mags + (size_t)s * geo.n_bits);
 		}
 	    } else {
 		const GlobalSrc src = { x, n };
@@ -302,15 +301,9 @@ k_find_frame(const __grid_constant__ fsk_b200_geom geo, const float4 *__restrict
 /* K2: the rx loop (src/minimodem.c:1137-1463) for whole streams            */
 /* ------------------------------------------------------------------------ */
 
-/* FILL 0: cp.async (LDGSTS) by all lanes of the group; FILL 1: cp.async.bulk (TMA engine)
- * issued by lane 0 with mbarrier completion.
- * EARLY_REQ (FILL 0): ask for the next iteration's samples as soon as the searches of this one
- * are over rather than at the top of the next iteration. */
-#ifdef FSK_NO_EARLY_REQ
-#define EARLY_REQ 0
-#else
-#define EARLY_REQ 1
-#endif
+/* FILL 0: cp.async (LDGSTS) by all lanes of the group, the next iteration's samples asked for as
+ * soon as the searches of this one are over rather than at the top of the next iteration;
+ * FILL 1 (MODE 3): cp.async.bulk (TMA engine) issued by lane 0 with mbarrier completion. */
 /* 128 threads x 4 blocks caps the kernel at 128 registers per thread: 8 blocks of 64 threads per
  * SM, which is also what the shared-memory rings allow */
 #ifndef FSK_MINBLOCKS
@@ -338,6 +331,7 @@ k_rx(const __grid_constant__ fsk_b200_geom geo, const __grid_constant__ fsk_b200
 	const float4 *__restrict__ tw_sample, const __grid_constant__ fsk_b200_pfx pg,
 	const __grid_constant__ AutoArgs au)
 {
+    static_assert(FILL == 0 || MODE == 3, "bulk fill: prefix-table kernel only");
     static_assert(!AUTO || (MODE == 0 && FILL == 0), "auto-carrier: per-candidate kernel, cp.async fill");
     FSK_DYN_SMEM(smem4);
     /* MODE 3 (chunk-prefix table): the ring's mirror covers one lane-run of the table build (not a bit window);
@@ -412,7 +406,6 @@ k_rx(const __grid_constant__ fsk_b200_geom geo, const __grid_constant__ fsk_b200
 	bool tail_fix = false;				/* bulk fill: [n, n4) holds row padding, not zeros */
 
 	const unsigned ring_s = rg.ring_s;
-	unsigned landed = pos & ~AL;			/* absolute index up to which copies are known to have landed */
 	/* block fill: this lane's running source and destination (its first 16-byte chunk of
 	 * the block that starts at absolute index `filled`), carried instead of recomputed */
 	const unsigned dst0 = ring_s + 16u * g, dst_end = dst0 + R * 4u;
@@ -459,29 +452,22 @@ k_rx(const __grid_constant__ fsk_b200_geom geo, const __grid_constant__ fsk_b200
 		    filled = to;
 	    }
 	};
-	/* wait for everything requested before the latest request (all of it if `all`) */
+	/* bulk fill: wait for everything requested before the latest request (all of it if `all`) */
 	auto settle = [&](bool all) {
-	    if (FILL == 0) {
-		if (all)
-		    cp_async_wait<0>();
-		else
-		    cp_async_wait<1>();
-	    } else {
-		/* phase k (0-based) lives on barrier k&1 with parity (k>>1)&1 */
-		if (kphase >= 2u) {
-		    const unsigned k = kphase - 2u;
-		    mbar_wait((k & 1u) ? bar1 : bar0, (k >> 1) & 1u);
-		}
-		if ((all || tail_fix) && kphase >= 1u) {
-		    const unsigned k = kphase - 1u;
-		    mbar_wait((k & 1u) ? bar1 : bar0, (k >> 1) & 1u);
-		}
-		if (tail_fix) {
-		    __syncwarp(gmask);
-		    if (n >= (pos & ~3u))
-			ring_zero<G>(rg, pos, pos_off, n, n4, g);
-		    tail_fix = false;
-		}
+	    /* phase k (0-based) lives on barrier k&1 with parity (k>>1)&1 */
+	    if (kphase >= 2u) {
+		const unsigned k = kphase - 2u;
+		mbar_wait((k & 1u) ? bar1 : bar0, (k >> 1) & 1u);
+	    }
+	    if ((all || tail_fix) && kphase >= 1u) {
+		const unsigned k = kphase - 1u;
+		mbar_wait((k & 1u) ? bar1 : bar0, (k >> 1) & 1u);
+	    }
+	    if (tail_fix) {
+		__syncwarp(gmask);
+		if (n >= (pos & ~3u))
+		    ring_zero<G>(rg, pos, pos_off, n, n4, g);
+		tail_fix = false;
 	    }
 	    __syncwarp(gmask);
 	};
@@ -548,7 +534,6 @@ k_rx(const __grid_constant__ fsk_b200_geom geo, const __grid_constant__ fsk_b200
 			/* restart the ring at the new position, as a resumed stream starts it */
 			drain();
 			filled = pos & ~AL;
-			landed = filled;
 			pos_off = pos & AL;
 			fdst = dst0;
 			fsrc = SRC ? x : x + filled + 4u * g;
@@ -570,21 +555,16 @@ k_rx(const __grid_constant__ fsk_b200_geom geo, const __grid_constant__ fsk_b200
 	    const unsigned try_first = carrier ? lc.nsamples_overscan : 0u;	/* :1263 */
 	    const int sel = carrier ? 0 : 1;			/* :1270 data / sync string */
 
-	    int ready = 0;
 	    bool pending = false;
 	    if (MODE != 1) {
-		/* The samples of this iteration were normally requested an iteration ago (EARLY_REQ,
+		/* The samples of this iteration were normally requested an iteration ago (FILL 0,
 		 * below); whatever is missing -- first iteration of a launch, a restarted ring, the
-		 * bulk variant -- is requested here together with what the next iteration can need
+		 * bulk fill -- is requested here together with what the next iteration can need
 		 * (it starts at most `lookahead` samples further) */
 		const unsigned need_now = (pos + try_max - 1u + geo.span + 3u) & ~3u;
 		const bool late = filled < need_now;	/* part of this window is only now requested */
-		/* what the previous search's wait has seen land (two-stage correlation only): the
-		 * requests made since -- the early one and the one below -- are still in flight */
-		ready = (int)(landed - pos);
-		if (FILL != 0 || !EARLY_REQ || late)	/* EARLY_REQ: normally asked for an iteration ago */
+		if (FILL != 0 || late)
 		    request(min((pos + lookahead + need_max + 3u) & ~3u, (pos & ~AL) + R));
-		landed = filled;			/* true once this iteration's search has waited */
 		if (SRC) {
 		    /* int16 rows: everything requested so far has to land and be widened in place
 		     * before the search reads it (the float fill lets the search itself wait) */
@@ -599,14 +579,8 @@ k_rx(const __grid_constant__ fsk_b200_geom geo, const __grid_constant__ fsk_b200
 		    }
 		    pending = false;
 		} else if (FILL == 0) {
-#if FSK_STAGE_J < 8
-		    settle(false);	/* two-stage correlation: the first stage needs the older copies */
-		    pending = true;
-#else
 		    /* the search waits for all copies itself, right before its first correlation */
-		    (void)late;
 		    pending = true;
-#endif
 		} else
 		    settle(late);
 	    }
@@ -664,9 +638,9 @@ k_rx(const __grid_constant__ fsk_b200_geom geo, const __grid_constant__ fsk_b200
 			if (pass == 0 && !mhint && !mp.always) {
 			    unsigned lo, hi;
 			    float am;
-			    const float c = frame_analyze_fast<G, W, L, false, true, LaneWinM<W> >(rg,
+			    const float c = frame_analyze_fast<G, W, L, true, LaneWinM<W> >(rg,
 				    ring_wrap(pos_off + try_first, R), geo, lwm, which, tw_s, g, gmask, lo, hi, am,
-				    ready - (int)try_first, pending);
+				    pending);
 			    ncand++;
 			    if (0.f < c) {					/* src/fsk.c:492 */
 				seed = Found{ c, am, try_first, lo, hi };
@@ -685,13 +659,13 @@ k_rx(const __grid_constant__ fsk_b200_geom geo, const __grid_constant__ fsk_b200
 			    if (pass == 0 && !skip)
 				mhint = r.ncand > 1u;
 			}
-		    } else if (MODE == 0 && FILL != 3 && pass == 1 && lc.slide)
+		    } else if (MODE == 0 && pass == 1 && lc.slide)
 			/* :1373, the fine search: its candidates in ascending order, each from the one before */
 			f = find_frame_slide<G, W, L>(rg, pos_off, geo, lw, which, tw_s, g, gmask, try_first, try_max,
 				step, ncand);
 		    else
 			f = find_frame_fast_body<G, W, L>(rg, pos_off, geo, lw, which, tw_s, g,
-				gmask, try_first, try_max, step, limit, ready, pending, ncand);
+				gmask, try_first, try_max, step, limit, pending, ncand);
 		    if (pass) {
 			refined = f;
 			break;
@@ -715,7 +689,7 @@ k_rx(const __grid_constant__ fsk_b200_geom geo, const __grid_constant__ fsk_b200
 		amplitude = first.amplitude;
 		frame_start = first.start;
 		bits = ((unsigned long long)first.bits_hi << 32) | first.bits_lo;
-		if (FILL == 0 && EARLY_REQ) {
+		if (FILL == 0) {
 		    /* The searches are over, so the samples before the next start are dead: ask for
 		     * the next iteration's samples now, ahead of the bookkeeping below, instead of
 		     * right before they are needed.  `adv` restates the advance of :1318/:1407;
@@ -836,7 +810,6 @@ k_rx(const __grid_constant__ fsk_b200_geom geo, const __grid_constant__ fsk_b200
 		    /* skipped past everything requested so far: restart the ring here */
 		    drain();
 		    filled = pos & ~AL;
-		    landed = filled;
 		    pos_off = pos & AL;
 		    fdst = dst0;
 		    fsrc = SRC ? x : x + filled + 4u * g;
@@ -874,218 +847,6 @@ k_rx(const __grid_constant__ fsk_b200_geom geo, const __grid_constant__ fsk_b200
     }
 }
 
-
-/* ------------------------------------------------------------------------ */
-/* K2, warp-synchronous form (FSK_B200_FILL=3; an alternative to the           */
-/* group-masked loop): the 32/G streams of a warp step through the loop together,*/
-/* which lets every shuffle and vote use the constant full mask                */
-/* ------------------------------------------------------------------------ */
-template <int G, int W, int L>
-__global__ void __launch_bounds__(128, FSK_MINBLOCKS)
-k_rx_ws(const __grid_constant__ fsk_b200_geom geo, const __grid_constant__ fsk_b200_loopc lc,
-	const float4 *__restrict__ tw_global, unsigned ring_floats, unsigned lookahead,
-	const __grid_constant__ RxArgs a)
-{
-    FSK_DYN_SMEM(smem4);
-    const Smem sm = carve<G>(smem4, geo, tw_global, 1u, ring_floats, (geo.bit_nsamples + 3u) & ~3u);
-    GROUP_VARS;
-    const Ring rg = { smem_u32(sm.ring), ring_floats, (geo.bit_nsamples + 3u) & ~3u };
-    const unsigned tw_s = smem_u32(sm.tw);
-    const LaneWin<W> lw = lane_windows<G, W, L>(geo, g);
-    const unsigned R = ring_floats;
-    const unsigned FULL = 0xffffffffu;
-    const unsigned need_max = lc.try_max_nocarrier - 1u + geo.span;
-
-    for (unsigned s0 = (blockIdx.x * wpb + warp) * spw; s0 < a.nstreams; s0 += gridDim.x * wpb * spw) {
-	const unsigned s = s0 + sidx;
-	const bool have = s < a.nstreams;
-	fsk_b200_stream_state st;
-	if (have)
-	    st = a.states[s];
-	else
-	    memset(&st, 0, sizeof(st));
-	bool alive = have && !st.done;
-	const float *x = a.samples + (size_t)(have ? s : 0) * a.stride;
-	const unsigned n = have ? (a.nsamples ? a.nsamples[s] : a.nsamples_all) : 0u;
-	fsk_b200_frame *out = a.frames + (size_t)(have ? s : 0) * a.max_frames;
-
-	unsigned pos = (unsigned)st.pos;
-	unsigned nframes = st.nframes;
-	unsigned carrier = st.carrier, noconfidence = st.noconfidence;
-	float track_amplitude = st.track_amplitude, peak_confidence = st.peak_confidence;
-	unsigned long long carrier_nsamples = st.carrier_nsamples;
-	float confidence_total = st.confidence_total, amplitude_total = st.amplitude_total;
-	unsigned nframes_decoded = st.nframes_decoded;
-	unsigned done = st.done;
-
-	unsigned pos_off = pos & 3u;		/* ring offset of `pos` */
-	unsigned filled = pos & ~3u;		/* absolute index up to which copies were issued */
-	unsigned foff = 0;			/* ring offset of `filled` */
-	auto request = [&](unsigned to) {	/* whole blocks up to `to`, never past what the ring can hold */
-	    const unsigned cap = (pos & ~3u) + R;
-	    while (filled < to && filled + RING_BLOCK <= cap) {
-		if (filled + RING_BLOCK <= n)
-		    ring_block<G>(rg, rg.ring_s, foff, x + filled, g);
-		else
-		    ring_block_tail<G>(rg, rg.ring_s, foff, x, n, filled, g);
-		filled += RING_BLOCK;
-		foff += RING_BLOCK;
-		if (foff >= R)
-		    foff = 0;
-	    }
-	};
-	__syncwarp();
-	if (alive)
-	    request(min((pos + need_max + 3u) & ~3u, (pos & ~3u) + R));
-	cp_async_commit();
-
-	for (;;) {
-	    unsigned remaining = 0;
-	    if (alive) {
-		if (pos >= n) { done = 1; alive = false; }			/* :1176 */
-		else {
-		    remaining = n - pos;
-		    if (remaining < lc.expect_nsamples) { done = 1; alive = false; }	/* :1229 */
-		    else if (nframes >= a.max_frames) alive = false;		/* output full: resumable */
-		}
-	    }
-	    if (!__any_sync(FULL, alive))
-		break;
-
-	    unsigned try_max = carrier ? lc.try_max_carrier : lc.try_max_nocarrier;	/* :1236-1241 */
-	    unsigned try_step = try_max / 3u;			/* :1248-1251 */
-	    if (try_step == 0)
-		try_step = 1;
-	    const unsigned try_first = carrier ? lc.nsamples_overscan : 0u;	/* :1263 */
-	    const int sel = carrier ? 0 : 1;			/* :1270 data / sync string */
-
-	    /* prefetch what the next iteration can need, wait only for what this one needs */
-	    bool late = false;
-	    if (alive) {
-		const unsigned need_now = (pos + try_max - 1u + geo.span + 3u) & ~3u;
-		late = filled < need_now;
-		request(min((pos + lookahead + need_max + 3u) & ~3u, (pos & ~3u) + R));
-	    }
-	    cp_async_commit();
-	    if (__any_sync(FULL, late))
-		cp_async_wait<0>();
-	    else
-		cp_async_wait<1>();
-	    __syncwarp();
-
-	    const Found f1 = find_frame_ws<G, W, L>(rg, pos_off, geo, lw, sel, tw_s, g, gmask, alive,
-		    try_first, try_max, try_step, lc.confidence_search_limit);	/* :1265 */
-	    unsigned long long bits = ((unsigned long long)f1.bits_hi << 32) | f1.bits_lo;
-	    float amplitude = f1.amplitude;
-	    unsigned frame_start = f1.start;
-	    float confidence = f1.confidence;
-
-	    bool want_refine = false;
-	    if (confidence < peak_confidence * 0.75f) {		/* :1278-1282 */
-		want_refine = true;
-		if (alive)
-		    peak_confidence = 0.f;
-	    }
-	    if (amplitude < track_amplitude * 0.25f)		/* :1286 */
-		confidence = 0.f;
-	    const bool confident = alive && !(confidence <= lc.confidence_threshold);	/* :1292 */
-	    unsigned advance = try_max;				/* :1318 */
-	    unsigned acquired = 0;
-	    if (alive && !confident) {
-		if (++noconfidence > 20u) {			/* :1295 */
-		    if (carrier) {
-			/* report_no_carrier(), :1299-1302, as a record */
-			if (g == 0)
-			    store_frame(out + nframes, carrier_nsamples, confidence_total,
-				    amplitude_total, FSK_B200_FRAME_REPORT);
-			nframes++;
-			carrier = 0;				/* :1303-1308 */
-			carrier_nsamples = 0;
-			confidence_total = 0.f;
-			amplitude_total = 0.f;
-			nframes_decoded = 0;
-			track_amplitude = 0.f;
-		    }
-		}
-	    }
-	    if (confident) {
-		carrier_nsamples += lc.frame_nsamples;		/* :1324 */
-		if (carrier) {
-		    carrier_nsamples += frame_start;		/* :1329-1330: the COARSE start */
-		    carrier_nsamples -= lc.nsamples_overscan;
-		} else {					/* :1332-1355 */
-		    carrier = 1;
-		    acquired = FSK_B200_FRAME_ACQUIRED;
-		    want_refine = true;
-		}
-	    }
-	    /* :1357-1389: the fine search, for the groups that want it (the whole warp rides along) */
-	    const bool refine = confident && want_refine && confidence < INFINITY && try_step > 1u;
-	    if (__any_sync(FULL, refine)) {
-		unsigned fine_step = try_max / 8u;
-		if (fine_step == 0)
-		    fine_step = 1;
-		/* `carrier` is 1 by now, so the data string is searched (:1378) */
-		const Found f2 = find_frame_ws<G, W, L>(rg, pos_off, geo, lw, 0, tw_s, g, gmask, refine,
-			try_first, try_max, fine_step, INFINITY);
-		if (refine && f2.confidence > confidence) {
-		    bits = ((unsigned long long)f2.bits_hi << 32) | f2.bits_lo;
-		    amplitude = f2.amplitude;
-		    frame_start = f2.start;
-		}
-	    }
-	    if (confident) {
-		track_amplitude = (track_amplitude + amplitude) / 2.f;	/* :1391 */
-		if (peak_confidence < confidence)
-		    peak_confidence = confidence;
-		confidence_total += confidence;			/* :1397-1400 */
-		amplitude_total += amplitude;
-		nframes_decoded++;
-		noconfidence = 0;
-		if (g == 0)
-		    store_frame(out + nframes, bits, confidence, amplitude, frame_start | acquired);
-		nframes++;
-		advance = frame_start + lc.frame_nsamples - lc.nsamples_overscan;	/* :1407 */
-	    }
-	    if (alive) {
-		if (advance > remaining) { done = 1; alive = false; }	/* :1151 */
-		else {
-		    pos += advance;
-		    pos_off = ring_wrap(pos_off + advance, R);	/* advance < R by construction */
-		}
-	    }
-	    /* a group that skipped past everything requested so far restarts its ring; the copies
-	     * still in flight into it have to land first */
-	    const bool rebase = alive && filled < (pos & ~3u);
-	    if (__any_sync(FULL, rebase)) {
-		cp_async_wait<0>();
-		if (rebase) {
-		    filled = pos & ~3u;
-		    pos_off = pos & 3u;
-		    foff = 0;
-		}
-	    }
-	    __syncwarp();		/* every read of this window precedes the next copies */
-	}
-	cp_async_wait<0>();		/* nothing in flight into these rings when the slots are reused */
-	__syncwarp();
-
-	if (have && g == 0) {
-	    st.pos = pos;
-	    st.nframes = nframes;
-	    st.carrier = carrier;
-	    st.noconfidence = noconfidence;
-	    st.track_amplitude = track_amplitude;
-	    st.peak_confidence = peak_confidence;
-	    st.carrier_nsamples = carrier_nsamples;
-	    st.confidence_total = confidence_total;
-	    st.amplitude_total = amplitude_total;
-	    st.nframes_decoded = nframes_decoded;
-	    st.done = done;
-	    a.states[s] = st;
-	}
-    }
-}
 
 /* ------------------------------------------------------------------------ */
 /* full-spectrum magnitudes for fsk_detect_carrier (src/fsk.c:543-581)      */
@@ -1601,7 +1362,7 @@ struct CudaEngine {
     int tw_fftsize;
     unsigned tw_bm, tw_bs;
     /* tuning (0 = automatic) */
-    int lanes, wpb, ring, split, fill;
+    int lanes, wpb, ring, split;
     char last_kernel[160];	/* what the latest rx / find_frame launch ran (diagnostics) */
     int multi;			/* 1 (default): shared-segment search where the mode allows it; 0: always per candidate */
     int pfx_fill;		/* mode 3, float rows: 1 (default) TMA bulk fill, 0 cp.async fill */
@@ -1657,8 +1418,6 @@ extern "C" void *fsk_b200_cuda_engine_new(void)
     if ((e = getenv("FSK_B200_WPB"))) ce->wpb = atoi(e);
     if ((e = getenv("FSK_B200_RING"))) ce->ring = atoi(e);
     if ((e = getenv("FSK_B200_SPLIT"))) ce->split = atoi(e);
-    ce->fill = 0;		/* see the dispatch in fsk_b200_cuda_rx_batch */
-    if ((e = getenv("FSK_B200_FILL"))) ce->fill = atoi(e);
     /* shared-segment search: -1 (default) = modes with long bit periods, every coarse search through
      * the shared segments (at short periods the per-candidate kernel is used); 0 never; 1 everywhere it
      * fits, with the single-candidate fast path; 2 everywhere it fits, always */
@@ -1860,16 +1619,12 @@ struct Shape {
 
 /* (G, W, L) combinations that are instantiated for the fast path: G lanes per
  * stream, L lanes per bit window, W windows per lane (W * G/L >= n_bits) */
-#ifdef FSK_EXPERIMENT		/* quick builds for tuning runs */
-#define FAST_COMBOS(X) X(8, 3, 2) X(8, 2, 1) X(4, 3, 1) X(16, 3, 4) X(8, 1, 1) X(8, 2, 2) X(8, 4, 4)
-#else
 #define FAST_COMBOS(X) \
     X(4, 1, 1) X(4, 2, 1) X(4, 3, 1) X(4, 4, 1) X(4, 2, 2) X(4, 4, 2) \
     X(8, 1, 1) X(8, 2, 1) X(8, 3, 1) X(8, 4, 1) X(8, 1, 2) X(8, 2, 2) X(8, 3, 2) X(8, 4, 2) X(8, 4, 4) \
     X(16, 1, 1) X(16, 2, 1) X(16, 3, 1) X(16, 4, 1) X(16, 1, 2) X(16, 2, 2) X(16, 3, 2) X(16, 4, 2) \
     X(16, 1, 4) X(16, 2, 4) X(16, 3, 4) X(16, 4, 4) \
     X(32, 1, 1) X(32, 2, 1) X(32, 1, 2) X(32, 2, 2) X(32, 3, 2) X(32, 4, 2) X(32, 1, 4) X(32, 2, 4) X(32, 3, 4) X(32, 4, 4)
-#endif
 
 #ifndef FSK_MULTI_MIN_N
 #define FSK_MULTI_MIN_N 96u	/* shortest bit period (samples) for which mode 2 is the default */
@@ -1887,10 +1642,6 @@ struct Shape {
 #define S16_FAST_COMBOS(X) \
     X(8, 1, 1) X(8, 2, 1) X(8, 3, 1) X(8, 2, 2) X(8, 3, 2) X(8, 4, 2) X(8, 4, 4) \
     X(16, 1, 2) X(16, 2, 2) X(16, 2, 4) X(16, 3, 4) X(16, 4, 4) X(32, 2, 4)
-
-/* the alternative kernels (TMA bulk fill, group-masked loop) are built for the shapes the
- * defaults pick for the BASELINE configurations only */
-#define ALT_COMBOS(X) X(8, 3, 2) X(8, 2, 2) X(16, 3, 4) X(16, 2, 4) X(16, 1, 2)
 
 static bool fast_combo(int G, int W, int L)
 {
@@ -2020,7 +1771,7 @@ static int pick_shape(const CudaEngine *ce, const fsk_b200_geom *g, unsigned nee
 	}
     }
     sh->mode = fast ? 0 : 1;
-    if (fast && lc && !per_stream_tw && ce->multi && ce->fill == 0 && (ce->multi > 0 || g->bit_nsamples >= FSK_MULTI_MIN_N)) {
+    if (fast && lc && !per_stream_tw && ce->multi && (ce->multi > 0 || g->bit_nsamples >= FSK_MULTI_MIN_N)) {
 	/* the rx loop's searches from shared segment sums, if this mode's windows tile and all of its
 	 * searches fit the period slots of a (W, L) split of this group size */
 	int W2 = 0, L2 = 0;
@@ -2033,7 +1784,7 @@ static int pick_shape(const CudaEngine *ce, const fsk_b200_geom *g, unsigned nee
 	}
     }
     memset(&sh->pfx, 0, sizeof(sh->pfx));
-    if (lc && !per_stream_tw && ce->prefix && ce->fill == 0 && ce->twc_n && ring_min >= 128u
+    if (lc && !per_stream_tw && ce->prefix && ce->twc_n && ring_min >= 128u
 	    && (ce->prefix > 0 || g->bit_nsamples >= FSK_PREFIX_MIN_N)) {
 	/* the rx loop's searches from a chunk-prefix table (mode 3): one stream per warp, one lane per
 	 * window boundary of a candidate, the ring without its mirror plus the table per stream */
@@ -2220,20 +1971,6 @@ extern "C" int fsk_b200_cuda_find_frame_batch(void *p, const fsk_b200_geom *g, c
     return 0;
 }
 
-template <int G, int W, int L>
-static cudaError_t launch_rx_ws_t(const Shape &sh, const CudaEngine *ce, const fsk_b200_loopc *lc,
-	const RxArgs &a, cudaStream_t st)
-{
-    cudaError_t e = cudaFuncSetAttribute(k_rx_ws<G, W, L>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-	    (int)sh.smem);
-    if (e != cudaSuccess)
-	return e;
-    FSK_LAUNCH((k_rx_ws<G, W, L>), sh.blocks, sh.wpb * 32, sh.smem, st, sh.geo, *lc, ce->d_tw, sh.ring,
-	    sh.lookahead, a);
-    g_launches++;
-    return cudaGetLastError();
-}
-
 template <int G, int W, int L, int MODE, int FILL, int SRC = 0, int AUTO = 0>
 static cudaError_t launch_rx_t(const Shape &sh, const CudaEngine *ce, const fsk_b200_loopc *lc,
 	const RxArgs &a, cudaStream_t st, const AutoArgs &au = AutoArgs())
@@ -2276,10 +2013,7 @@ static int rx_batch_any(CudaEngine *ce, const fsk_b200_geom *g, const fsk_b200_l
     cudaStream_t st = (cudaStream_t)stream;
     cudaError_t e = cudaErrorInvalidValue;
     bool launched = false;
-    int fill = ce->fill;	/* mode 0: the fill of the kernel that actually ran (last_kernel) */
     if (elem == 2) {
-	if (ce->fill != 0)
-	    return -ENOTSUP;
 	if (sh.mode == 3) {
 #define X(WW) if (sh.W == WW) { e = launch_rx_t<32, WW, 1, 3, 0, 1>(sh, ce, lc, a, st); launched = true; }
 	    PFX_SLOTS(X)
@@ -2315,31 +2049,16 @@ static int rx_batch_any(CudaEngine *ce, const fsk_b200_geom *g, const fsk_b200_l
 	MULTI_COMBOS(X)
 #undef X
     } else if (sh.mode == 0) {
-	/* FSK_B200_FILL: 0 (default) cp.async fill, group-masked loop; 1 TMA bulk copies
-	 * (cp.async.bulk + mbarrier); 3 cp.async fill, warp-synchronous loop.  The two alternatives
-	 * pass the same tests; they are built for the shapes of the BASELINE configurations only. */
-	if (ce->fill == 1) {
-#define X(GG, WW, LL) if (sh.G == GG && sh.W == WW && sh.L == LL) { e = launch_rx_t<GG, WW, LL, 0, 1>(sh, ce, lc, a, st); launched = true; }
-	    ALT_COMBOS(X)
-#undef X
-	} else if (ce->fill == 3) {
-#define X(GG, WW, LL) if (sh.G == GG && sh.W == WW && sh.L == LL) { e = launch_rx_ws_t<GG, WW, LL>(sh, ce, lc, a, st); launched = true; }
-	    ALT_COMBOS(X)
-#undef X
-	}
-	if (!launched) {
-	    fill = 0;		/* the alternatives are not built for this shape: the default kernel runs */
 #define X(GG, WW, LL) if (sh.G == GG && sh.W == WW && sh.L == LL) e = launch_rx_t<GG, WW, LL, 0, 0>(sh, ce, lc, a, st);
-	    FAST_COMBOS(X)
+	FAST_COMBOS(X)
 #undef X
-	}
     } else {
 	e = launch_rx_t<32, 1, 1, 1, 0>(sh, ce, lc, a, st);
     }
     snprintf(ce->last_kernel, sizeof(ce->last_kernel),
 	    "k_rx<G=%d,W=%d,L=%d,mode=%d(%s),fill=%d,src=%s> threads=%d ring=%u smem=%zu blocks=%d", sh.G, sh.W, sh.L,
 	    sh.mode, sh.mode == 3 ? "prefix-table" : sh.mode == 2 ? "shared-segment" : sh.mode == 0 ? "per-candidate" : "generic",
-	    sh.mode == 0 ? fill : (sh.mode == 3 && elem == 4) ? ce->pfx_fill : 0, elem == 2 ? (sh.slide ? "s16,slide" : "s16") : (sh.slide ? "f32,slide" : "f32"),
+	    (sh.mode == 3 && elem == 4) ? ce->pfx_fill : 0, elem == 2 ? (sh.slide ? "s16,slide" : "s16") : (sh.slide ? "f32,slide" : "f32"),
 	    sh.wpb * 32, sh.ring, sh.smem, sh.blocks);
     if (e != cudaSuccess) {
 	fsk_b200_set_error("rx_batch launch (G=%d W=%d L=%d mode=%d ring=%u smem=%zu): %s", sh.G, sh.W,
@@ -2477,7 +2196,7 @@ static int rx_batch_host_common(CudaEngine *ce, const fsk_b200_geom *g, const fs
     size_t slab = ce->slab_bytes / (stride * (size_t)elem);
     if (slab < 1) slab = 1;
     if (slab > nstreams) slab = nstreams;
-    bool fused = elem == 2 && (stride & 7) == 0 && ce->fill == 0;
+    bool fused = elem == 2 && (stride & 7) == 0;
     int rc = 0;
 #define HOST_TRY(call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) { \
 	fsk_b200_set_error("%s: %s", #call, cudaGetErrorString(e_)); rc = -EIO; goto fail; } } while (0)

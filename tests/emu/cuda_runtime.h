@@ -352,7 +352,7 @@ template <int NKEEP>
 static inline void cp_async_wait() { emu::cp_async_wait_group(NKEEP); }
 static inline void ldgsts16(unsigned dst, const float *src) { emu::cp_async_16(dst, src, 16); }
 static inline void ldgsts16_zfill(unsigned dst, const float *src, unsigned valid) { emu::cp_async_16(dst, src, valid); }
-/* the TMA/mbarrier fill variant (FSK_B200_FILL=1) is not emulated */
+/* the TMA/mbarrier fill of the prefix-table kernel (FSK_B200_PFX_FILL=1) is not emulated */
 static inline void mbar_init(unsigned, unsigned) { emu::die("mbarrier path is not emulated"); }
 static inline void mbar_fence_init() {}
 static inline void mbar_arrive_expect_tx(unsigned, unsigned) { emu::die("mbarrier path is not emulated"); }

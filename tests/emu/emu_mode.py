@@ -26,7 +26,7 @@ def build():
 
 def activate():
     """Call before minimodem_b200 is imported.  FSK_EMU_LIB selects another emulation build
-    (e.g. one made with `make OUT=... BUILD=... EXTRA=-DFSK_STAGE_J=1` to try a compile-time variant)."""
+    (e.g. one made with `make OUT=... BUILD=... EXTRA=-DFSK_MULTI_MIN_N=64` to try a compile-time variant)."""
     global LIB
     if os.environ.get("FSK_EMU_LIB"):
         LIB = os.environ["FSK_EMU_LIB"]

@@ -81,7 +81,6 @@ FAST_SHAPES = [(4, 1, 1), (4, 2, 1), (4, 3, 1), (4, 4, 1), (4, 2, 2), (4, 4, 2),
                (32, 3, 4), (32, 4, 4)]
 S16_SHAPES = [(8, 1, 1), (8, 2, 1), (8, 3, 1), (8, 2, 2), (8, 3, 2), (8, 4, 2), (8, 4, 4),
               (16, 1, 2), (16, 2, 2), (16, 2, 4), (16, 3, 4), (16, 4, 4), (32, 2, 4)]
-ALT_SHAPES = [(8, 3, 2), (8, 2, 2), (16, 3, 4), (16, 2, 4), (16, 1, 2)]
 # shared-segment (mode 2): the launcher takes the (W, L) of the fewest period slots W G/L >= n + 1
 MULTI_ROWS = {(8, 2, 2): 7, (8, 3, 2): 10, (8, 4, 2): 14, (16, 2, 4): 6, (16, 3, 4): 11, (16, 4, 4): 13,
               (16, 3, 2): 20, (16, 4, 2): 28, (32, 2, 4): 14, (32, 3, 4): 19, (32, 4, 4): 27}
@@ -102,11 +101,6 @@ for (G, W, L) in FAST_SHAPES:
     RX_TABLE[(G, W, L, 0, 0, "f32")] = _fast(G, W, L, _n_for(G, W, L))
 for (G, W, L) in S16_SHAPES:
     RX_TABLE[(G, W, L, 0, 0, "s16")] = _fast(G, W, L, _n_for(G, W, L))
-for (G, W, L) in ALT_SHAPES:
-    for fill in (1, 3):
-        row = _fast(G, W, L, _n_for(G, W, L))
-        row["env"] = dict(FSK_B200_FILL=str(fill), FSK_B200_LANES=str(G), FSK_B200_SPLIT=str(L))
-        RX_TABLE[(G, W, L, 0, fill, "f32")] = row
 for (G, W, L), n in MULTI_ROWS.items():
     for src in ("f32", "s16"):
         RX_TABLE[(G, W, L, 2, 0, src)] = _multi(G, n)
@@ -154,15 +148,13 @@ def kernel_key(s):
 def launchable():
     """(rx keys, find-frame keys, tx keys) the kernel source can dispatch, from its combo lists"""
     src = open(KERNELS).read()
-    src = re.sub(r"#ifdef FSK_EXPERIMENT.*?#else", "", src, flags=re.S)
 
     def combos(name):
         m = re.search(r"#define %s\(X\)((?:[^\n]*\\\n)*[^\n]*)" % name, src)
         return [tuple(int(v) for v in t.split(",")) for t in re.findall(r"X\(([\d, ]+)\)", m.group(1))]
     fast, multi, s16 = combos("FAST_COMBOS"), combos("MULTI_COMBOS"), combos("S16_FAST_COMBOS")
-    alt, pfx = combos("ALT_COMBOS"), [w for (w,) in combos("PFX_SLOTS")]
+    pfx = [w for (w,) in combos("PFX_SLOTS")]
     rx = {(G, W, L, 0, 0, "f32") for G, W, L in fast} | {(G, W, L, 0, 0, "s16") for G, W, L in s16}
-    rx |= {(G, W, L, 0, f, "f32") for G, W, L in alt for f in (1, 3)}
     rx |= {(G, W, L, 2, 0, s) for G, W, L in multi for s in ("f32", "s16")}
     rx |= {(32, W, 1, 3, f, "f32") for W in pfx for f in (0, 1)} | {(32, W, 1, 3, 0, "s16") for W in pfx}
     rx |= {("generic", "f32"), ("generic", "s16")}
@@ -287,8 +279,7 @@ def compare_rx(case, recs, st, what):
 
 
 def _setenv(monkeypatch, env):
-    for k in ("FSK_B200_LANES", "FSK_B200_SPLIT", "FSK_B200_MULTI", "FSK_B200_PREFIX", "FSK_B200_PFX_FILL",
-              "FSK_B200_FILL"):
+    for k in ("FSK_B200_LANES", "FSK_B200_SPLIT", "FSK_B200_MULTI", "FSK_B200_PREFIX", "FSK_B200_PFX_FILL"):
         monkeypatch.delenv(k, raising=False)
     for k, v in env.items():
         monkeypatch.setenv(k, v)                # read when the engine is created
@@ -303,7 +294,7 @@ def _rows(streams, n, dtype, align=4):
 
 
 def _skip_tma(key):
-    if emulated() and len(key) == 6 and key[3] in (0, 3) and key[4] == 1:
+    if emulated() and len(key) == 6 and key[3] == 3 and key[4] == 1:
         pytest.skip("the host emulation does not model cp.async.bulk / mbarrier")
 
 

@@ -1090,23 +1090,20 @@ def test_per_bit_magnitudes_vs_oracle(mode, kw):
 
 
 # --------------------------------------------------------------------------
-# every shipped rx kernel variant on hardware: the cp.async fill with the shared-segment search
-# (default where the mode allows it) and with the per-candidate search, the TMA bulk fill
-# (cp.async.bulk + mbarrier, FILL=1) and the warp-synchronous loop (FILL=3), each against the
-# oracle on the same streams
+# every shipped rx kernel variant on hardware: the prefix-table search with the TMA bulk fill
+# (cp.async.bulk + mbarrier) and with the cp.async fill, the shared-segment search (default where
+# the mode allows it), alone and with the single-candidate fast path, and the per-candidate
+# search, each against the oracle on the same streams
 # --------------------------------------------------------------------------
-@pytest.mark.parametrize("variant", ["prefix", "prefix-cpasync", "multi", "multi-hybrid", "per-candidate", "tma-bulk", "warp-sync"])
+@pytest.mark.parametrize("variant", ["prefix", "prefix-cpasync", "multi", "multi-hybrid", "per-candidate"])
 @pytest.mark.parametrize("name", ["01-self-test-1200", "02-self-test-300", "small-rtty"])
 def test_rx_kernel_variants_agree_with_the_oracle(name, variant, monkeypatch):
     env = {"prefix": {"FSK_B200_PREFIX": "1"},
            "prefix-cpasync": {"FSK_B200_PREFIX": "1", "FSK_B200_PFX_FILL": "0"},      # (what int16 rows and the emulator run)
            "multi": {"FSK_B200_MULTI": "2", "FSK_B200_PREFIX": "0"},
            "multi-hybrid": {"FSK_B200_MULTI": "1", "FSK_B200_PREFIX": "0"},
-           "per-candidate": {"FSK_B200_MULTI": "0", "FSK_B200_PREFIX": "0"},
-           "tma-bulk": {"FSK_B200_FILL": "1"}, "warp-sync": {"FSK_B200_FILL": "3"}}[variant]
+           "per-candidate": {"FSK_B200_MULTI": "0", "FSK_B200_PREFIX": "0"}}[variant]
     import conftest
-    if variant == "tma-bulk" and conftest.EMU_DEVICE is not None:
-        pytest.skip("the host emulation does not model cp.async.bulk / mbarrier")
     for k, v in env.items():
         monkeypatch.setenv(k, v)                # read when the engine is created
     case = refcases.BY_NAME[name]
@@ -1125,8 +1122,6 @@ def test_rx_kernel_variants_agree_with_the_oracle(name, variant, monkeypatch):
         assert "shared-segment" in kern, kern
     elif variant == "per-candidate":
         assert "per-candidate" in kern, kern
-    else:
-        assert "fill=%s" % env["FSK_B200_FILL"] in kern, kern       # (FILL != 0 also keeps the prefix-table search out)
     for s, x in enumerate(streams):
         want = orc.rx_run(rx, x, literal=False)
         compare_frames(as_oracle_frames(recs[s]), want["frames"], "%s %s stream %d" % (name, variant, s))
