@@ -335,6 +335,34 @@ int fsk_b200_rx_batch_auto_s16(fsk_b200_engine *e, const int16_t *samples, size_
 	fsk_b200_auto_state *auto_states, uint32_t *rec_band, void *stream);
 uint32_t fsk_b200_auto_stream_window(const fsk_b200_rx_params *p);
 
+/* -M / -S per stream: every stream of one call on its own tone pair, the rest of the engine (band width,
+ * data rate, framing, thresholds, sample rate) shared.  Stream s gives the records and states that
+ * fsk_b200_rx_batch gives on an engine built for its pair (fsk_b200_rx_config_for_mode with overrides
+ * mark and space): the reference CLI run on that row with -M f_mark[s] -S f_space[s].
+ *
+ * fsk_b200_tone_bands: the bands of one pair on an engine of these params, with fsk_plan_new's float32
+ * arithmetic (src/fsk.c:52-57): b = (unsigned)((f + band_width/2) / band_width).  bands[0] = mark band,
+ * bands[1] = space band.  Returns 0, or -EINVAL where fsk_plan_new fails (a band >= nbands) and for a
+ * negative or non-finite frequency.  --inverted (src/minimodem.c:953-957) is the two tones swapped.  Host
+ * only; no device needed.
+ * fsk_b200_rx_batch_tones / _s16: fsk_b200_rx_batch / _s16 with tone_bands, device memory
+ * [nstreams][2] (mark band, space band) as fsk_b200_tone_bands gives them.  It is read at every call, so a
+ * stream may move to another pair between calls; a carrier loss keeps the pair.  A stream whose pair has a
+ * band >= nbands is skipped: it gets no records and its state is left untouched (the device cannot return
+ * an error per stream; fsk_b200_tone_bands rejects such a pair on the host).  The first call on an engine
+ * builds its unit-circle table (shared with fsk_b200_engine_set_auto_carrier) and synchronises the device.
+ * -ENOTSUP, with nothing launched, where the per-candidate rx kernel cannot take the mode (e.g. 0.5 baud) or
+ * has no per-stream-table build for its launch shape; -EINVAL for a NULL tone_bands and wherever
+ * fsk_b200_rx_batch / _s16 return it.  Runs the per-candidate kernel even where fsk_b200_rx_batch would
+ * pick the shared-segment or prefix-table one (DESIGN.md section 3). */
+int fsk_b200_tone_bands(const fsk_b200_rx_params *p, float f_mark, float f_space, uint32_t bands[2]);
+int fsk_b200_rx_batch_tones(fsk_b200_engine *e, const float *samples, size_t nstreams,
+	size_t stride, const uint32_t *nsamples, uint32_t nsamples_all, const uint32_t *tone_bands,
+	fsk_b200_frame *frames, uint32_t max_frames, fsk_b200_stream_state *states, void *stream);
+int fsk_b200_rx_batch_tones_s16(fsk_b200_engine *e, const int16_t *samples, size_t nstreams,
+	size_t stride, const uint32_t *nsamples, uint32_t nsamples_all, const uint32_t *tone_bands,
+	fsk_b200_frame *frames, uint32_t max_frames, fsk_b200_stream_state *states, void *stream);
+
 /* N2 -- 16-bit PCM ingest (the reference transmitter's default sample format, read back by
  * its rx as float = short / 32768: src/simpleaudio-sndfile.c:43-57, src/minimodem.c:786-788).
  * fsk_b200_s16_to_f32: device conversion (exact: a power-of-two scale), asynchronous on `stream`.
@@ -521,7 +549,8 @@ int fsk_b200_tx_text_batch(fsk_b200_tx_engine *te, const uint8_t *text, size_t n
 
 /* Diagnostics: which kernel instance the engine's latest fsk_b200_rx_batch or fsk_b200_find_frame_batch
  * launched ("k_rx<G=8,W=3,L=2,mode=2(shared-segment),fill=0,src=f32> threads=64 ring=640 smem=23232
- * blocks=8192", "k_find_frame<G=8,W=2,L=1,mode=0(per-candidate)> ..."; "" before the first launch).  `fill`
+ * blocks=8192", "k_find_frame<G=8,W=2,L=1,mode=0(per-candidate)> ..."; "" before the first launch);
+ * k_rx_auto<...> and k_rx_tones<...> for fsk_b200_rx_batch_auto and fsk_b200_rx_batch_tones.  `fill`
  * is 1 for the prefix-table kernel's TMA bulk fill (float rows, FSK_B200_PFX_FILL not 0) and 0 otherwise. */
 const char *fsk_b200_engine_last_kernel(const fsk_b200_engine *e);
 

@@ -125,6 +125,7 @@ EXPORTS = [
     "fsk_b200_tx_max_samples", "fsk_b200_tx_text_batch",
     "fsk_b200_rx_config_autodetect_shift", "fsk_b200_engine_set_auto_carrier", "fsk_b200_rx_batch_auto",
     "fsk_b200_rx_batch_auto_s16", "fsk_b200_auto_stream_window",
+    "fsk_b200_tone_bands", "fsk_b200_rx_batch_tones", "fsk_b200_rx_batch_tones_s16",
 ]
 
 _lib = None
@@ -260,6 +261,13 @@ def lib():
     L.fsk_b200_rx_batch_auto_s16.restype = C.c_int
     L.fsk_b200_auto_stream_window.argtypes = [C.POINTER(RxParams)]
     L.fsk_b200_auto_stream_window.restype = C.c_uint32
+    L.fsk_b200_tone_bands.argtypes = [C.POINTER(RxParams), C.c_float, C.c_float, C.POINTER(C.c_uint32)]
+    L.fsk_b200_tone_bands.restype = C.c_int
+    L.fsk_b200_rx_batch_tones.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t, u32p, C.c_uint32, u32p,
+                                          C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p]
+    L.fsk_b200_rx_batch_tones.restype = C.c_int
+    L.fsk_b200_rx_batch_tones_s16.argtypes = list(L.fsk_b200_rx_batch_tones.argtypes)
+    L.fsk_b200_rx_batch_tones_s16.restype = C.c_int
     L.fsk_b200_version.restype = C.c_char_p
     L.fsk_b200_launch_count.restype = C.c_ulonglong
     L.fsk_b200_last_error.restype = C.c_char_p
@@ -310,6 +318,17 @@ def rx_params(cfg):
 
 def max_frames(params, nsamples):
     return int(lib().fsk_b200_max_frames(C.byref(params), int(nsamples)))
+
+
+def tone_bands(params, f_mark, f_space):
+    """fsk_b200_tone_bands: the (mark band, space band) of one tone pair on an engine of `params`, with
+    fsk_plan_new's float32 arithmetic.  Raises ValueError where fsk_plan_new fails and for negative or
+    non-finite frequencies."""
+    b = (C.c_uint32 * 2)()
+    rc = lib().fsk_b200_tone_bands(C.byref(params), float(f_mark), float(f_space), b)
+    if rc:
+        raise ValueError("fsk_b200_tone_bands (%d): %s" % (rc, lib().fsk_b200_last_error().decode(errors="replace")))
+    return int(b[0]), int(b[1])
 
 
 def frame_databits(params, rec):
@@ -574,6 +593,50 @@ class RxEngine:
     def auto_stream_window(self):
         """fsk_b200_auto_stream_window: the live-stream holdback with auto-carrier."""
         return int(lib().fsk_b200_auto_stream_window(C.byref(self.params)))
+
+    def tone_bands(self, marks_hz, spaces_hz, inverted=False, device=None):
+        """The tone_bands argument of rx_batch_tones: an int32 tensor [n, 2] of (mark band, space band), one
+        row per stream, for the CLI's -M marks_hz[s] -S spaces_hz[s] (scalars or sequences, broadcast);
+        inverted (a bool or one per stream) swaps a stream's two tones, as --inverted does.  Every distinct
+        pair goes through fsk_b200_tone_bands once; an invalid pair raises ValueError.  device: where the
+        tensor goes (default cuda:0)."""
+        torch = _torch()
+        m, s, inv = np.broadcast_arrays(np.asarray(marks_hz, np.float32), np.asarray(spaces_hz, np.float32),
+                                        np.asarray(inverted, bool))
+        m, s, inv = m.reshape(-1), s.reshape(-1), inv.reshape(-1)
+        mark, space = np.where(inv, s, m), np.where(inv, m, s)
+        known = {}
+        out = np.zeros((mark.size, 2), np.int32)
+        for i, pair in enumerate(zip(mark.tolist(), space.tolist())):
+            if pair not in known:
+                known[pair] = tone_bands(self.params, *pair)
+            out[i] = known[pair]
+        return torch.from_numpy(out).to(device if device is not None else torch.device("cuda:0"))
+
+    def rx_batch_tones(self, samples, tone_bands, nsamples=None, max_frames=None, frames=None, states=None,
+                       nsamples_each=None, stream=None):
+        """rx_batch with a tone pair per stream (fsk_b200_rx_batch_tones / _s16): row s is decoded as the
+        CLI would with its own -M / -S.  samples: [nstreams, stride] float32 or int16 CUDA tensor;
+        tone_bands: int32 CUDA tensor [nstreams, 2] (tone_bands()), read at every call.  A row whose pair
+        has a band >= nbands gets no records and keeps its state.  Returns (frames, states)."""
+        torch = _torch()
+        assert samples.is_cuda and samples.dtype in (torch.float32, torch.int16) and samples.is_contiguous()
+        nstreams, stride = samples.shape
+        assert (tone_bands.is_cuda and tone_bands.dtype == torch.int32 and tone_bands.is_contiguous()
+                and tuple(tone_bands.shape) == (nstreams, 2))
+        n_all = int(nsamples if nsamples is not None else stride)
+        if max_frames is None:
+            max_frames = self.max_frames(n_all)
+        if frames is None:
+            frames = torch.empty((nstreams, max_frames, 5), dtype=torch.int32, device=samples.device)
+        if states is None:
+            states = torch.zeros((nstreams, STATE_WORDS), dtype=torch.int32, device=samples.device)
+        fn = lib().fsk_b200_rx_batch_tones if samples.dtype == torch.float32 else lib().fsk_b200_rx_batch_tones_s16
+        rc = fn(self._e, _ptr(samples), nstreams, stride, _ptr(nsamples_each), n_all, _ptr(tone_bands),
+                _ptr(frames), max_frames, _ptr(states), _stream_handle(stream))
+        if rc:
+            _err("fsk_b200_rx_batch_tones", rc)
+        return frames, states
 
     def set_holdback(self, nsamples):
         """fsk_b200_engine_set_holdback: searches start only with this many samples left (0 = the

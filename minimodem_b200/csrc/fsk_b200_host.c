@@ -820,6 +820,78 @@ int fsk_b200_rx_batch_auto_s16(fsk_b200_engine *e, const int16_t *samples, size_
 	    auto_states, rec_band, stream);
 }
 
+/* ---- -M / -S per stream ------------------------------------------------------------ */
+
+int fsk_b200_tone_bands(const fsk_b200_rx_params *p, float f_mark, float f_space, uint32_t bands[2])
+{
+    if (!p || !bands || !(p->band_width > 0)) {
+	fsk_b200_set_error("tone_bands: NULL argument or no band width");
+	return -EINVAL;
+    }
+    /* a negative or non-finite tone would make the cast below undefined */
+    if (!isfinite(f_mark) || !isfinite(f_space) || f_mark < 0.0f || f_space < 0.0f) {
+	fsk_b200_set_error("tone_bands: tones must be finite and non-negative (%g, %g)", (double)f_mark,
+		(double)f_space);
+	return -EINVAL;
+    }
+    /* derive_bands: float32 throughout; (unsigned)q >= nbands exactly when q >= nbands, nbands being whole */
+    const float bw = p->band_width, half = bw / 2.0f;
+    const float qm = (f_mark + half) / bw, qs = (f_space + half) / bw;
+    if (!(qm < (float)p->nbands) || !(qs < (float)p->nbands)) {
+	fsk_b200_set_error("tone_bands: %g Hz or %g Hz lies outside the %u bands of %g Hz", (double)f_mark,
+		(double)f_space, p->nbands, (double)bw);
+	return -EINVAL;
+    }
+    bands[0] = (unsigned int)qm;
+    bands[1] = (unsigned int)qs;
+    return 0;
+}
+
+static int rx_batch_tones_any(fsk_b200_engine *e, const void *samples, int elem, size_t nstreams, size_t stride,
+	const uint32_t *nsamples, uint32_t nsamples_all, const uint32_t *tone_bands, fsk_b200_frame *frames,
+	uint32_t max_frames, fsk_b200_stream_state *states, void *stream)
+{
+    if (!e || !tone_bands) {
+	fsk_b200_set_error("rx_batch_tones: NULL engine or tone_bands");
+	return -EINVAL;
+    }
+    if (nstreams == 0)
+	return 0;
+    const size_t align = elem == 2 ? 7 : 3;
+    if (!samples || ((uintptr_t)samples & 15) || (stride & align)) {
+	fsk_b200_set_error("rx_batch_tones: samples must be 16-byte aligned and the stride a multiple of %zu samples",
+		align + 1);
+	return -EINVAL;
+    }
+    if (!frames || !states || max_frames == 0) {
+	fsk_b200_set_error("rx_batch_tones: NULL argument");
+	return -EINVAL;
+    }
+    if ((!nsamples && (size_t)nsamples_all > stride) || nstreams > 0x7fffffffu) {
+	fsk_b200_set_error("rx_batch_tones: nsamples_all (%u) exceeds the row stride (%zu), or too many streams",
+		nsamples_all, stride);
+	return -EINVAL;
+    }
+    return fsk_b200_cuda_rx_batch_tones(e->ce, &e->geom, &e->loopc, e->params.fftsize, e->params.nbands, samples,
+	    elem, nstreams, stride, nsamples, nsamples_all, tone_bands, frames, max_frames, states, stream);
+}
+
+int fsk_b200_rx_batch_tones(fsk_b200_engine *e, const float *samples, size_t nstreams, size_t stride,
+	const uint32_t *nsamples, uint32_t nsamples_all, const uint32_t *tone_bands, fsk_b200_frame *frames,
+	uint32_t max_frames, fsk_b200_stream_state *states, void *stream)
+{
+    return rx_batch_tones_any(e, samples, 4, nstreams, stride, nsamples, nsamples_all, tone_bands, frames,
+	    max_frames, states, stream);
+}
+
+int fsk_b200_rx_batch_tones_s16(fsk_b200_engine *e, const int16_t *samples, size_t nstreams, size_t stride,
+	const uint32_t *nsamples, uint32_t nsamples_all, const uint32_t *tone_bands, fsk_b200_frame *frames,
+	uint32_t max_frames, fsk_b200_stream_state *states, void *stream)
+{
+    return rx_batch_tones_any(e, samples, 2, nstreams, stride, nsamples, nsamples_all, tone_bands, frames,
+	    max_frames, states, stream);
+}
+
 /* ---- live streams ------------------------------------------------------------ */
 
 uint32_t fsk_b200_stream_window(const fsk_b200_rx_params *p)

@@ -181,7 +181,8 @@ __device__ __forceinline__ float band_mag(const T *__restrict__ x, unsigned nsam
     return sqrtf(fr * fr + fi * fi) * magscalar;
 }
 
-/* --auto-carrier (src/minimodem.c:1179-1220) in the per-candidate rx kernel (AUTO = 1) */
+/* --auto-carrier (src/minimodem.c:1179-1220) in the per-candidate rx kernel (AUTO = 1); its table fields
+ * also serve a fixed pair per stream (AUTO = 2) */
 struct AutoArgs {
     fsk_b200_auto_state *states;
     uint32_t *rec_band;		/* optional: [nstreams][max_frames], the mark band of every record */
@@ -192,6 +193,7 @@ struct AutoArgs {
     unsigned fftsize, nbands;
     unsigned half_ring;		/* samplebuf_size / 2: the refill of the virtual ring count */
     unsigned expect_nsamples;	/* the loop's own stop rule; lc.expect_nsamples above it is a live stream's holdback */
+    const uint32_t *tones;	/* AUTO 2: [nstreams][2], each stream's (mark band, space band) */
 };
 
 /* fsk_detect_carrier (src/fsk.c:543-581) on one window, by the G lanes of a group: lane g takes the
@@ -321,7 +323,10 @@ k_find_frame(const __grid_constant__ fsk_b200_geom geo, const float4 *__restrict
  * reference's float = short / 32768 inside the ring fill: 2 bytes per sample of HBM traffic.
  * AUTO 1 (MODE 0, FILL 0 only): --auto-carrier.  Each stream has its own tone table in shared memory
  * behind the mbarriers (geo.tw_entries float4 per slot, filled from au.unit when a band is accepted),
- * and scans for a carrier band over its virtual ring count while it has none (DESIGN.md 5). */
+ * and scans for a carrier band over its virtual ring count while it has none (DESIGN.md 5).
+ * AUTO 2 (same shapes): -M / -S per stream.  The same per-stream table, filled once at the start of each
+ * stream from its pair in au.tones; no scan, no auto state, and a carrier loss keeps the pair.  A stream
+ * whose pair has a band >= au.nbands is skipped: no records, its state untouched. */
 template <int G, int W, int L, int MODE, int FILL, int SRC = 0, int AUTO = 0>
 __global__ void __launch_bounds__(MODE == 3 ? FSK_PFX_MAXTHREADS : FSK_MAXTHREADS,
 	MODE == 3 ? 1 : (MODE == 2 && G >= 16) ? 3 : FSK_MINBLOCKS)
@@ -377,12 +382,11 @@ k_rx(const __grid_constant__ fsk_b200_geom geo, const __grid_constant__ fsk_b200
 	unsigned done = 0;
 	unsigned ncand = 0, nsearch = 0;	/* statistics: candidates analysed, searches run */
 	bool mhint = st.reserved != 0u;		/* MODE 2: the latest coarse search needed more than its first candidate */
-	/* AUTO: the accepted mark band (0: none, :1180) and the virtual ring count */
-	unsigned band = AUTO ? au.states[s].carrier_band : 0u, vring = AUTO ? au.states[s].v : 0u;
+	/* AUTO 1: the accepted mark band (0: none, :1180) and the virtual ring count */
+	unsigned band = AUTO == 1 ? au.states[s].carrier_band : 0u, vring = AUTO == 1 ? au.states[s].v : 0u;
 	/* fsk_set_tones_by_bandshift (src/fsk.c:585-598) for this stream's table: entry e of the tone b is
 	 * the unit-circle entry (b * e) mod fftsize, the value fsk_b200_cuda_set_table computes for it */
-	auto set_tones = [&](unsigned bm) {
-	    const unsigned bsp = (unsigned)((int)bm + au.b_shift);
+	auto set_tones = [&](unsigned bm, unsigned bsp) {
 	    __syncwarp(gmask);
 	    for (unsigned e = g; e < geo.tw_entries; e += G) {
 		const float2 um = au.unit[(unsigned)(((unsigned long long)bm * e) % au.fftsize)];
@@ -391,8 +395,14 @@ k_rx(const __grid_constant__ fsk_b200_geom geo, const __grid_constant__ fsk_b200
 	    }
 	    __syncwarp(gmask);
 	};
-	if (AUTO && band)
-	    set_tones(band);
+	if (AUTO == 1 && band)
+	    set_tones(band, (unsigned)((int)band + au.b_shift));
+	if (AUTO == 2) {
+	    const unsigned bm = au.tones[2u * s], bsp = au.tones[2u * s + 1u];
+	    if (bm >= au.nbands || bsp >= au.nbands)
+		continue;				/* no such pair (fsk_plan_new fails): skipped */
+	    set_tones(bm, bsp);
+	}
 
 	/* ring bookkeeping (MODE 0): ring offset of `pos`, and the absolute index up to
 	 * which the ring content has been REQUESTED (copies issued or zeros stored) */
@@ -502,7 +512,7 @@ k_rx(const __grid_constant__ fsk_b200_geom geo, const __grid_constant__ fsk_b200
 	for (;;) {
 	    if (pos >= n) { done = 1; break; }			/* :1176 */
 	    const unsigned remaining = n - pos;
-	    if (AUTO) {
+	    if (AUTO == 1) {
 		/* a live stream's holdback (lc.expect_nsamples raised above the loop's own rule) stops the
 		 * loop before the scan: the refill below must not see where the stream was cut */
 		if (lc.expect_nsamples > au.expect_nsamples && remaining < lc.expect_nsamples) { done = 1; break; }
@@ -526,7 +536,7 @@ k_rx(const __grid_constant__ fsk_b200_geom geo, const __grid_constant__ fsk_b200
 		    const int b_space = found + au.b_shift;
 		    if (found >= 0 && b_space >= 1 && b_space < (int)au.nbands) {
 			band = (unsigned)found;
-			set_tones(band);			/* and search at the ring start */
+			set_tones(band, (unsigned)b_space);	/* and search at the ring start */
 		    } else {
 			const unsigned adv = min((unsigned)((float)i + sf), vring);
 			pos += adv;
@@ -734,7 +744,7 @@ k_rx(const __grid_constant__ fsk_b200_geom geo, const __grid_constant__ fsk_b200
 			if (g == 0)
 			    store_frame(out + nframes, carrier_nsamples, confidence_total,
 				    amplitude_total, FSK_B200_FRAME_REPORT);
-			if (AUTO && g == 0 && au.rec_band)
+			if (AUTO == 1 && g == 0 && au.rec_band)
 			    au.rec_band[(size_t)s * a.max_frames + nframes] = band;
 			nframes++;
 			carrier = 0;				/* :1303-1308 */
@@ -744,8 +754,8 @@ k_rx(const __grid_constant__ fsk_b200_geom geo, const __grid_constant__ fsk_b200
 			nframes_decoded = 0;
 			track_amplitude = 0.f;
 		    }
-		    if (AUTO)
-			band = 0;				/* :1297 */
+		    if (AUTO == 1)
+			band = 0;				/* :1297 (AUTO 2 keeps its pair) */
 		}
 		advance = try_max;				/* :1318 */
 	    } else {
@@ -795,14 +805,14 @@ k_rx(const __grid_constant__ fsk_b200_geom geo, const __grid_constant__ fsk_b200
 		noconfidence = 0;
 		if (g == 0)
 		    store_frame(out + nframes, bits, confidence, amplitude, frame_start | acquired);
-		if (AUTO && g == 0 && au.rec_band)
+		if (AUTO == 1 && g == 0 && au.rec_band)
 		    au.rec_band[(size_t)s * a.max_frames + nframes] = band;
 		nframes++;
 		advance = frame_start + lc.frame_nsamples - lc.nsamples_overscan;	/* :1407 */
 	    }
 	    if (advance > remaining) { done = 1; break; }	/* :1151 */
 	    pos += advance;
-	    if (AUTO)
+	    if (AUTO == 1)
 		vring = advance >= vring ? 0u : vring - advance;
 	    if (MODE != 1) {
 		pos_off = ring_wrap(pos_off + advance, R);	/* advance < R by construction */
@@ -838,7 +848,7 @@ k_rx(const __grid_constant__ fsk_b200_geom geo, const __grid_constant__ fsk_b200
 	    st.stat_searches += nsearch;
 	    st.reserved = mhint ? 1u : 0u;
 	    a.states[s] = st;
-	    if (AUTO) {
+	    if (AUTO == 1) {
 		au.states[s].carrier_band = band;
 		au.states[s].v = vring;
 	    }
@@ -2175,6 +2185,67 @@ extern "C" int fsk_b200_cuda_rx_batch_auto(void *p, const fsk_b200_geom *g, cons
 	    sh.wpb * 32, sh.ring, sh.smem, sh.blocks);
     if (e != cudaSuccess) {
 	fsk_b200_set_error("rx_batch_auto launch (G=%d W=%d L=%d ring=%u smem=%zu): %s", sh.G, sh.W, sh.L, sh.ring,
+		sh.smem, cudaGetErrorString(e));
+	return -EIO;
+    }
+    return 0;
+}
+
+/* -M / -S per stream: the AUTO_COMBOS shapes with AUTO 2, elem 4: float32 rows, elem 2: int16 rows.  The
+ * engine's unit-circle table is built on first use (synchronous).  -ENOTSUP, with nothing launched or built,
+ * where the per-candidate kernel cannot take the mode or the shape has no build of it. */
+extern "C" int fsk_b200_cuda_rx_batch_tones(void *p, const fsk_b200_geom *g, const fsk_b200_loopc *lc, int fftsize,
+	unsigned nbands, const void *samples, int elem, size_t nstreams, size_t stride, const uint32_t *nsamples,
+	uint32_t nsamples_all, const uint32_t *tone_bands, fsk_b200_frame *frames, uint32_t max_frames,
+	fsk_b200_stream_state *states, void *stream)
+{
+    CudaEngine *ce = (CudaEngine *)p;
+    if (engine_device_check(ce, "rx_batch_tones"))
+	return -EINVAL;
+    Shape sh;
+    const unsigned tmax = lc->try_max_nocarrier > lc->try_max_carrier ? lc->try_max_nocarrier : lc->try_max_carrier;
+    const unsigned max_advance = tmax - 1u + lc->frame_nsamples;
+    pick_shape(ce, g, tmax - 1u + g->span, max_advance, nstreams, &sh, lc, true);
+    fsk_b200_loopc lc_launch = *lc;
+    lc_launch.slide = sh.slide;
+    bool built = false;
+    if (sh.mode == 0) {
+#define X(GG, WW, LL) if (sh.G == GG && sh.W == WW && sh.L == LL) built = true;
+	AUTO_COMBOS(X)
+#undef X
+    }
+    if (!built) {
+	fsk_b200_set_error("rx_batch_tones: no per-stream tone build of the per-candidate kernel for this mode "
+		"(launch shape G=%d W=%d L=%d mode=%d)", sh.G, sh.W, sh.L, sh.mode);
+	return -ENOTSUP;
+    }
+    const int rc = fsk_b200_cuda_set_unit_table(ce, fftsize);
+    if (rc)
+	return rc;
+    const RxArgs a = { elem == 4 ? (const float *)samples : NULL, elem == 2 ? (const int16_t *)samples : NULL,
+	(unsigned)nstreams, stride, nsamples, nsamples_all, frames, max_frames, states };
+    AutoArgs au = AutoArgs();
+    au.unit = ce->d_unit;
+    au.fftsize = (unsigned)fftsize;
+    au.nbands = nbands;
+    au.tones = tone_bands;
+    cudaStream_t st = (cudaStream_t)stream;
+    cudaError_t e = cudaErrorInvalidValue;
+    if (elem == 2) {
+#define X(GG, WW, LL) if (sh.G == GG && sh.W == WW && sh.L == LL) e = launch_rx_t<GG, WW, LL, 0, 0, 1, 2>(sh, ce, &lc_launch, a, st, au);
+	AUTO_COMBOS(X)
+#undef X
+    } else {
+#define X(GG, WW, LL) if (sh.G == GG && sh.W == WW && sh.L == LL) e = launch_rx_t<GG, WW, LL, 0, 0, 0, 2>(sh, ce, &lc_launch, a, st, au);
+	AUTO_COMBOS(X)
+#undef X
+    }
+    snprintf(ce->last_kernel, sizeof(ce->last_kernel),
+	    "k_rx_tones<G=%d,W=%d,L=%d,mode=0(per-candidate),fill=0,src=%s> threads=%d ring=%u smem=%zu blocks=%d",
+	    sh.G, sh.W, sh.L, elem == 2 ? (sh.slide ? "s16,slide" : "s16") : (sh.slide ? "f32,slide" : "f32"),
+	    sh.wpb * 32, sh.ring, sh.smem, sh.blocks);
+    if (e != cudaSuccess) {
+	fsk_b200_set_error("rx_batch_tones launch (G=%d W=%d L=%d ring=%u smem=%zu): %s", sh.G, sh.W, sh.L, sh.ring,
 		sh.smem, cudaGetErrorString(e));
 	return -EIO;
     }

@@ -14,6 +14,9 @@ the stream was cut into chunks (tests/test_gpu_parity.py::test_live_receiver_*).
 stays on the device; there is no per-stream work on the host.  With auto_carrier=threshold (0.001 is
 the CLI's -a) every stream finds its own tone pair: fsk_b200_rx_batch_auto with the per-stream
 auto states and the auto holdback (fsk_b200_auto_stream_window) in place of fsk_b200_rx_batch.
+With tones=bands (an int32 tensor [nstreams, 2] from RxEngine.tone_bands on an engine of the same mode,
+or rx.engine.tone_bands) every stream keeps its own -M / -S pair: fsk_b200_rx_batch_tones with the
+ordinary holdback; tones and auto_carrier exclude each other.
 
     tx = LiveTransmitter("rtty", sample_rate=8000, nstreams=4096, max_text=64)
     for text, lengths in source:                  # uint8 CUDA tensor [nstreams, <= max_text], int32 [nstreams]
@@ -31,8 +34,10 @@ from . import api
 
 class LiveReceiver:
     def __init__(self, baudmode, sample_rate=48000, nstreams=1, max_chunk=4800, device=None,
-                 binary_output=False, auto_carrier=None, **overrides):
+                 binary_output=False, auto_carrier=None, tones=None, **overrides):
         torch = api._torch()
+        if auto_carrier is not None and tones is not None:
+            raise ValueError("LiveReceiver: auto_carrier and tones exclude each other")
         self.engine = api.RxEngine.for_mode(baudmode, sample_rate, **overrides)
         self.kind = api.decoder_for_mode(baudmode, self.engine.params.n_data_bits, binary_output)
         self.auto = auto_carrier is not None
@@ -55,10 +60,18 @@ class LiveReceiver:
         self.dropped = z((self.nstreams,), torch.int32)
         self._empty = z((self.nstreams, 4), torch.float32)
         self.auto_states = z((self.nstreams, api.AUTO_STATE_BYTES), torch.uint8) if self.auto else None
+        self.tones = None
+        if tones is not None:
+            assert tuple(tones.shape) == (self.nstreams, 2)
+            self.tones = tones.to(device=dev, dtype=torch.int32).contiguous()
 
     def _step(self, chunk, lengths):
         api.stream_push(self.rows, self.fill, self.states, chunk, lengths, dropped=self.dropped)
-        if self.auto:
+        if self.tones is not None:
+            frames, self.states = self.engine.rx_batch_tones(
+                self.rows, self.tones, nsamples=self.stride, nsamples_each=self.fill, max_frames=self.max_frames,
+                states=self.states)
+        elif self.auto:
             frames, self.states, self.auto_states = self.engine.rx_batch_auto(
                 self.rows, nsamples=self.stride, nsamples_each=self.fill, max_frames=self.max_frames,
                 states=self.states, auto_states=self.auto_states)
