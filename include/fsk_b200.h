@@ -204,8 +204,22 @@ fsk_b200_engine *fsk_b200_engine_new(const fsk_b200_rx_params *params);
 void fsk_b200_engine_destroy(fsk_b200_engine *e);
 const fsk_b200_rx_params *fsk_b200_engine_params(const fsk_b200_engine *e);
 
-/* Tuning knobs (0 = engine default): lanes per stream (1..32, power of two),
- * warps per block, ring floats per stream (power of two). */
+/* Tuning knobs of the rx launches (0 = engine default; the FSK_B200_LANES /
+ * _WPB / _RING variables set the same at engine creation).  -EINVAL, with the
+ * previous tuning kept, unless lanes_per_stream is 0, 4, 8, 16 or 32,
+ * warps_per_block is 0..4 and ring_floats is 0 or at least 128.
+ * - ring_floats: the shared-memory ring of each stream, rounded up to whole
+ *   128-float blocks and raised to the mode's minimum.  Beyond the minimum it
+ *   buys look-ahead: the next iteration's samples are copied while the current
+ *   one is searched (last_kernel()'s lookahead=, at most the largest advance).
+ * - These are requests.  The launcher lowers the warps per block first, then
+ *   raises the lanes per stream, until the block fits in shared memory, and
+ *   takes the generic kernel (no ring) if not even one 32-lane stream fits.
+ *   With lanes_per_stream 0 the lane count follows the streams that fit per SM,
+ *   so a deeper ring can raise it.  The prefix-table kernel picks its own warps
+ *   per block unless FSK_B200_PREFIX=1.  last_kernel() shows what ran.
+ * At a fixed lane count and window split the records do not depend on the
+ * ring or the warps per block. */
 int fsk_b200_engine_tune(fsk_b200_engine *e, int lanes_per_stream, int warps_per_block,
 	int ring_floats);
 

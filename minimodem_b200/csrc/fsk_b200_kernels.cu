@@ -2066,10 +2066,10 @@ static int rx_batch_any(CudaEngine *ce, const fsk_b200_geom *g, const fsk_b200_l
 	e = launch_rx_t<32, 1, 1, 1, 0>(sh, ce, lc, a, st);
     }
     snprintf(ce->last_kernel, sizeof(ce->last_kernel),
-	    "k_rx<G=%d,W=%d,L=%d,mode=%d(%s),fill=%d,src=%s> threads=%d ring=%u smem=%zu blocks=%d", sh.G, sh.W, sh.L,
-	    sh.mode, sh.mode == 3 ? "prefix-table" : sh.mode == 2 ? "shared-segment" : sh.mode == 0 ? "per-candidate" : "generic",
+	    "k_rx<G=%d,W=%d,L=%d,mode=%d(%s),fill=%d,src=%s> threads=%d ring=%u smem=%zu blocks=%d lookahead=%u",
+	    sh.G, sh.W, sh.L, sh.mode, sh.mode == 3 ? "prefix-table" : sh.mode == 2 ? "shared-segment" : sh.mode == 0 ? "per-candidate" : "generic",
 	    (sh.mode == 3 && elem == 4) ? ce->pfx_fill : 0, elem == 2 ? (sh.slide ? "s16,slide" : "s16") : (sh.slide ? "f32,slide" : "f32"),
-	    sh.wpb * 32, sh.ring, sh.smem, sh.blocks);
+	    sh.wpb * 32, sh.ring, sh.smem, sh.blocks, sh.lookahead);
     if (e != cudaSuccess) {
 	fsk_b200_set_error("rx_batch launch (G=%d W=%d L=%d mode=%d ring=%u smem=%zu): %s", sh.G, sh.W,
 		sh.L, sh.mode, sh.ring, sh.smem, cudaGetErrorString(e));
@@ -2180,9 +2180,9 @@ extern "C" int fsk_b200_cuda_rx_batch_auto(void *p, const fsk_b200_geom *g, cons
 	return -ENOTSUP;
     }
     snprintf(ce->last_kernel, sizeof(ce->last_kernel),
-	    "k_rx_auto<G=%d,W=%d,L=%d,mode=0(per-candidate),fill=0,src=%s> threads=%d ring=%u smem=%zu blocks=%d",
+	    "k_rx_auto<G=%d,W=%d,L=%d,mode=0(per-candidate),fill=0,src=%s> threads=%d ring=%u smem=%zu blocks=%d lookahead=%u",
 	    sh.G, sh.W, sh.L, elem == 2 ? (sh.slide ? "s16,slide" : "s16") : (sh.slide ? "f32,slide" : "f32"),
-	    sh.wpb * 32, sh.ring, sh.smem, sh.blocks);
+	    sh.wpb * 32, sh.ring, sh.smem, sh.blocks, sh.lookahead);
     if (e != cudaSuccess) {
 	fsk_b200_set_error("rx_batch_auto launch (G=%d W=%d L=%d ring=%u smem=%zu): %s", sh.G, sh.W, sh.L, sh.ring,
 		sh.smem, cudaGetErrorString(e));
@@ -2241,9 +2241,9 @@ extern "C" int fsk_b200_cuda_rx_batch_tones(void *p, const fsk_b200_geom *g, con
 #undef X
     }
     snprintf(ce->last_kernel, sizeof(ce->last_kernel),
-	    "k_rx_tones<G=%d,W=%d,L=%d,mode=0(per-candidate),fill=0,src=%s> threads=%d ring=%u smem=%zu blocks=%d",
+	    "k_rx_tones<G=%d,W=%d,L=%d,mode=0(per-candidate),fill=0,src=%s> threads=%d ring=%u smem=%zu blocks=%d lookahead=%u",
 	    sh.G, sh.W, sh.L, elem == 2 ? (sh.slide ? "s16,slide" : "s16") : (sh.slide ? "f32,slide" : "f32"),
-	    sh.wpb * 32, sh.ring, sh.smem, sh.blocks);
+	    sh.wpb * 32, sh.ring, sh.smem, sh.blocks, sh.lookahead);
     if (e != cudaSuccess) {
 	fsk_b200_set_error("rx_batch_tones launch (G=%d W=%d L=%d ring=%u smem=%zu): %s", sh.G, sh.W, sh.L, sh.ring,
 		sh.smem, cudaGetErrorString(e));

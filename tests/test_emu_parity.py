@@ -59,6 +59,15 @@ def test_every_instantiation_on_the_emulated_kernels_with_perturbed_units():
     assert " passed" in tail and "failed" not in tail
 
 
+@pytest.mark.parametrize("async_mode", ["eager", "late"])
+def test_launch_shapes_on_the_emulated_kernels(async_mode):
+    """tests/test_gpu_launch_shapes.py: ring depths, warps per block and neighbours leave every record and
+    state as it is (the TMA bulk fill excepted: not emulated).  With copies landing at issue, a look-ahead
+    copy that overwrote a window still being read would show."""
+    tail = run_emulated("", async_mode, 1800, module="test_gpu_launch_shapes.py")
+    assert " passed" in tail and "failed" not in tail
+
+
 def test_the_emulator_itself():
     """tests/emu/selftest.cpp: hand-verifiable kernels.  Group-masked shuffles / votes with
     divergent trip counts, block barriers and dynamic shared memory give CUDA's results; cp.async
