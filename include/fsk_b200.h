@@ -377,6 +377,39 @@ int fsk_b200_rx_batch_tones_s16(fsk_b200_engine *e, const int16_t *samples, size
 	size_t stride, const uint32_t *nsamples, uint32_t nsamples_all, const uint32_t *tone_bands,
 	fsk_b200_frame *frames, uint32_t max_frames, fsk_b200_stream_state *states, void *stream);
 
+/* Tone-pair channels over shared rows: several -M / -S pairs decoded from one recording without copying
+ * it (both directions of a full-duplex line, k signals in one passband).  A channel is a (row, tone pair)
+ * combination; every row carries k = channels_per_row channels, and channel c = r*k + j reads row r.
+ * Rows (samples, nsamples [nrows]) are indexed as in fsk_b200_rx_batch; tone_bands [nrows*k][2], frames
+ * [nrows*k][max_frames] and states [nrows*k] are indexed by channel.  Channel (r, j) gives the records and
+ * states that fsk_b200_rx_batch_tones gives on a copy of row r with that pair: the reference CLI run on
+ * row r with -M / -S of that pair.  A row that needs fewer channels pads the rest with disabled channels
+ * (a band >= nbands), which are skipped as in the tone calls.
+ * fsk_b200_rx_batch_channels / _s16: fsk_b200_rx_batch_tones / _s16 are the channels_per_row = 1 case.
+ * -EINVAL, with nothing launched, for channels_per_row == 0, nrows * channels_per_row > 2^31 - 1 and
+ * wherever fsk_b200_rx_batch_tones returns it; -ENOTSUP where it does.  The launch shape is the tone call's
+ * for nrows * channels_per_row streams; last_kernel() appends " channels=K" to the k_rx_tones<...> line
+ * when K > 1.
+ * fsk_b200_stream_push_channels: fsk_b200_stream_push for rows that carry k channels; fill [nrows],
+ * states [nrows*k], tone_bands [nrows*k][2] or NULL.  A channel is active when tone_bands is NULL or both
+ * of its bands are < nbands.  Per row r: m = the smallest min(pos, fill[r]) over the row's active
+ * channels (fill[r] when none is active); [m, fill[r]) moves to the front, the chunk is appended (what
+ * does not fit is counted in dropped[r]), fill[r] becomes the new length, and every channel of the row
+ * gets pos = min(pos, old fill) - min(min(pos, old fill), m), nframes = 0, done = 0 (carrier, squelch and
+ * session fields untouched).  A disabled channel therefore never pins its row's tail, and a channel
+ * enabled later starts at the oldest sample the row still holds.  fsk_b200_stream_push is the k = 1,
+ * tone_bands = NULL case.  -EINVAL for channels_per_row == 0 and nrows * channels_per_row > 2^31 - 1. */
+int fsk_b200_rx_batch_channels(fsk_b200_engine *e, const float *samples, size_t nrows, size_t stride,
+	const uint32_t *nsamples, uint32_t nsamples_all, uint32_t channels_per_row, const uint32_t *tone_bands,
+	fsk_b200_frame *frames, uint32_t max_frames, fsk_b200_stream_state *states, void *stream);
+int fsk_b200_rx_batch_channels_s16(fsk_b200_engine *e, const int16_t *samples, size_t nrows, size_t stride,
+	const uint32_t *nsamples, uint32_t nsamples_all, uint32_t channels_per_row, const uint32_t *tone_bands,
+	fsk_b200_frame *frames, uint32_t max_frames, fsk_b200_stream_state *states, void *stream);
+int fsk_b200_stream_push_channels(float *samples, size_t nrows, size_t stride, uint32_t *fill,
+	uint32_t channels_per_row, const uint32_t *tone_bands, uint32_t nbands, fsk_b200_stream_state *states,
+	const float *chunk, size_t chunk_stride, const uint32_t *chunk_len, uint32_t chunk_len_all, uint32_t *dropped,
+	void *stream);
+
 /* N2 -- 16-bit PCM ingest (the reference transmitter's default sample format, read back by
  * its rx as float = short / 32768: src/simpleaudio-sndfile.c:43-57, src/minimodem.c:786-788).
  * fsk_b200_s16_to_f32: device conversion (exact: a power-of-two scale), asynchronous on `stream`.
@@ -564,7 +597,8 @@ int fsk_b200_tx_text_batch(fsk_b200_tx_engine *te, const uint8_t *text, size_t n
 /* Diagnostics: which kernel instance the engine's latest fsk_b200_rx_batch or fsk_b200_find_frame_batch
  * launched ("k_rx<G=8,W=3,L=2,mode=2(shared-segment),fill=0,src=f32> threads=64 ring=640 smem=23232
  * blocks=8192", "k_find_frame<G=8,W=2,L=1,mode=0(per-candidate)> ..."; "" before the first launch);
- * k_rx_auto<...> and k_rx_tones<...> for fsk_b200_rx_batch_auto and fsk_b200_rx_batch_tones.  `fill`
+ * k_rx_auto<...> and k_rx_tones<...> for fsk_b200_rx_batch_auto and fsk_b200_rx_batch_tones (" channels=K"
+ * appended for fsk_b200_rx_batch_channels with K > 1).  `fill`
  * is 1 for the prefix-table kernel's TMA bulk fill (float rows, FSK_B200_PFX_FILL not 0) and 0 otherwise. */
 const char *fsk_b200_engine_last_kernel(const fsk_b200_engine *e);
 

@@ -126,6 +126,7 @@ EXPORTS = [
     "fsk_b200_rx_config_autodetect_shift", "fsk_b200_engine_set_auto_carrier", "fsk_b200_rx_batch_auto",
     "fsk_b200_rx_batch_auto_s16", "fsk_b200_auto_stream_window",
     "fsk_b200_tone_bands", "fsk_b200_rx_batch_tones", "fsk_b200_rx_batch_tones_s16",
+    "fsk_b200_rx_batch_channels", "fsk_b200_rx_batch_channels_s16", "fsk_b200_stream_push_channels",
 ]
 
 _lib = None
@@ -268,6 +269,15 @@ def lib():
     L.fsk_b200_rx_batch_tones.restype = C.c_int
     L.fsk_b200_rx_batch_tones_s16.argtypes = list(L.fsk_b200_rx_batch_tones.argtypes)
     L.fsk_b200_rx_batch_tones_s16.restype = C.c_int
+    L.fsk_b200_rx_batch_channels.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t, u32p, C.c_uint32,
+                                             C.c_uint32, u32p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p]
+    L.fsk_b200_rx_batch_channels.restype = C.c_int
+    L.fsk_b200_rx_batch_channels_s16.argtypes = list(L.fsk_b200_rx_batch_channels.argtypes)
+    L.fsk_b200_rx_batch_channels_s16.restype = C.c_int
+    L.fsk_b200_stream_push_channels.argtypes = [C.c_void_p, C.c_size_t, C.c_size_t, C.c_void_p, C.c_uint32,
+                                                C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_size_t,
+                                                C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p]
+    L.fsk_b200_stream_push_channels.restype = C.c_int
     L.fsk_b200_version.restype = C.c_char_p
     L.fsk_b200_launch_count.restype = C.c_ulonglong
     L.fsk_b200_last_error.restype = C.c_char_p
@@ -614,14 +624,19 @@ class RxEngine:
         return torch.from_numpy(out).to(device if device is not None else torch.device("cuda:0"))
 
     def rx_batch_tones(self, samples, tone_bands, nsamples=None, max_frames=None, frames=None, states=None,
-                       nsamples_each=None, stream=None):
+                       nsamples_each=None, stream=None, channels_per_row=1):
         """rx_batch with a tone pair per stream (fsk_b200_rx_batch_tones / _s16): row s is decoded as the
         CLI would with its own -M / -S.  samples: [nstreams, stride] float32 or int16 CUDA tensor;
         tone_bands: int32 CUDA tensor [nstreams, 2] (tone_bands()), read at every call.  A row whose pair
-        has a band >= nbands gets no records and keeps its state.  Returns (frames, states)."""
+        has a band >= nbands gets no records and keeps its state.  Returns (frames, states).
+        channels_per_row=k > 1 (fsk_b200_rx_batch_channels / _s16): samples [nrows, stride] carry k channels
+        each, channel c = r*k + j reads row r with pair tone_bands[c] ([nrows*k, 2]); nsamples_each is per
+        row, frames and states are per channel ([nrows*k, ...])."""
         torch = _torch()
         assert samples.is_cuda and samples.dtype in (torch.float32, torch.int16) and samples.is_contiguous()
-        nstreams, stride = samples.shape
+        nrows, stride = samples.shape
+        k = int(channels_per_row)
+        nstreams = nrows * k
         assert (tone_bands.is_cuda and tone_bands.dtype == torch.int32 and tone_bands.is_contiguous()
                 and tuple(tone_bands.shape) == (nstreams, 2))
         n_all = int(nsamples if nsamples is not None else stride)
@@ -631,11 +646,19 @@ class RxEngine:
             frames = torch.empty((nstreams, max_frames, 5), dtype=torch.int32, device=samples.device)
         if states is None:
             states = torch.zeros((nstreams, STATE_WORDS), dtype=torch.int32, device=samples.device)
-        fn = lib().fsk_b200_rx_batch_tones if samples.dtype == torch.float32 else lib().fsk_b200_rx_batch_tones_s16
-        rc = fn(self._e, _ptr(samples), nstreams, stride, _ptr(nsamples_each), n_all, _ptr(tone_bands),
+        if k == 1:
+            fn = lib().fsk_b200_rx_batch_tones if samples.dtype == torch.float32 else lib().fsk_b200_rx_batch_tones_s16
+            rc = fn(self._e, _ptr(samples), nrows, stride, _ptr(nsamples_each), n_all, _ptr(tone_bands),
+                    _ptr(frames), max_frames, _ptr(states), _stream_handle(stream))
+            if rc:
+                _err("fsk_b200_rx_batch_tones", rc)
+            return frames, states
+        fn = (lib().fsk_b200_rx_batch_channels if samples.dtype == torch.float32
+              else lib().fsk_b200_rx_batch_channels_s16)
+        rc = fn(self._e, _ptr(samples), nrows, stride, _ptr(nsamples_each), n_all, k, _ptr(tone_bands),
                 _ptr(frames), max_frames, _ptr(states), _stream_handle(stream))
         if rc:
-            _err("fsk_b200_rx_batch_tones", rc)
+            _err("fsk_b200_rx_batch_channels", rc)
         return frames, states
 
     def set_holdback(self, nsamples):
@@ -716,22 +739,36 @@ def detect_carrier_batch(fftsize, samples, nsamples, min_mag_threshold, offset=N
     return out
 
 
-def stream_push(rows, fill, states, chunk, chunk_len=None, dropped=None, stream=None):
+def stream_push(rows, fill, states, chunk, chunk_len=None, dropped=None, stream=None, channels_per_row=1,
+                tone_bands=None, nbands=0):
     """fsk_b200_stream_push on CUDA tensors: rows [n, stride] float32, fill [n] int32 (in/out), states
-    [n, STATE_WORDS] int32 (in/out), chunk [n, chunk_stride] float32, chunk_len [n] int32 or an int."""
+    [n, STATE_WORDS] int32 (in/out), chunk [n, chunk_stride] float32, chunk_len [n] int32 or an int.
+    channels_per_row=k or tone_bands given (fsk_b200_stream_push_channels): states are per channel,
+    [n*k, STATE_WORDS]; tone_bands (int32 [n*k, 2] or None) marks which channels are active (both bands
+    < nbands), and only those keep a row's tail."""
     torch = _torch()
     # the C call takes raw pointers and row strides: the tensors must be what it assumes
     assert rows.is_contiguous() and rows.dtype == torch.float32 and chunk.is_contiguous() and chunk.dtype == torch.float32
     assert fill.is_contiguous() and fill.dtype == torch.int32 and states.is_contiguous() and states.dtype == torch.int32
-    assert chunk.shape[0] == rows.shape[0] and states.shape == (rows.shape[0], STATE_WORDS)
+    k = int(channels_per_row)
+    assert chunk.shape[0] == rows.shape[0] and states.shape == (rows.shape[0] * k, STATE_WORDS)
     n, stride = rows.shape
     per = chunk_len if hasattr(chunk_len, "data_ptr") else None
     assert per is None or (per.dtype == torch.int32 and per.is_contiguous())
     common = 0 if per is not None else int(chunk.shape[1] if chunk_len is None else chunk_len)
-    rc = lib().fsk_b200_stream_push(_ptr(rows), n, stride, _ptr(fill), _ptr(states), _ptr(chunk),
-                                    chunk.shape[1], _ptr(per), common, _ptr(dropped), _stream_handle(stream))
+    if k == 1 and tone_bands is None:
+        rc = lib().fsk_b200_stream_push(_ptr(rows), n, stride, _ptr(fill), _ptr(states), _ptr(chunk),
+                                        chunk.shape[1], _ptr(per), common, _ptr(dropped), _stream_handle(stream))
+        if rc:
+            _err("fsk_b200_stream_push", rc)
+        return
+    assert tone_bands is None or (tone_bands.dtype == torch.int32 and tone_bands.is_contiguous()
+                                  and tuple(tone_bands.shape) == (n * k, 2))
+    rc = lib().fsk_b200_stream_push_channels(_ptr(rows), n, stride, _ptr(fill), k, _ptr(tone_bands), int(nbands),
+                                             _ptr(states), _ptr(chunk), chunk.shape[1], _ptr(per), common,
+                                             _ptr(dropped), _stream_handle(stream))
     if rc:
-        _err("fsk_b200_stream_push", rc)
+        _err("fsk_b200_stream_push_channels", rc)
 
 
 def wav_locate(image):

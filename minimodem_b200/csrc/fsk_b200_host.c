@@ -847,15 +847,20 @@ int fsk_b200_tone_bands(const fsk_b200_rx_params *p, float f_mark, float f_space
     return 0;
 }
 
-static int rx_batch_tones_any(fsk_b200_engine *e, const void *samples, int elem, size_t nstreams, size_t stride,
-	const uint32_t *nsamples, uint32_t nsamples_all, const uint32_t *tone_bands, fsk_b200_frame *frames,
-	uint32_t max_frames, fsk_b200_stream_state *states, void *stream)
+/* k channels per row (k = 1: the tone calls); pairs, records and states per channel */
+static int rx_batch_tones_any(fsk_b200_engine *e, const void *samples, int elem, size_t nrows, uint32_t k,
+	size_t stride, const uint32_t *nsamples, uint32_t nsamples_all, const uint32_t *tone_bands,
+	fsk_b200_frame *frames, uint32_t max_frames, fsk_b200_stream_state *states, void *stream)
 {
     if (!e || !tone_bands) {
 	fsk_b200_set_error("rx_batch_tones: NULL engine or tone_bands");
 	return -EINVAL;
     }
-    if (nstreams == 0)
+    if (k == 0 || nrows > 0x7fffffffu / k) {
+	fsk_b200_set_error("rx_batch_tones: channels_per_row (%u) is 0, or more than 2^31 - 1 streams", k);
+	return -EINVAL;
+    }
+    if (nrows == 0)
 	return 0;
     const size_t align = elem == 2 ? 7 : 3;
     if (!samples || ((uintptr_t)samples & 15) || (stride & align)) {
@@ -867,20 +872,19 @@ static int rx_batch_tones_any(fsk_b200_engine *e, const void *samples, int elem,
 	fsk_b200_set_error("rx_batch_tones: NULL argument");
 	return -EINVAL;
     }
-    if ((!nsamples && (size_t)nsamples_all > stride) || nstreams > 0x7fffffffu) {
-	fsk_b200_set_error("rx_batch_tones: nsamples_all (%u) exceeds the row stride (%zu), or too many streams",
-		nsamples_all, stride);
+    if (!nsamples && (size_t)nsamples_all > stride) {
+	fsk_b200_set_error("rx_batch_tones: nsamples_all (%u) exceeds the row stride (%zu)", nsamples_all, stride);
 	return -EINVAL;
     }
     return fsk_b200_cuda_rx_batch_tones(e->ce, &e->geom, &e->loopc, e->params.fftsize, e->params.nbands, samples,
-	    elem, nstreams, stride, nsamples, nsamples_all, tone_bands, frames, max_frames, states, stream);
+	    elem, nrows, k, stride, nsamples, nsamples_all, tone_bands, frames, max_frames, states, stream);
 }
 
 int fsk_b200_rx_batch_tones(fsk_b200_engine *e, const float *samples, size_t nstreams, size_t stride,
 	const uint32_t *nsamples, uint32_t nsamples_all, const uint32_t *tone_bands, fsk_b200_frame *frames,
 	uint32_t max_frames, fsk_b200_stream_state *states, void *stream)
 {
-    return rx_batch_tones_any(e, samples, 4, nstreams, stride, nsamples, nsamples_all, tone_bands, frames,
+    return rx_batch_tones_any(e, samples, 4, nstreams, 1, stride, nsamples, nsamples_all, tone_bands, frames,
 	    max_frames, states, stream);
 }
 
@@ -888,8 +892,24 @@ int fsk_b200_rx_batch_tones_s16(fsk_b200_engine *e, const int16_t *samples, size
 	const uint32_t *nsamples, uint32_t nsamples_all, const uint32_t *tone_bands, fsk_b200_frame *frames,
 	uint32_t max_frames, fsk_b200_stream_state *states, void *stream)
 {
-    return rx_batch_tones_any(e, samples, 2, nstreams, stride, nsamples, nsamples_all, tone_bands, frames,
+    return rx_batch_tones_any(e, samples, 2, nstreams, 1, stride, nsamples, nsamples_all, tone_bands, frames,
 	    max_frames, states, stream);
+}
+
+int fsk_b200_rx_batch_channels(fsk_b200_engine *e, const float *samples, size_t nrows, size_t stride,
+	const uint32_t *nsamples, uint32_t nsamples_all, uint32_t channels_per_row, const uint32_t *tone_bands,
+	fsk_b200_frame *frames, uint32_t max_frames, fsk_b200_stream_state *states, void *stream)
+{
+    return rx_batch_tones_any(e, samples, 4, nrows, channels_per_row, stride, nsamples, nsamples_all, tone_bands,
+	    frames, max_frames, states, stream);
+}
+
+int fsk_b200_rx_batch_channels_s16(fsk_b200_engine *e, const int16_t *samples, size_t nrows, size_t stride,
+	const uint32_t *nsamples, uint32_t nsamples_all, uint32_t channels_per_row, const uint32_t *tone_bands,
+	fsk_b200_frame *frames, uint32_t max_frames, fsk_b200_stream_state *states, void *stream)
+{
+    return rx_batch_tones_any(e, samples, 2, nrows, channels_per_row, stride, nsamples, nsamples_all, tone_bands,
+	    frames, max_frames, states, stream);
 }
 
 /* ---- live streams ------------------------------------------------------------ */
@@ -920,11 +940,17 @@ int fsk_b200_engine_set_holdback(fsk_b200_engine *e, uint32_t nsamples)
     return 0;
 }
 
-int fsk_b200_stream_push(float *samples, size_t nstreams, size_t stride, uint32_t *fill,
-	fsk_b200_stream_state *states, const float *chunk, size_t chunk_stride, const uint32_t *chunk_len,
-	uint32_t chunk_len_all, uint32_t *dropped, void *stream)
+int fsk_b200_stream_push_channels(float *samples, size_t nrows, size_t stride, uint32_t *fill,
+	uint32_t channels_per_row, const uint32_t *tone_bands, uint32_t nbands, fsk_b200_stream_state *states,
+	const float *chunk, size_t chunk_stride, const uint32_t *chunk_len, uint32_t chunk_len_all, uint32_t *dropped,
+	void *stream)
 {
-    if (nstreams == 0)
+    if (channels_per_row == 0 || nrows > 0x7fffffffu / channels_per_row) {
+	fsk_b200_set_error("stream_push: channels_per_row (%u) is 0, or more than 2^31 - 1 channels",
+		channels_per_row);
+	return -EINVAL;
+    }
+    if (nrows == 0)
 	return 0;
     int rc = check_layout(samples, stride);
     if (rc)
@@ -937,8 +963,16 @@ int fsk_b200_stream_push(float *samples, size_t nstreams, size_t stride, uint32_
 	fsk_b200_set_error("no usable CUDA device (there is no CPU fallback)");
 	return -ENODEV;
     }
-    return fsk_b200_cuda_stream_push(samples, nstreams, stride, fill, states, chunk, chunk_stride, chunk_len,
-	    chunk_len_all, dropped, stream);
+    return fsk_b200_cuda_stream_push(samples, nrows, stride, fill, channels_per_row, tone_bands, nbands, states,
+	    chunk, chunk_stride, chunk_len, chunk_len_all, dropped, stream);
+}
+
+int fsk_b200_stream_push(float *samples, size_t nstreams, size_t stride, uint32_t *fill,
+	fsk_b200_stream_state *states, const float *chunk, size_t chunk_stride, const uint32_t *chunk_len,
+	uint32_t chunk_len_all, uint32_t *dropped, void *stream)
+{
+    return fsk_b200_stream_push_channels(samples, nstreams, stride, fill, 1, NULL, 0, states, chunk, chunk_stride,
+	    chunk_len, chunk_len_all, dropped, stream);
 }
 
 int fsk_b200_rx_batch_host(fsk_b200_engine *e, const float *host_samples, size_t nstreams,

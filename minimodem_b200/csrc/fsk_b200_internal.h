@@ -200,14 +200,16 @@ int  fsk_b200_cuda_rx_batch_auto(void *ce, const fsk_b200_geom *g, const fsk_b20
 	const fsk_b200_auto_args *aa, const void *samples, int elem, size_t nstreams, size_t stride,
 	const uint32_t *nsamples, uint32_t nsamples_all, fsk_b200_frame *frames, uint32_t max_frames,
 	fsk_b200_stream_state *states, fsk_b200_auto_state *auto_states, uint32_t *rec_band, void *stream);
-/* -M / -S per stream: tone_bands (device) [nstreams][2] (mark band, space band) */
+/* -M / -S per channel: k channels per row, tone_bands (device) [nrows * k][2] (mark band, space band);
+ * nsamples (device, optional) [nrows], frames and states per channel */
 int  fsk_b200_cuda_rx_batch_tones(void *ce, const fsk_b200_geom *g, const fsk_b200_loopc *lc, int fftsize,
-	unsigned int nbands, const void *samples, int elem, size_t nstreams, size_t stride, const uint32_t *nsamples,
-	uint32_t nsamples_all, const uint32_t *tone_bands, fsk_b200_frame *frames, uint32_t max_frames,
-	fsk_b200_stream_state *states, void *stream);
-int  fsk_b200_cuda_stream_push(float *samples, size_t nstreams, size_t stride, uint32_t *fill,
-	fsk_b200_stream_state *states, const float *chunk, size_t chunk_stride, const uint32_t *chunk_len,
-	uint32_t chunk_len_all, uint32_t *dropped, void *stream);
+	unsigned int nbands, const void *samples, int elem, size_t nrows, unsigned int k, size_t stride,
+	const uint32_t *nsamples, uint32_t nsamples_all, const uint32_t *tone_bands, fsk_b200_frame *frames,
+	uint32_t max_frames, fsk_b200_stream_state *states, void *stream);
+/* live rows: k channels (states) per row, tone_bands (device, optional) [nrows * k][2] */
+int  fsk_b200_cuda_stream_push(float *samples, size_t nrows, size_t stride, uint32_t *fill, unsigned int k,
+	const uint32_t *tone_bands, unsigned int nbands, fsk_b200_stream_state *states, const float *chunk,
+	size_t chunk_stride, const uint32_t *chunk_len, uint32_t chunk_len_all, uint32_t *dropped, void *stream);
 /* the synthesis kernel; lut: device table of plan->lut_len float or int16 entries */
 int  fsk_b200_cuda_tx_synth(const fsk_b200_tx_plan *plan, const void *lut, const fsk_b200_tx_io *io,
 	void *stream);

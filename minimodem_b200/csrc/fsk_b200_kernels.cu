@@ -194,6 +194,7 @@ struct AutoArgs {
     unsigned half_ring;		/* samplebuf_size / 2: the refill of the virtual ring count */
     unsigned expect_nsamples;	/* the loop's own stop rule; lc.expect_nsamples above it is a live stream's holdback */
     const uint32_t *tones;	/* AUTO 2: [nstreams][2], each stream's (mark band, space band) */
+    unsigned k;			/* AUTO 2: channels per row; stream s reads row s / k */
 };
 
 /* fsk_detect_carrier (src/fsk.c:543-581) on one window, by the G lanes of a group: lane g takes the
@@ -326,7 +327,8 @@ k_find_frame(const __grid_constant__ fsk_b200_geom geo, const float4 *__restrict
  * and scans for a carrier band over its virtual ring count while it has none (DESIGN.md 5).
  * AUTO 2 (same shapes): -M / -S per stream.  The same per-stream table, filled once at the start of each
  * stream from its pair in au.tones; no scan, no auto state, and a carrier loss keeps the pair.  A stream
- * whose pair has a band >= au.nbands is skipped: no records, its state untouched. */
+ * whose pair has a band >= au.nbands is skipped: no records, its state untouched.  Streams are channels:
+ * stream s reads row s / au.k (au.k = 1: one stream per row). */
 template <int G, int W, int L, int MODE, int FILL, int SRC = 0, int AUTO = 0>
 __global__ void __launch_bounds__(MODE == 3 ? FSK_PFX_MAXTHREADS : FSK_MAXTHREADS,
 	MODE == 3 ? 1 : (MODE == 2 && G >= 16) ? 3 : FSK_MINBLOCKS)
@@ -364,10 +366,12 @@ k_rx(const __grid_constant__ fsk_b200_geom geo, const __grid_constant__ fsk_b200
 	fsk_b200_stream_state st = a.states[s];
 	if (st.done)
 	    continue;
-	const float *x = SRC ? (const float *)nullptr : a.samples + (size_t)s * a.stride;
-	const int16_t *x16 = SRC ? a.samples16 + (size_t)s * a.stride : (const int16_t *)nullptr;
-	/* a row never extends past its stride (per-stream lengths are caller data) */
-	const unsigned n = (unsigned)min((size_t)(a.nsamples ? a.nsamples[s] : a.nsamples_all), a.stride);
+	/* AUTO 2: the k channels of a row are consecutive streams; records, states and pairs stay per stream */
+	const unsigned row = AUTO == 2 ? s / au.k : s;
+	const float *x = SRC ? (const float *)nullptr : a.samples + (size_t)row * a.stride;
+	const int16_t *x16 = SRC ? a.samples16 + (size_t)row * a.stride : (const int16_t *)nullptr;
+	/* a row never extends past its stride (per-row lengths are caller data) */
+	const unsigned n = (unsigned)min((size_t)(a.nsamples ? a.nsamples[row] : a.nsamples_all), a.stride);
 	fsk_b200_frame *out = a.frames + (size_t)s * a.max_frames;
 	/* 16-byte chunks of the source line up with 16-byte chunks of the ring: 4 floats, or 8 int16 */
 	constexpr unsigned AL = SRC ? 7u : 3u;
@@ -1276,48 +1280,66 @@ __global__ void k_s16_to_f32_scalar(const short *__restrict__ src, float *__rest
 }
 
 /* ------------------------------------------------------------------------ */
-/* live streams: between two rx launches, each stream's unconsumed tail moves to */
-/* the front of its row and the new samples are appended (one warp per stream)   */
+/* live streams: between two rx launches, each row's unconsumed tail moves to    */
+/* the front of the row and the new samples are appended (one warp per row)      */
 /* ------------------------------------------------------------------------ */
-__global__ void k_stream_push(float *__restrict__ samples, unsigned nstreams, size_t stride,
-	uint32_t *__restrict__ fill, fsk_b200_stream_state *__restrict__ states,
+/* Row r carries the k channels (streams) r*k .. r*k + k-1.  The tail starts at m, the smallest
+ * min(pos, fill) over the row's active channels (all of them when bands is NULL, else those with both
+ * bands < nbands), or at fill when none is active; every channel is then rewound by m. */
+__global__ void k_stream_push(float *__restrict__ samples, unsigned nrows, size_t stride,
+	uint32_t *__restrict__ fill, unsigned k, const uint32_t *__restrict__ bands, unsigned nbands,
+	fsk_b200_stream_state *__restrict__ states,
 	const float *__restrict__ chunk, size_t chunk_stride, const uint32_t *__restrict__ chunk_len,
 	uint32_t chunk_len_all, uint32_t *__restrict__ dropped)
 {
     const unsigned lane = threadIdx.x & 31;
-    const unsigned s = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-    if (s >= nstreams)
+    const unsigned r = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    if (r >= nrows)
 	return;						/* whole warps leave together */
-    float *row = samples + (size_t)s * stride;
-    const unsigned have = fill[s];
-    unsigned long long pos64 = states[s].pos;
-    const unsigned pos = pos64 < have ? (unsigned)pos64 : have;
-    const unsigned tail = have - pos;
+    float *row = samples + (size_t)r * stride;
+    const unsigned have = fill[r];
+    fsk_b200_stream_state *const st = states + (size_t)r * k;
+    const uint32_t *const bd = bands ? bands + 2u * (size_t)r * k : nullptr;
+    unsigned m = 0xffffffffu;
+    for (unsigned j = lane; j < k; j += 32) {
+	if (bd && (bd[2u * j] >= nbands || bd[2u * j + 1u] >= nbands))
+	    continue;					/* a disabled channel does not pin the row */
+	const unsigned long long pos64 = st[j].pos;
+	m = min(m, pos64 < have ? (unsigned)pos64 : have);
+    }
+    for (unsigned o = 16; o; o >>= 1)
+	m = min(m, __shfl_xor_sync(0xffffffffu, m, o));
+    m = min(m, have);					/* no active channel: nothing is kept */
+    const unsigned tail = have - m;
     /* forward move in tiles of 32: a tile is read completely before it is written, and the
-     * destination of tile k ends below the source of tile k+1 (dst = src - pos, pos >= 0) */
-    if (pos)
-	for (unsigned k = 0; k < tail; k += 32) {
-	    const float v = k + lane < tail ? row[pos + k + lane] : 0.f;
+     * destination of tile k ends below the source of tile k+1 (dst = src - m, m >= 0) */
+    if (m)
+	for (unsigned t = 0; t < tail; t += 32) {
+	    const float v = t + lane < tail ? row[m + t + lane] : 0.f;
 	    __syncwarp();
-	    if (k + lane < tail)
-		row[k + lane] = v;
+	    if (t + lane < tail)
+		row[t + lane] = v;
 	    __syncwarp();
 	}
-    unsigned len = chunk_len ? chunk_len[s] : chunk_len_all;
+    unsigned len = chunk_len ? chunk_len[r] : chunk_len_all;
     const unsigned room = (unsigned)min((size_t)0xffffffffu, stride) - tail;
     const unsigned drop = len > room ? len - room : 0u;
     len -= drop;
-    const float *src = chunk + (size_t)s * chunk_stride;
+    const float *src = chunk + (size_t)r * chunk_stride;
     for (unsigned i = lane; i < len; i += 32)
 	row[tail + i] = src[i];
-    __syncwarp();		/* every lane has read fill[s] and states[s] before lane 0 rewrites them */
+    __syncwarp();		/* every lane has read fill[r] and the states before any lane rewrites them */
+    for (unsigned j = lane; j < k; j += 32) {
+	const unsigned long long pos64 = st[j].pos;
+	const unsigned pos = pos64 < have ? (unsigned)pos64 : have;
+	st[j].pos = pos - min(pos, m);
+	st[j].nframes = 0;				/* the record buffer starts over */
+	st[j].done = 0;
+    }
     if (lane == 0) {
-	fill[s] = tail + len;
-	states[s].pos = 0;
-	states[s].nframes = 0;				/* the record buffer starts over */
-	states[s].done = 0;
+	fill[r] = tail + len;
 	if (dropped)
-	    dropped[s] = drop;
+	    dropped[r] = drop;
     }
 }
 
@@ -2192,16 +2214,19 @@ extern "C" int fsk_b200_cuda_rx_batch_auto(void *p, const fsk_b200_geom *g, cons
 }
 
 /* -M / -S per stream: the AUTO_COMBOS shapes with AUTO 2, elem 4: float32 rows, elem 2: int16 rows.  The
- * engine's unit-circle table is built on first use (synchronous).  -ENOTSUP, with nothing launched or built,
- * where the per-candidate kernel cannot take the mode or the shape has no build of it. */
+ * streams are nrows * k channels, k per row (k = 1: a stream per row); the launch shape is the one of
+ * nrows * k streams.  The engine's unit-circle table is built on first use (synchronous).  -ENOTSUP, with
+ * nothing launched or built, where the per-candidate kernel cannot take the mode or the shape has no build
+ * of it. */
 extern "C" int fsk_b200_cuda_rx_batch_tones(void *p, const fsk_b200_geom *g, const fsk_b200_loopc *lc, int fftsize,
-	unsigned nbands, const void *samples, int elem, size_t nstreams, size_t stride, const uint32_t *nsamples,
-	uint32_t nsamples_all, const uint32_t *tone_bands, fsk_b200_frame *frames, uint32_t max_frames,
-	fsk_b200_stream_state *states, void *stream)
+	unsigned nbands, const void *samples, int elem, size_t nrows, unsigned k, size_t stride,
+	const uint32_t *nsamples, uint32_t nsamples_all, const uint32_t *tone_bands, fsk_b200_frame *frames,
+	uint32_t max_frames, fsk_b200_stream_state *states, void *stream)
 {
     CudaEngine *ce = (CudaEngine *)p;
     if (engine_device_check(ce, "rx_batch_tones"))
 	return -EINVAL;
+    const size_t nstreams = nrows * k;
     Shape sh;
     const unsigned tmax = lc->try_max_nocarrier > lc->try_max_carrier ? lc->try_max_nocarrier : lc->try_max_carrier;
     const unsigned max_advance = tmax - 1u + lc->frame_nsamples;
@@ -2229,6 +2254,7 @@ extern "C" int fsk_b200_cuda_rx_batch_tones(void *p, const fsk_b200_geom *g, con
     au.fftsize = (unsigned)fftsize;
     au.nbands = nbands;
     au.tones = tone_bands;
+    au.k = k;
     cudaStream_t st = (cudaStream_t)stream;
     cudaError_t e = cudaErrorInvalidValue;
     if (elem == 2) {
@@ -2244,6 +2270,10 @@ extern "C" int fsk_b200_cuda_rx_batch_tones(void *p, const fsk_b200_geom *g, con
 	    "k_rx_tones<G=%d,W=%d,L=%d,mode=0(per-candidate),fill=0,src=%s> threads=%d ring=%u smem=%zu blocks=%d lookahead=%u",
 	    sh.G, sh.W, sh.L, elem == 2 ? (sh.slide ? "s16,slide" : "s16") : (sh.slide ? "f32,slide" : "f32"),
 	    sh.wpb * 32, sh.ring, sh.smem, sh.blocks, sh.lookahead);
+    if (k > 1) {
+	const size_t used = strlen(ce->last_kernel);
+	snprintf(ce->last_kernel + used, sizeof(ce->last_kernel) - used, " channels=%u", k);
+    }
     if (e != cudaSuccess) {
 	fsk_b200_set_error("rx_batch_tones launch (G=%d W=%d L=%d ring=%u smem=%zu): %s", sh.G, sh.W, sh.L, sh.ring,
 		sh.smem, cudaGetErrorString(e));
@@ -2422,16 +2452,17 @@ extern "C" int fsk_b200_cuda_s16_to_f32(const int16_t *src, float *dst, size_t n
     return 0;
 }
 
-extern "C" int fsk_b200_cuda_stream_push(float *samples, size_t nstreams, size_t stride, uint32_t *fill,
-	fsk_b200_stream_state *states, const float *chunk, size_t chunk_stride, const uint32_t *chunk_len,
-	uint32_t chunk_len_all, uint32_t *dropped, void *stream)
+/* one warp per row; k channels (states) per row, tone_bands optional ([nrows * k][2]) */
+extern "C" int fsk_b200_cuda_stream_push(float *samples, size_t nrows, size_t stride, uint32_t *fill,
+	unsigned k, const uint32_t *tone_bands, unsigned nbands, fsk_b200_stream_state *states, const float *chunk,
+	size_t chunk_stride, const uint32_t *chunk_len, uint32_t chunk_len_all, uint32_t *dropped, void *stream)
 {
-    if (nstreams == 0)
+    if (nrows == 0)
 	return 0;
     const unsigned threads = 128;
-    const size_t blocks = (nstreams * 32 + threads - 1) / threads;
-    FSK_LAUNCH(k_stream_push, (unsigned)blocks, threads, 0, (cudaStream_t)stream, samples, (unsigned)nstreams,
-	    stride, fill, states, chunk, chunk_stride, chunk_len, chunk_len_all, dropped);
+    const size_t blocks = (nrows * 32 + threads - 1) / threads;
+    FSK_LAUNCH(k_stream_push, (unsigned)blocks, threads, 0, (cudaStream_t)stream, samples, (unsigned)nrows,
+	    stride, fill, k, tone_bands, nbands, states, chunk, chunk_stride, chunk_len, chunk_len_all, dropped);
     g_launches++;
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) {

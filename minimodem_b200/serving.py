@@ -16,7 +16,10 @@ the CLI's -a) every stream finds its own tone pair: fsk_b200_rx_batch_auto with 
 auto states and the auto holdback (fsk_b200_auto_stream_window) in place of fsk_b200_rx_batch.
 With tones=bands (an int32 tensor [nstreams, 2] from RxEngine.tone_bands on an engine of the same mode,
 or rx.engine.tone_bands) every stream keeps its own -M / -S pair: fsk_b200_rx_batch_tones with the
-ordinary holdback; tones and auto_carrier exclude each other.
+ordinary holdback; tones and auto_carrier exclude each other.  With channels_per_row=k and tones [nstreams*k, 2]
+each fed row carries k channels (both directions of a duplex line, k signals of a passband): one push per row
+(fsk_b200_stream_push_channels, where a disabled channel does not hold the row back), one
+fsk_b200_rx_batch_channels, and text and decoder state per channel, [nstreams*k, ...].
 
     tx = LiveTransmitter("rtty", sample_rate=8000, nstreams=4096, max_text=64)
     for text, lengths in source:                  # uint8 CUDA tensor [nstreams, <= max_text], int32 [nstreams]
@@ -34,10 +37,13 @@ from . import api
 
 class LiveReceiver:
     def __init__(self, baudmode, sample_rate=48000, nstreams=1, max_chunk=4800, device=None,
-                 binary_output=False, auto_carrier=None, tones=None, **overrides):
+                 binary_output=False, auto_carrier=None, tones=None, channels_per_row=1, **overrides):
         torch = api._torch()
         if auto_carrier is not None and tones is not None:
             raise ValueError("LiveReceiver: auto_carrier and tones exclude each other")
+        self.k = int(channels_per_row)
+        if self.k != 1 and tones is None:
+            raise ValueError("LiveReceiver: channels_per_row needs tones, a pair per channel")
         self.engine = api.RxEngine.for_mode(baudmode, sample_rate, **overrides)
         self.kind = api.decoder_for_mode(baudmode, self.engine.params.n_data_bits, binary_output)
         self.auto = auto_carrier is not None
@@ -53,24 +59,29 @@ class LiveReceiver:
         self.row_bytes = api.decode_max_bytes(self.kind, self.engine.params.n_data_bits, self.max_frames)
         dev = device if device is not None else torch.device("cuda:0")
         z = lambda shape, dt: torch.zeros(shape, dtype=dt, device=dev)
+        nchannels = self.nstreams * self.k
         self.rows = z((self.nstreams, self.stride), torch.float32)
         self.fill = z((self.nstreams,), torch.int32)
-        self.states = z((self.nstreams, api.STATE_WORDS), torch.int32)
-        self.dstates = z((self.nstreams, api.DECODER_STATE_BYTES), torch.uint8)
+        self.states = z((nchannels, api.STATE_WORDS), torch.int32)
+        self.dstates = z((nchannels, api.DECODER_STATE_BYTES), torch.uint8)
         self.dropped = z((self.nstreams,), torch.int32)
         self._empty = z((self.nstreams, 4), torch.float32)
         self.auto_states = z((self.nstreams, api.AUTO_STATE_BYTES), torch.uint8) if self.auto else None
         self.tones = None
         if tones is not None:
-            assert tuple(tones.shape) == (self.nstreams, 2)
+            assert tuple(tones.shape) == (nchannels, 2)
             self.tones = tones.to(device=dev, dtype=torch.int32).contiguous()
 
     def _step(self, chunk, lengths):
-        api.stream_push(self.rows, self.fill, self.states, chunk, lengths, dropped=self.dropped)
+        if self.k > 1:
+            api.stream_push(self.rows, self.fill, self.states, chunk, lengths, dropped=self.dropped,
+                            channels_per_row=self.k, tone_bands=self.tones, nbands=self.engine.params.nbands)
+        else:
+            api.stream_push(self.rows, self.fill, self.states, chunk, lengths, dropped=self.dropped)
         if self.tones is not None:
             frames, self.states = self.engine.rx_batch_tones(
                 self.rows, self.tones, nsamples=self.stride, nsamples_each=self.fill, max_frames=self.max_frames,
-                states=self.states)
+                states=self.states, channels_per_row=self.k)
         elif self.auto:
             frames, self.states, self.auto_states = self.engine.rx_batch_auto(
                 self.rows, nsamples=self.stride, nsamples_each=self.fill, max_frames=self.max_frames,
