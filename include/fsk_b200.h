@@ -594,6 +594,44 @@ int fsk_b200_tx_text_batch(fsk_b200_tx_engine *te, const uint8_t *text, size_t n
 	const uint32_t *text_len, unsigned int flags, fsk_b200_tx_state *states, void *out, size_t out_stride,
 	uint32_t *out_len, void *stream);
 
+/* fsk_b200_tx_text_batch with a tone pair per stream (the CLI's -M / -S for each stream in one call).
+ * tone_hz: device float32 [nstreams][2] = (mark Hz, space Hz), read at every call.  Stream s gets, sample
+ * for sample, what fsk_b200_tx_text_batch gives on an engine built with f_mark = tone_hz[s][0], f_space =
+ * tone_hz[s][1]; rate, framing, sync bytes, leader and trailer, encoder, volume, table and sample format
+ * are the engine's.  --inverted is the two tones swapped; with invert_start_stop the leader, idle tone,
+ * start and stop bits take the stream's own pair.  A stream may move to another pair between calls: its
+ * phase carries over, as in the reference when consecutive tones change frequency.  A stream whose pair
+ * has a frequency that is not finite or not > 0 is skipped: out_len[s] = 0, its row and state are left
+ * untouched (the device cannot return an error per stream).  -EINVAL, with nothing launched, for a NULL
+ * tone_hz and wherever fsk_b200_tx_text_batch returns it. */
+int fsk_b200_tx_text_batch_tones(fsk_b200_tx_engine *te, const uint8_t *text, size_t nstreams, size_t text_stride,
+	const uint32_t *text_len, const float *tone_hz, unsigned int flags, fsk_b200_tx_state *states, void *out,
+	size_t out_stride, uint32_t *out_len, void *stream);
+
+/* Tone-pair channels summed into shared rows: the input fsk_b200_rx_batch_channels decodes (both directions of
+ * a full-duplex line, k signals of a passband), made on the device without a row per channel.  Channel
+ * c = r*k + j (k = channels_per_row) belongs to row r.  text [nrows*k][text_stride], text_len [nrows*k],
+ * tone_hz [nrows*k][2] (mark Hz, space Hz), lead_in [nrows*k] or NULL, out [nrows][out_stride] in the
+ * engine's sample format, out_len [nrows*k]; all device memory, asynchronous on `stream`.
+ * Every channel is one complete transmission from a fresh state (leader, preamble, its text, trailer:
+ * fsk_b200_tx_text_batch_tones with FSK_B200_TX_FINAL on zeroed states) behind lead_in[c] samples of
+ * silence; a channel with no text is silent.  Row r gets exactly nsamples_out samples: the sum of its
+ * channels' audio, each zero-padded or cut to nsamples_out.  float32: added left to right in channel order,
+ * one IEEE add each (c0 + c1 + ... + c(k-1)); int16: summed exactly in int32, then saturated to
+ * [-32768, 32767].  A disabled channel (a pair that is not finite and > 0, as in the tone call) adds
+ * nothing; a row with no enabled channel is all zeros; samples past nsamples_out are not touched.
+ * out_len[c] = lead_in[c] + the channel's signal, uncut by nsamples_out (saturated at 2^32 - 1), or 0 for a
+ * disabled channel.  int16 rows of k > 1 channels hold their int32 partial sums in scratch device memory
+ * taken from the stream's pool for the call (4 bytes per sample of the rows): -ENOMEM when it cannot be had.
+ * -EINVAL, with nothing launched, for a NULL pointer other than lead_in, channels_per_row == 0,
+ * nrows * channels_per_row > 2^31 - 1, nsamples_out > out_stride, and a text_stride whose longest channel
+ * plus nsamples_out exceeds 2^32 - 1 samples.  k = 1 with no lead-ins is fsk_b200_tx_text_batch_tones +
+ * FSK_B200_TX_FINAL on fresh states, each row zero-padded to nsamples_out.  There is no live (tick by tick)
+ * form: the channels of a row would need one clock across ticks, which the reference's transmitter has not. */
+int fsk_b200_tx_text_channels(fsk_b200_tx_engine *te, const uint8_t *text, size_t nrows, uint32_t channels_per_row,
+	size_t text_stride, const uint32_t *text_len, const float *tone_hz, const uint32_t *lead_in, void *out,
+	size_t out_stride, uint32_t nsamples_out, uint32_t *out_len, void *stream);
+
 /* Diagnostics: which kernel instance the engine's latest fsk_b200_rx_batch or fsk_b200_find_frame_batch
  * launched ("k_rx<G=8,W=3,L=2,mode=2(shared-segment),fill=0,src=f32> threads=64 ring=640 smem=23232
  * blocks=8192", "k_find_frame<G=8,W=2,L=1,mode=0(per-candidate)> ..."; "" before the first launch);

@@ -122,7 +122,7 @@ EXPORTS = [
     "fsk_b200_stream_window", "fsk_b200_engine_set_holdback", "fsk_b200_stream_push", "fsk_b200_wav_locate",
     "fsk_b200_version", "fsk_b200_launch_count", "fsk_b200_last_error", "fsk_b200_engine_last_kernel",
     "fsk_b200_encoder_for_mode", "fsk_b200_tx_config_from_rx", "fsk_b200_tx_engine_new", "fsk_b200_tx_engine_destroy",
-    "fsk_b200_tx_max_samples", "fsk_b200_tx_text_batch",
+    "fsk_b200_tx_max_samples", "fsk_b200_tx_text_batch", "fsk_b200_tx_text_batch_tones", "fsk_b200_tx_text_channels",
     "fsk_b200_rx_config_autodetect_shift", "fsk_b200_engine_set_auto_carrier", "fsk_b200_rx_batch_auto",
     "fsk_b200_rx_batch_auto_s16", "fsk_b200_auto_stream_window",
     "fsk_b200_tone_bands", "fsk_b200_rx_batch_tones", "fsk_b200_rx_batch_tones_s16",
@@ -250,6 +250,14 @@ def lib():
     L.fsk_b200_tx_text_batch.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t, C.c_void_p, C.c_uint,
                                          C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p]
     L.fsk_b200_tx_text_batch.restype = C.c_int
+    L.fsk_b200_tx_text_batch_tones.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t, C.c_void_p,
+                                               C.c_void_p, C.c_uint, C.c_void_p, C.c_void_p, C.c_size_t,
+                                               C.c_void_p, C.c_void_p]
+    L.fsk_b200_tx_text_batch_tones.restype = C.c_int
+    L.fsk_b200_tx_text_channels.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_uint32, C.c_size_t, C.c_void_p,
+                                            C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_uint32, C.c_void_p,
+                                            C.c_void_p]
+    L.fsk_b200_tx_text_channels.restype = C.c_int
     L.fsk_b200_sin_table.argtypes = [C.POINTER(C.c_float), C.c_uint, C.c_float]
     L.fsk_b200_sin_table.restype = None
     L.fsk_b200_rx_config_autodetect_shift.argtypes = [C.POINTER(RxConfig)]
@@ -890,10 +898,30 @@ class TxEngine:
         return torch.zeros((int(nstreams), TX_STATE_BYTES), dtype=torch.uint8,
                            device=device if device is not None else torch.device("cuda:0"))
 
-    def text_batch(self, text, lengths, states, flags=0, out=None, out_len=None, stream=None):
+    @staticmethod
+    def tone_pairs(marks_hz, spaces_hz, inverted=False, device=None):
+        """The tones argument of text_batch: a float32 tensor [n, 2] of (mark Hz, space Hz), one row per
+        stream, for the CLI's -M marks_hz[s] -S spaces_hz[s] (scalars or sequences, broadcast); inverted (a
+        bool or one per stream) swaps a stream's two tones, as --inverted does.  A frequency that is not
+        finite or not > 0 raises ValueError.  device: where the tensor goes (default cuda:0)."""
+        torch = _torch()
+        m, s, inv = np.broadcast_arrays(np.asarray(marks_hz, np.float32), np.asarray(spaces_hz, np.float32),
+                                        np.asarray(inverted, bool))
+        m, s, inv = m.reshape(-1), s.reshape(-1), inv.reshape(-1)
+        out = np.stack([np.where(inv, s, m), np.where(inv, m, s)], axis=1).astype(np.float32)
+        bad = ~(np.isfinite(out) & (out > 0)).all(axis=1)
+        if bad.any():
+            i = int(np.nonzero(bad)[0][0])
+            raise ValueError("tone_pairs: pair %d (%r, %r) needs finite frequencies > 0" % (i, float(m[i]), float(s[i])))
+        return torch.from_numpy(out).to(device if device is not None else torch.device("cuda:0"))
+
+    def text_batch(self, text, lengths, states, flags=0, out=None, out_len=None, stream=None, tones=None):
         """fsk_b200_tx_text_batch.  text: uint8 CUDA tensor [nstreams, text_stride]; lengths: int32
         [nstreams]; states: uint8 [nstreams, TX_STATE_BYTES] (updated in place).  Returns (samples
-        [nstreams, out_stride] int16 or float32, counts [nstreams] int32)."""
+        [nstreams, out_stride] int16 or float32, counts [nstreams] int32).  tones: float32 CUDA tensor
+        [nstreams, 2] of (mark Hz, space Hz) (tone_pairs()), read at every call
+        (fsk_b200_tx_text_batch_tones): stream s is sent as by an engine built for its pair; a stream whose
+        pair is not finite and > 0 gets count 0 and keeps its row and state."""
         torch = _torch()
         assert text.dtype == torch.uint8 and text.is_contiguous() and text.dim() == 2
         nstreams, text_stride = text.shape
@@ -906,11 +934,51 @@ class TxEngine:
         assert out.is_contiguous() and out.dtype == (torch.float32 if self.float_samples else torch.int16)
         if out_len is None:
             out_len = torch.empty((nstreams,), dtype=torch.int32, device=text.device)
-        rc = lib().fsk_b200_tx_text_batch(self._te, _ptr(text), nstreams, text_stride, _ptr(lengths), int(flags),
-                                          _ptr(states), _ptr(out), out.shape[1], _ptr(out_len),
-                                          _stream_handle(stream))
+        if tones is None:
+            rc = lib().fsk_b200_tx_text_batch(self._te, _ptr(text), nstreams, text_stride, _ptr(lengths), int(flags),
+                                              _ptr(states), _ptr(out), out.shape[1], _ptr(out_len),
+                                              _stream_handle(stream))
+            if rc:
+                _err("fsk_b200_tx_text_batch", rc)
+            return out, out_len
+        assert (tones.is_cuda and tones.dtype == torch.float32 and tones.is_contiguous()
+                and tuple(tones.shape) == (nstreams, 2))
+        rc = lib().fsk_b200_tx_text_batch_tones(self._te, _ptr(text), nstreams, text_stride, _ptr(lengths),
+                                                _ptr(tones), int(flags), _ptr(states), _ptr(out), out.shape[1],
+                                                _ptr(out_len), _stream_handle(stream))
         if rc:
-            _err("fsk_b200_tx_text_batch", rc)
+            _err("fsk_b200_tx_text_batch_tones", rc)
+        return out, out_len
+
+    def text_channels(self, text, lengths, tones, channels_per_row, nsamples_out, lead_in=None, out=None,
+                      out_len=None, stream=None):
+        """fsk_b200_tx_text_channels: k = channels_per_row transmissions summed into each row.  text: uint8 CUDA
+        tensor [nrows*k, text_stride], channel c = r*k + j of row r; lengths: int32 [nrows*k]; tones: float32
+        [nrows*k, 2] (tone_pairs()); lead_in: int32 [nrows*k] samples of silence before each channel, or None.
+        Every channel is a whole transmission from a fresh state; row r holds exactly nsamples_out samples,
+        the sum of its channels (float32 left to right, int16 saturated).  Returns (rows [nrows, out_stride]
+        int16 or float32, zeros past nsamples_out when allocated here; out_len [nrows*k] int32, each channel's
+        uncut length, 0 when its pair is invalid)."""
+        torch = _torch()
+        k = int(channels_per_row)
+        assert text.dtype == torch.uint8 and text.is_contiguous() and text.dim() == 2
+        nch, text_stride = text.shape
+        assert k > 0 and nch % k == 0, "text rows must be nrows * channels_per_row"
+        nrows = nch // k
+        assert lengths.dtype == torch.int32 and lengths.is_contiguous() and lengths.numel() == nch
+        assert tones.is_cuda and tones.dtype == torch.float32 and tones.is_contiguous() and tuple(tones.shape) == (nch, 2)
+        assert lead_in is None or (lead_in.dtype == torch.int32 and lead_in.is_contiguous() and lead_in.numel() == nch)
+        if out is None:
+            out = torch.zeros((nrows, (int(nsamples_out) + 7) & ~7),
+                              dtype=torch.float32 if self.float_samples else torch.int16, device=text.device)
+        assert out.is_contiguous() and out.dtype == (torch.float32 if self.float_samples else torch.int16)
+        if out_len is None:
+            out_len = torch.empty((nch,), dtype=torch.int32, device=text.device)
+        rc = lib().fsk_b200_tx_text_channels(self._te, _ptr(text), nrows, k, text_stride, _ptr(lengths), _ptr(tones),
+                                             _ptr(lead_in), _ptr(out), out.shape[1], int(nsamples_out), _ptr(out_len),
+                                             _stream_handle(stream))
+        if rc:
+            _err("fsk_b200_tx_text_channels", rc)
         return out, out_len
 
     def destroy(self):

@@ -1344,23 +1344,24 @@ uint64_t fsk_b200_tx_max_samples(const fsk_b200_tx_engine *te, uint32_t nbytes, 
     return n > 0xffffffffu ? 0 : n;
 }
 
-int fsk_b200_tx_text_batch(fsk_b200_tx_engine *te, const uint8_t *text, size_t nstreams, size_t text_stride,
-	const uint32_t *text_len, unsigned int flags, fsk_b200_tx_state *states, void *out, size_t out_stride,
-	uint32_t *out_len, void *stream)
+/* fsk_b200_tx_text_batch, and with tone_hz != NULL its pair-per-stream form: one set of checks */
+static int tx_text_launch(const char *what, fsk_b200_tx_engine *te, const uint8_t *text, size_t nstreams,
+	size_t text_stride, const uint32_t *text_len, const float *tone_hz, unsigned int flags,
+	fsk_b200_tx_state *states, void *out, size_t out_stride, uint32_t *out_len, void *stream)
 {
     if (!te || !text || !text_len || !states || !out || !out_len) {
-	fsk_b200_set_error("tx_text_batch: NULL argument");
+	fsk_b200_set_error("%s: NULL argument", what);
 	return -EINVAL;
     }
     if (flags & ~(FSK_B200_TX_IDLE_IF_EMPTY | FSK_B200_TX_FINAL)) {
-	fsk_b200_set_error("tx_text_batch: unknown flags 0x%x", flags);
+	fsk_b200_set_error("%s: unknown flags 0x%x", what, flags);
 	return -EINVAL;
     }
     const uint64_t need = fsk_b200_tx_max_samples(te, text_stride > 0xffffffffu ? 0xffffffffu : (uint32_t)text_stride,
 	    flags);
     if (text_stride > 0xffffffffu || (need == 0 && text_stride > 0) || out_stride < need) {
-	fsk_b200_set_error("tx_text_batch: out_stride %zu is below the %llu samples a row of %zu bytes can need",
-		out_stride, (unsigned long long)need, text_stride);
+	fsk_b200_set_error("%s: out_stride %zu is below the %llu samples a row of %zu bytes can need",
+		what, out_stride, (unsigned long long)need, text_stride);
 	return -EINVAL;
     }
     fsk_b200_tx_io io;
@@ -1374,6 +1375,68 @@ int fsk_b200_tx_text_batch(fsk_b200_tx_engine *te, const uint8_t *text, size_t n
     io.out_len = out_len;
     io.flags = flags;
     io.nstreams = nstreams;
+    io.tones = tone_hz;
+    return fsk_b200_cuda_tx_synth(&te->plan, te->d_lut, &io, stream);
+}
+
+int fsk_b200_tx_text_batch(fsk_b200_tx_engine *te, const uint8_t *text, size_t nstreams, size_t text_stride,
+	const uint32_t *text_len, unsigned int flags, fsk_b200_tx_state *states, void *out, size_t out_stride,
+	uint32_t *out_len, void *stream)
+{
+    return tx_text_launch("tx_text_batch", te, text, nstreams, text_stride, text_len, NULL, flags, states, out,
+	    out_stride, out_len, stream);
+}
+
+int fsk_b200_tx_text_batch_tones(fsk_b200_tx_engine *te, const uint8_t *text, size_t nstreams, size_t text_stride,
+	const uint32_t *text_len, const float *tone_hz, unsigned int flags, fsk_b200_tx_state *states, void *out,
+	size_t out_stride, uint32_t *out_len, void *stream)
+{
+    if (!tone_hz) {
+	fsk_b200_set_error("tx_text_batch_tones: NULL tone_hz");
+	return -EINVAL;
+    }
+    return tx_text_launch("tx_text_batch_tones", te, text, nstreams, text_stride, text_len, tone_hz, flags, states,
+	    out, out_stride, out_len, stream);
+}
+
+int fsk_b200_tx_text_channels(fsk_b200_tx_engine *te, const uint8_t *text, size_t nrows, uint32_t channels_per_row,
+	size_t text_stride, const uint32_t *text_len, const float *tone_hz, const uint32_t *lead_in, void *out,
+	size_t out_stride, uint32_t nsamples_out, uint32_t *out_len, void *stream)
+{
+    if (!te || !text || !text_len || !tone_hz || !out || !out_len) {
+	fsk_b200_set_error("tx_text_channels: NULL argument");
+	return -EINVAL;
+    }
+    if (channels_per_row == 0 || nrows > 0x7fffffffu / channels_per_row) {
+	fsk_b200_set_error("tx_text_channels: %zu rows of %u channels (1..2^31 - 1 channels in all)", nrows,
+		channels_per_row);
+	return -EINVAL;
+    }
+    if (nsamples_out > out_stride) {
+	fsk_b200_set_error("tx_text_channels: nsamples_out %u exceeds out_stride %zu", nsamples_out, out_stride);
+	return -EINVAL;
+    }
+    /* a channel's position runs up to nsamples_out (its lead-in, clamped) plus its longest signal */
+    const uint64_t need = fsk_b200_tx_max_samples(te, text_stride > 0xffffffffu ? 0xffffffffu : (uint32_t)text_stride,
+	    FSK_B200_TX_FINAL);
+    if (text_stride > 0xffffffffu || (need == 0 && text_stride > 0) || need + nsamples_out > 0xffffffffu) {
+	fsk_b200_set_error("tx_text_channels: a channel of %zu bytes can run past 2^32 - 1 samples", text_stride);
+	return -EINVAL;
+    }
+    fsk_b200_tx_io io;
+    memset(&io, 0, sizeof(io));
+    io.text = text;
+    io.text_stride = text_stride;
+    io.text_len = text_len;
+    io.lead_in = lead_in;
+    io.tones = tone_hz;
+    io.out = out;
+    io.out_stride = out_stride;
+    io.out_len = out_len;
+    io.cap = nsamples_out;
+    io.flags = FSK_B200_TX_FINAL;
+    io.channels_per_row = channels_per_row;
+    io.nstreams = nrows * channels_per_row;
     return fsk_b200_cuda_tx_synth(&te->plan, te->d_lut, &io, stream);
 }
 

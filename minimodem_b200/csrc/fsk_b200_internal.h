@@ -144,6 +144,10 @@ typedef struct fsk_b200_tx_io {
     uint32_t	cap;			/* 0: a row ends with its signal; else exactly cap samples, zero padded / truncated */
     uint32_t	flags;			/* FSK_B200_TX_* */
     size_t	nstreams;
+    const float *tones;			/* [nstreams][2] (mark Hz, space Hz) per stream; NULL: the plan's pair */
+    uint32_t	channels_per_row;	/* 0: one row per stream; k: mixed rows of k channels (nstreams = rows * k) */
+    int32_t	*acc;			/* mixed int16 rows of k > 1 channels: int32 partial sums [rows][acc_stride] */
+    size_t	acc_stride;
 } fsk_b200_tx_io;
 
 void fsk_b200_set_error(const char *fmt, ...);

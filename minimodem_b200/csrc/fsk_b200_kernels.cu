@@ -30,7 +30,8 @@
  *                         3 prefix table (G = 32; W codes the candidate slot); FILL 0 cp.async, 1 TMA bulk
  *                         copies (MODE 3 only); SRC 0 float32 rows, 1 int16 PCM rows widened inside the fill
  * k_find_frame<G,W,L,MODE> batched fsk_find_frame
- * k_tx_synth<T,VEC,LUT>   the transmitter: text (or data words) -> int16 / float32 samples
+ * k_tx_synth<T,VEC,LUT,TONES>  the transmitter: text (or data words) -> int16 / float32 samples; TONES a
+ *                         tone pair per stream
  * k_band_mags, k_detect_carrier, k_s16_to_f32, k_decode<KIND>   the "next" rows (DESIGN.md 0)
  *
  * Compiled with -fmad=false: every a*b+c below is either an explicit fmaf() (the
@@ -1027,13 +1028,93 @@ __device__ __forceinline__ void tx_store(T *row, unsigned q0, unsigned end, cons
 	    row[q0 + e] = v[e];
 }
 
+/* The passes of a mixed row (fsk_b200_tx_text_channels), one per channel in channel order: STORE the
+ * first of k > 1 channels, ADD a middle one, LAST the last one, ONLY the channel of a row of one.
+ * float32: the row holds c0 + ... + cj, one IEEE add per pass (-fmad=false: nothing fuses with the
+ * sample's product).  int16: the partial sums are exact in `acc`, an int32 row; LAST saturates them
+ * into the row. */
+#define TX_MIX_STORE 0u
+#define TX_MIX_ADD 1u
+#define TX_MIX_LAST 2u
+#define TX_MIX_ONLY 3u
+
+template <typename T, int VEC>
+__device__ __forceinline__ void tx_mix_store(T *row, int *acc, unsigned q0, unsigned end, T (&v)[VEC], unsigned mode)
+{
+    if (mode == TX_MIX_ONLY || (sizeof(T) == 4 && mode == TX_MIX_STORE)) {
+	tx_store<T, VEC>(row, q0, end, v);
+	return;
+    }
+    if constexpr (sizeof(T) == 4) {
+	if constexpr (VEC > 1) {
+	    if (q0 + VEC <= end) {
+		const float4 o = *reinterpret_cast<const float4 *>(row + q0);
+		v[0] = o.x + v[0];
+		v[1] = o.y + v[1];
+		v[2] = o.z + v[2];
+		v[3] = o.w + v[3];
+		tx_store<T, VEC>(row, q0, end, v);
+		return;
+	    }
+	}
+	for (int e = 0; e < VEC; e++)
+	    if (q0 + e < end)
+		row[q0 + e] = row[q0 + e] + v[e];
+    } else {
+	if constexpr (VEC == 8) {
+	    if (q0 + VEC <= end) {				/* acc rows are 32-byte aligned, q0 a multiple of 8 */
+		int4 *a = reinterpret_cast<int4 *>(acc + q0);
+#pragma unroll
+		for (int h = 0; h < 2; h++) {			/* a half at a time: fewer live registers */
+		    int4 t;
+		    t.x = v[4 * h], t.y = v[4 * h + 1], t.z = v[4 * h + 2], t.w = v[4 * h + 3];
+		    if (mode != TX_MIX_STORE) {
+			const int4 x = a[h];
+			t.x += x.x, t.y += x.y, t.z += x.z, t.w += x.w;
+		    }
+		    if (mode != TX_MIX_LAST) {
+			a[h] = t;
+		    } else {
+			v[4 * h] = (T)min(max(t.x, -32768), 32767);
+			v[4 * h + 1] = (T)min(max(t.y, -32768), 32767);
+			v[4 * h + 2] = (T)min(max(t.z, -32768), 32767);
+			v[4 * h + 3] = (T)min(max(t.w, -32768), 32767);
+		    }
+		}
+		if (mode == TX_MIX_LAST)
+		    tx_store<T, VEC>(row, q0, end, v);
+		return;
+	    }
+	}
+	for (int e = 0; e < VEC; e++) {
+	    if (q0 + e < end) {
+		int sum = (int)v[e];
+		if (mode != TX_MIX_STORE)
+		    sum += acc[q0 + e];
+		if (mode == TX_MIX_LAST)
+		    v[e] = (T)min(max(sum, -32768), 32767);
+		else
+		    acc[q0 + e] = sum;
+	    }
+	}
+	if (mode == TX_MIX_LAST)
+	    tx_store<T, VEC>(row, q0, end, v);
+    }
+}
+
 /* samples [from, to) of the row (from a multiple of VEC): the tones [lo, hi) are in the ring,
- * tones end at sample `sig_end`, zeros follow */
-template <typename T, int VEC, bool LUT>
+ * tones end at sample `sig_end`, zeros follow.  MIX: stored as pass `mode` of a mixed row. */
+template <typename T, int VEC, bool LUT, bool MIX = false>
 __device__ __forceinline__ void tx_write(const fsk_b200_tx_plan &P, const T *lut, const float4 *ring,
-	unsigned lo, unsigned hi, unsigned sig_end, T *row, unsigned from, unsigned to, unsigned lane)
+	unsigned lo, unsigned hi, unsigned sig_end, T *row, unsigned from, unsigned to, unsigned lane,
+	int *acc = nullptr, unsigned mode = 0)
 {
     for (unsigned q0 = from + lane * VEC; q0 < to; q0 += 32 * VEC) {
+	if constexpr (MIX) {
+	    /* a vector of zeros adds nothing to what the row (or acc) already holds */
+	    if (q0 >= sig_end && (mode == TX_MIX_ADD || (sizeof(T) == 4 && mode == TX_MIX_LAST)))
+		continue;
+	}
 	T v[VEC];
 	unsigned idx = lo, next = 0xffffffffu;
 	float wave = 0.0f, cph = 0.0f;
@@ -1067,45 +1148,46 @@ __device__ __forceinline__ void tx_write(const fsk_b200_tx_plan &P, const T *lut
 	    }
 	    v[e] = tx_sample<T, LUT>(P, lut, q - start, wave, cph);
 	}
-	tx_store<T, VEC>(row, q0, to, v);
+	if constexpr (MIX)
+	    tx_mix_store<T, VEC>(row, acc, q0, to, v, mode);
+	else
+	    tx_store<T, VEC>(row, q0, to, v);
     }
 }
 
-template <typename T, int VEC, bool LUT>
-__global__ void __launch_bounds__(TX_WARPS * 32, 8) k_tx_synth(const __grid_constant__ fsk_b200_tx_plan P,
-	const __grid_constant__ fsk_b200_tx_io io, const T *__restrict__ lut_global, unsigned lut_in_smem)
+/* One stream (or channel) of k_tx_synth.  MIX (implies TONES): channel s is one pass of a mixed row -- a fresh state and FSK_B200_TX_FINAL, row
+ * exactly io.cap samples long (io.cap = 0 included) and stored as pass `mode`; a disabled channel sends
+ * no tone but still does its pass's part (the first pass writes the whole row, the last one saturates
+ * the int16 sums); out_len[s] = lead_in[s] + the signal, uncut by cap, 0 when disabled. */
+template <typename T, int VEC, bool LUT, bool TONES, bool MIX>
+__device__ __forceinline__ void tx_stream(const fsk_b200_tx_plan &P, const fsk_b200_tx_io &io, const T *lut,
+	const unsigned *btab, float4 *ring, unsigned *wring, unsigned lane, size_t s, T *row, int *acc,
+	unsigned mode)
 {
-    FSK_DYN_SMEM(smem);
-    T *lut_s = reinterpret_cast<T *>(smem);
-    const unsigned lut_bytes = lut_in_smem ? ((P.lut_len * (unsigned)sizeof(T) + 15u) & ~15u) : 0u;
-    unsigned *btab = reinterpret_cast<unsigned *>(reinterpret_cast<unsigned char *>(smem) + lut_bytes);
-    float4 *rings = reinterpret_cast<float4 *>(btab + 96);
-    unsigned *wrings = reinterpret_cast<unsigned *>(rings + TX_WARPS * TX_RING);
-    if (lut_in_smem)
-	for (unsigned i = threadIdx.x; i < P.lut_len; i += blockDim.x)
-	    lut_s[i] = lut_global[i];
-    if (P.encoder == FSK_B200_ENCODE_BAUDOT)
-	for (unsigned i = threadIdx.x; i < 96; i += blockDim.x)
-	    btab[i] = fsk_enc_baudot_entry((int)i);
-    __syncthreads();
-    const T *lut = lut_in_smem ? lut_s : lut_global;
-
-    const unsigned lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const size_t s = (size_t)blockIdx.x * TX_WARPS + warp;
-    if (s >= io.nstreams)
-	return;						/* whole warps leave together */
-    float4 *ring = rings + warp * TX_RING;
-    unsigned *wring = wrings + warp * TX_WRING;
-    T *row = reinterpret_cast<T *>(io.out) + s * io.out_stride;
+    float f_mark = P.f_mark, f_space = P.f_space;
+    bool off = false;
+    if constexpr (TONES) {
+	f_mark = io.tones[2 * s];
+	f_space = io.tones[2 * s + 1];
+	if (!(f_mark > 0.0f && f_mark < INFINITY && f_space > 0.0f && f_space < INFINITY)) {
+	    if constexpr (!MIX) {
+		if (lane == 0)
+		    io.out_len[s] = 0;
+		return;						/* the whole warp */
+	    }
+	    off = true;
+	}
+    }
 
     fsk_b200_tx_state st = { 0.0f, 0u, 0u, 0u };
     if (io.states)
 	st = io.states[s];
     const unsigned flags = io.states ? io.flags : FSK_B200_TX_FINAL;
     const unsigned tpf = P.tones_per_frame;
-    const unsigned n_in = P.encoder == FSK_B200_ENCODE_WORDS ? io.nwords
+    const unsigned n_in = off ? 0u : P.encoder == FSK_B200_ENCODE_WORDS ? io.nwords
 	    : io.text_len[s] < io.text_stride ? io.text_len[s] : (unsigned)io.text_stride;
-    const unsigned lead = io.lead_in ? min(io.lead_in[s], io.cap) : 0u;
+    const unsigned lead_in = MIX && io.lead_in && !off ? io.lead_in[s] : 0u;
+    const unsigned lead = MIX ? min(lead_in, io.cap) : io.lead_in ? min(io.lead_in[s], io.cap) : 0u;
 
     /* the tone sequence, src/minimodem.c:202-237, :246-247, :60-66 */
     const unsigned nS = lead ? 1u : 0u;
@@ -1115,7 +1197,7 @@ __global__ void __launch_bounds__(TX_WARPS * 32, 8) k_tx_synth(const __grid_cons
     const unsigned tx_after = n_in ? 2u : nI ? 1u : st.transmitting;
     const unsigned nT = (flags & FSK_B200_TX_FINAL) && tx_after ? P.trailer : 0u;
     const unsigned d0 = nS + nL + nP;			/* the first tone of the data frames */
-    const float mark_idle = P.invert_start_stop ? P.f_space : P.f_mark;
+    const float mark_idle = P.invert_start_stop ? f_space : f_mark;
 
     unsigned nread = 0, nenc = 0, charset = st.baudot_charset;
     float cphase = st.cphase;
@@ -1200,17 +1282,17 @@ __global__ void __launch_bounds__(TX_WARPS * 32, 8) k_tx_synth(const __grid_cons
 		const unsigned word = sync ? P.sync_byte : wring[((k - nP) / tpf) % TX_WRING];
 		const int msb = sync ? 0 : P.msb_first;
 		if (P.has_start && b-- == 0) {
-		    freq = P.invert_start_stop ? P.f_mark : P.f_space, dur = P.start;
+		    freq = P.invert_start_stop ? f_mark : f_space, dur = P.start;
 		} else if (b < P.n_data_bits) {
 		    const unsigned bit = msb ? (word >> (P.n_data_bits - b - 1)) & 1u : (word >> b) & 1u;
-		    freq = bit ? P.f_mark : P.f_space, dur = P.bit;
+		    freq = bit ? f_mark : f_space, dur = P.bit;
 		} else {
-		    freq = P.invert_start_stop ? P.f_space : P.f_mark, dur = P.stop;
+		    freq = P.invert_start_stop ? f_space : f_mark, dur = P.stop;
 		}
 	    } else if ((k -= nP + nD) < nI) {
 		freq = mark_idle, dur = P.idle;			/* idle tone, :233-236 */
 	    } else {
-		freq = P.f_mark, dur = P.bit;			/* trailer, :65-66 */
+		freq = f_mark, dur = P.bit;			/* trailer, :65-66 */
 	    }
 	}
 	const unsigned end = tx_scan_add(dur, lane);
@@ -1232,24 +1314,79 @@ __global__ void __launch_bounds__(TX_WARPS * 32, 8) k_tx_synth(const __grid_cons
 	    ring[(G + lane) % TX_RING] = make_float4(__uint_as_float(start), wave, my_cph, 0.0f);
 	__syncwarp();
 	const bool last = G + nb >= total;
-	unsigned to = last ? (cap ? cap : sig_end) : sig_end / VEC * VEC;
-	if (cap)
+	unsigned to = last ? (MIX || cap ? cap : sig_end) : sig_end / VEC * VEC;
+	if (MIX || cap)
 	    to = min(to, cap);
 	const unsigned hi = G + nb;
-	tx_write<T, VEC, LUT>(P, lut, ring, hi > TX_RING ? hi - TX_RING : 0u, hi, sig_end, row, written, to, lane);
+	tx_write<T, VEC, LUT, MIX>(P, lut, ring, hi > TX_RING ? hi - TX_RING : 0u, hi, sig_end, row, written, to, lane,
+		acc, mode);
 	written = max(written, to);
 	__syncwarp();
-	if (last || (cap && written >= cap))
+	/* a mixed channel goes on past the row without writing: its out_len is the uncut length */
+	if (last || (!MIX && cap && written >= cap))
 	    break;
     }
-    if (cap && written < cap)				/* no tones at all: a silent row */
-	tx_write<T, VEC, LUT>(P, lut, ring, 0u, 0u, 0u, row, written, cap, lane);
-    if (io.states && lane == 0) {
+    if ((MIX || cap) && written < cap)			/* no tones at all: a silent row */
+	tx_write<T, VEC, LUT, MIX>(P, lut, ring, 0u, 0u, 0u, row, written, cap, lane, acc, mode);
+    if constexpr (MIX) {
+	if (lane == 0) {
+	    const unsigned long long n = off ? 0ull : (unsigned long long)(sig_end - lead) + lead_in;
+	    io.out_len[s] = n > 0xffffffffull ? 0xffffffffu : (uint32_t)n;
+	}
+    } else if (io.states && lane == 0) {
 	st.cphase = cphase;
 	st.baudot_charset = charset;
 	st.transmitting = flags & FSK_B200_TX_FINAL ? 0u : tx_after;	/* :71 */
 	io.states[s] = st;
 	io.out_len[s] = sig_end;
+    }
+}
+
+/* TONES: stream s sends on io.tones[s] = (mark Hz, space Hz) instead of the plan's pair; a stream whose
+ * pair has a frequency that is not finite or not > 0 is skipped (out_len 0, row and state untouched).
+ * The arithmetic per tone is the fixed pair's, so a pair gives the audio of an engine built for it.
+ * MIX: one warp per row r of io.nstreams / io.channels_per_row rows; its channels r*k .. r*k + k-1 run
+ * one after the other, each adding its samples to the row (tx_mix_store), with a __syncwarp between
+ * passes: which lane writes a sample depends on each channel's batch edges. */
+template <typename T, int VEC, bool LUT, bool TONES, bool MIX>
+__global__ void __launch_bounds__(TX_WARPS * 32, 8) k_tx_synth(const __grid_constant__ fsk_b200_tx_plan P,
+	const __grid_constant__ fsk_b200_tx_io io, const T *__restrict__ lut_global, unsigned lut_in_smem)
+{
+    FSK_DYN_SMEM(smem);
+    T *lut_s = reinterpret_cast<T *>(smem);
+    const unsigned lut_bytes = lut_in_smem ? ((P.lut_len * (unsigned)sizeof(T) + 15u) & ~15u) : 0u;
+    unsigned *btab = reinterpret_cast<unsigned *>(reinterpret_cast<unsigned char *>(smem) + lut_bytes);
+    float4 *rings = reinterpret_cast<float4 *>(btab + 96);
+    unsigned *wrings = reinterpret_cast<unsigned *>(rings + TX_WARPS * TX_RING);
+    if (lut_in_smem)
+	for (unsigned i = threadIdx.x; i < P.lut_len; i += blockDim.x)
+	    lut_s[i] = lut_global[i];
+    if (P.encoder == FSK_B200_ENCODE_BAUDOT)
+	for (unsigned i = threadIdx.x; i < 96; i += blockDim.x)
+	    btab[i] = fsk_enc_baudot_entry((int)i);
+    __syncthreads();
+    const T *lut = lut_in_smem ? lut_s : lut_global;
+
+    const unsigned lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    float4 *ring = rings + warp * TX_RING;
+    unsigned *wring = wrings + warp * TX_WRING;
+    const size_t w = (size_t)blockIdx.x * TX_WARPS + warp;
+    if constexpr (MIX) {
+	const unsigned k = io.channels_per_row;
+	if (w >= io.nstreams / k)
+	    return;						/* whole warps leave together */
+	T *row = reinterpret_cast<T *>(io.out) + w * io.out_stride;
+	int *acc = io.acc ? io.acc + w * io.acc_stride : nullptr;
+	for (unsigned j = 0; j < k; j++) {
+	    const unsigned mode = k == 1 ? TX_MIX_ONLY : j == 0 ? TX_MIX_STORE : j + 1 == k ? TX_MIX_LAST : TX_MIX_ADD;
+	    tx_stream<T, VEC, LUT, TONES, MIX>(P, io, lut, btab, ring, wring, lane, w * k + j, row, acc, mode);
+	    __syncwarp();
+	}
+    } else {
+	if (w >= io.nstreams)
+	    return;						/* whole warps leave together */
+	T *row = reinterpret_cast<T *>(io.out) + w * io.out_stride;
+	tx_stream<T, VEC, LUT, TONES, MIX>(P, io, lut, btab, ring, wring, lane, w, row, nullptr, 0u);
     }
 }
 /* ------------------------------------------------------------------------ */
@@ -2606,10 +2743,11 @@ extern "C" void fsk_b200_cuda_free(void *d)
     cudaFree(d);
 }
 
-template <typename T>
+template <typename T, bool TONES, bool MIX = false>
 static void tx_launch(const fsk_b200_tx_plan *p, const void *lut, const fsk_b200_tx_io *io, cudaStream_t st)
 {
-    const unsigned blocks = (unsigned)((io->nstreams + TX_WARPS - 1) / TX_WARPS);
+    const size_t warps = MIX ? io->nstreams / io->channels_per_row : io->nstreams;	/* a warp per row when mixing */
+    const unsigned blocks = (unsigned)((warps + TX_WARPS - 1) / TX_WARPS);
     /* the sine table goes to shared memory when it is small (16 KB at the default --lut=4096) */
     const unsigned lut_bytes = p->lut_len * (unsigned)sizeof(T);
     const unsigned in_smem = p->lut_len && lut_bytes <= 32768u;
@@ -2619,13 +2757,13 @@ static void tx_launch(const fsk_b200_tx_plan *p, const void *lut, const fsk_b200
     const bool wide = ((uintptr_t)io->out & 15u) == 0 && (io->out_stride * sizeof(T)) % 16u == 0;
     const T *l = (const T *)lut;
     if (wide && p->lut_len)
-	FSK_LAUNCH((k_tx_synth<T, 16 / sizeof(T), true>), blocks, TX_WARPS * 32, smem, st, *p, *io, l, in_smem);
+	FSK_LAUNCH((k_tx_synth<T, 16 / sizeof(T), true, TONES, MIX>), blocks, TX_WARPS * 32, smem, st, *p, *io, l, in_smem);
     else if (wide)
-	FSK_LAUNCH((k_tx_synth<T, 16 / sizeof(T), false>), blocks, TX_WARPS * 32, smem, st, *p, *io, l, in_smem);
+	FSK_LAUNCH((k_tx_synth<T, 16 / sizeof(T), false, TONES, MIX>), blocks, TX_WARPS * 32, smem, st, *p, *io, l, in_smem);
     else if (p->lut_len)
-	FSK_LAUNCH((k_tx_synth<T, 1, true>), blocks, TX_WARPS * 32, smem, st, *p, *io, l, in_smem);
+	FSK_LAUNCH((k_tx_synth<T, 1, true, TONES, MIX>), blocks, TX_WARPS * 32, smem, st, *p, *io, l, in_smem);
     else
-	FSK_LAUNCH((k_tx_synth<T, 1, false>), blocks, TX_WARPS * 32, smem, st, *p, *io, l, in_smem);
+	FSK_LAUNCH((k_tx_synth<T, 1, false, TONES, MIX>), blocks, TX_WARPS * 32, smem, st, *p, *io, l, in_smem);
 }
 
 extern "C" int fsk_b200_cuda_tx_synth(const fsk_b200_tx_plan *p, const void *lut, const fsk_b200_tx_io *io,
@@ -2633,10 +2771,55 @@ extern "C" int fsk_b200_cuda_tx_synth(const fsk_b200_tx_plan *p, const void *lut
 {
     if (io->nstreams == 0)
 	return 0;
-    if (p->float_samples)
-	tx_launch<float>(p, lut, io, (cudaStream_t)stream);
+    if (io->channels_per_row) {
+	/* mixed rows: float32 sums in the rows themselves; int16 sums of k > 1 channels are exact in an
+	 * int32 scratch row each, held for the launch only */
+	fsk_b200_tx_io m = *io;
+	const size_t nrows = io->nstreams / io->channels_per_row;
+	void *scratch = NULL;
+	if (!p->float_samples && io->channels_per_row > 1 && io->cap) {
+	    m.acc_stride = ((size_t)io->cap + 7) & ~(size_t)7;
+	    const size_t bytes = nrows * m.acc_stride * sizeof(int32_t);
+#ifdef FSK_EMU
+	    cudaError_t e = cudaMalloc(&scratch, bytes);
+#else
+	    cudaError_t e = cudaMallocAsync(&scratch, bytes, (cudaStream_t)stream);
+#endif
+	    if (e != cudaSuccess) {
+		fsk_b200_set_error("tx mix: %zu bytes of int32 sums: %s", bytes, cudaGetErrorString(e));
+		cudaGetLastError();
+		return -ENOMEM;
+	    }
+	    m.acc = (int32_t *)scratch;
+	}
+	if (p->float_samples)
+	    tx_launch<float, true, true>(p, lut, &m, (cudaStream_t)stream);
+	else
+	    tx_launch<int16_t, true, true>(p, lut, &m, (cudaStream_t)stream);
+	g_launches++;
+	cudaError_t e = cudaGetLastError();
+	if (scratch) {
+#ifdef FSK_EMU
+	    cudaFree(scratch);
+#else
+	    cudaFreeAsync(scratch, (cudaStream_t)stream);
+#endif
+	}
+	if (e != cudaSuccess) {
+	    fsk_b200_set_error("tx launch: %s", cudaGetErrorString(e));
+	    return -EIO;
+	}
+	return 0;
+    }
+    /* the pair per stream is its own instance: the fixed-pair instances keep their code */
+    if (p->float_samples && io->tones)
+	tx_launch<float, true>(p, lut, io, (cudaStream_t)stream);
+    else if (p->float_samples)
+	tx_launch<float, false>(p, lut, io, (cudaStream_t)stream);
+    else if (io->tones)
+	tx_launch<int16_t, true>(p, lut, io, (cudaStream_t)stream);
     else
-	tx_launch<int16_t>(p, lut, io, (cudaStream_t)stream);
+	tx_launch<int16_t, false>(p, lut, io, (cudaStream_t)stream);
     g_launches++;
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) {

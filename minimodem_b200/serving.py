@@ -29,7 +29,9 @@ fsk_b200_rx_batch_channels, and text and decoder state per channel, [nstreams*k,
 Per call one fsk_b200_tx_text_batch: the reference transmitter (src/minimodem.c:114-250) for each
 stream's bytes, its tone phase, Baudot charset and carrier state carried on the device, so the
 audio does not depend on how the text was cut into feeds.  With idle=True a stream that has no
-bytes in a feed sends the reference's idle tone, as the reference does when its input pipe pauses."""
+bytes in a feed sends the reference's idle tone, as the reference does when its input pipe pauses.
+With tones=pairs (a float32 tensor [nstreams, 2] from TxEngine.tone_pairs) every stream sends on its own
+-M / -S pair: fsk_b200_tx_text_batch_tones, the tensor read at every feed and at finish."""
 import ctypes as C
 
 from . import api
@@ -109,7 +111,7 @@ class LiveReceiver:
 
 class LiveTransmitter:
     def __init__(self, baudmode, sample_rate=48000, nstreams=1, max_text=256, float_samples=False, amplitude=1.0,
-                 lut=4096, idle=True, device=None, **overrides):
+                 lut=4096, idle=True, device=None, tones=None, **overrides):
         torch = api._torch()
         self.engine = api.TxEngine.for_mode(baudmode, sample_rate, amplitude, lut, float_samples, **overrides)
         self.nstreams, self.max_text = int(nstreams), int(max_text)
@@ -118,6 +120,12 @@ class LiveTransmitter:
         self.states = self.engine.new_states(self.nstreams, dev)
         self._empty = torch.zeros((self.nstreams, 1), dtype=torch.uint8, device=dev)
         self._zero = torch.zeros((self.nstreams,), dtype=torch.int32, device=dev)
+        # float32 [nstreams, 2] (TxEngine.tone_pairs): kept by reference and read at every call, so a caller
+        # may move a stream to another pair between feeds by writing into it
+        self.tones = None
+        if tones is not None:
+            assert tuple(tones.shape) == (self.nstreams, 2) and tones.dtype == torch.float32 and tones.is_contiguous()
+            self.tones = tones
 
     def feed(self, text, lengths=None):
         """text: uint8 CUDA tensor [nstreams, width <= max_text]; lengths: int32 CUDA tensor [nstreams]
@@ -127,8 +135,8 @@ class LiveTransmitter:
         assert text.shape[0] == self.nstreams and text.shape[1] <= self.max_text
         if lengths is None:
             lengths = torch.full((self.nstreams,), text.shape[1], dtype=torch.int32, device=text.device)
-        return self.engine.text_batch(text.contiguous(), lengths, self.states, self.flags)
+        return self.engine.text_batch(text.contiguous(), lengths, self.states, self.flags, tones=self.tones)
 
     def finish(self):
         """End of input: every stream that is transmitting sends the trailer (src/minimodem.c:246-249)."""
-        return self.engine.text_batch(self._empty, self._zero, self.states, api.TX_FINAL)
+        return self.engine.text_batch(self._empty, self._zero, self.states, api.TX_FINAL, tones=self.tones)
