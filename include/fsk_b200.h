@@ -87,6 +87,7 @@ void fsk_set_tones_by_bandshift(fsk_plan *fskp, unsigned int b_mark, int b_shift
 /* ======================================================================== */
 
 #define FSK_B200_MAX_BITS 64	/* assert at src/fsk.c:463 */
+#define FSK_B200_MAX_ROW_SAMPLES 0xfffffffcu	/* samples per row of the rx calls: 2^32 - 4 */
 
 /* What the reference's main() derives from `{baudmode}` + options before it
  * enters the rx loop (src/minimodem.c:819-965).  Fill by hand or with
@@ -252,9 +253,13 @@ int fsk_b200_find_frame_batch_bits(fsk_b200_engine *e, const float *samples,
  * all `nsamples_all` long; -EINVAL if that exceeds `stride`, per-stream lengths are
  * clamped to it).  Frame records go to frames[s*max_frames ...].  `states` (device,
  * one per stream) must be zeroed for a fresh stream; it is updated in place.
- * Limits: a row holds at most 2^32 - 4 samples (lengths and positions inside a row are
- * 32-bit; longer recordings are fed in pieces, see fsk_b200_stream_push), a call at most
- * 2^31 - 1 streams.
+ * Limits: a row holds at most FSK_B200_MAX_ROW_SAMPLES = 2^32 - 4 samples (lengths and positions
+ * inside a row are 32-bit; longer recordings are fed in pieces, see fsk_b200_stream_push), a call at
+ * most 2^31 - 1 streams.  nsamples_all above that limit returns -EINVAL with nothing launched, in
+ * every rx call (the tone, channel, auto-carrier, int16 and host forms too); a per-row length above
+ * it is clamped to it on the device, as it is clamped to `stride`.  Every position up to the limit
+ * decodes as it would at the start of a short row: the kernels' request and fill bookkeeping does not
+ * wrap near 2^32.
  * Output overflow: a stream that has written max_frames records stops there with done = 0
  * and nframes == max_frames; its position and loop state are saved, so it CAN be continued,
  * but only after the caller has consumed the records and set states[s].nframes back to 0
@@ -290,7 +295,8 @@ int fsk_b200_rx_batch_host(fsk_b200_engine *e, const float *host_samples, size_t
  *
  * fsk_b200_stream_push: per stream s, the unconsumed tail [states[s].pos, fill[s]) of row s moves to
  * the front, chunk_len[s] (or chunk_len_all when chunk_len is NULL) floats of chunk row s are
- * appended (what does not fit in `stride` is dropped and counted in dropped[s], if given),
+ * appended (what does not fit in min(stride, FSK_B200_MAX_ROW_SAMPLES) is dropped and counted in
+ * dropped[s], if given, so fill[s] never passes the rx calls' row limit),
  * fill[s] becomes the new length, and the state is set to pos = 0, nframes = 0, done = 0 with the
  * carrier/squelch/session fields untouched.  All pointers are device memory. */
 uint32_t fsk_b200_stream_window(const fsk_b200_rx_params *p);

@@ -120,7 +120,9 @@ __device__ __forceinline__ float confidence_from_scratch(float2 *scr, unsigned n
 /* GENERIC path                                                             */
 /* ======================================================================== */
 
-/* straight from global memory, zero beyond the valid length */
+/* straight from global memory, zero beyond the valid length.  Callers index it from the search position
+ * (x = the row + pos, n = what is left of the row), so that base + offset stays small: an absolute index
+ * near 2^32 would wrap past n and read the row's start */
 struct GlobalSrc {
     const float *x;
     unsigned n;
@@ -1486,17 +1488,18 @@ __device__ __forceinline__ void ring_block_at(unsigned dst, const float *__restr
     }
 }
 
-/* a block that reaches past the valid length n: bytes at or past n arrive as zeros */
+/* a block that reaches past the valid length n: bytes at or past n arrive as zeros.  `first` is 64-bit:
+ * the ring holds zeros past the end of a row, and a row may end just below 2^32 */
 template <int G>
 __device__ __forceinline__ void ring_block_tail(const Ring rg, unsigned ring_s, unsigned foff,
-	const float *__restrict__ x, unsigned n, unsigned first, unsigned g)
+	const float *__restrict__ x, unsigned n, unsigned long long first, unsigned g)
 {
     constexpr int CPL = (int)(RING_BLOCK / 4u) / G;
 #pragma unroll
     for (int k = 0; k < CPL; k++) {
 	const unsigned c = 4u * (g + (unsigned)k * G);
-	const unsigned i = first + c;
-	const unsigned valid = i + 4u <= n ? 16u : (i < n ? (n - i) * 4u : 0u);
+	const unsigned long long i = first + c;
+	const unsigned valid = i + 4u <= n ? 16u : (i < n ? (n - (unsigned)i) * 4u : 0u);
 	const float *sp = valid ? x + i : x;
 	ldgsts16_zfill(ring_s + (foff + c) * 4u, sp, valid);
 	if (foff + c < rg.pad)
@@ -1601,14 +1604,14 @@ __device__ __forceinline__ void ring_block16(unsigned ring_s, unsigned foff, con
 /* the same for a block that reaches past the valid length n: bytes at or past n arrive as zeros */
 template <int G>
 __device__ __forceinline__ void ring_block16_tail(unsigned ring_s, unsigned foff, const int16_t *__restrict__ x,
-	unsigned n, unsigned first, unsigned g)
+	unsigned n, unsigned long long first, unsigned g)
 {
 #pragma unroll
     for (int c0 = 0; c0 < 16; c0 += G) {
 	const unsigned c = (unsigned)c0 + g;
 	if (G <= 16 || c < 16u) {
-	    const unsigned i = first + 8u * c;
-	    const unsigned valid = i + 8u <= n ? 16u : (i < n ? (n - i) * 2u : 0u);
+	    const unsigned long long i = first + 8u * c;
+	    const unsigned valid = i + 8u <= n ? 16u : (i < n ? (n - (unsigned)i) * 2u : 0u);
 	    ldgsts16_zfill(ring_s + foff * 4u + 256u + 16u * c,
 		    reinterpret_cast<const float *>(valid ? x + i : x), valid);
 	}
@@ -1664,13 +1667,14 @@ struct GlobalSrc16 {
     }
 };
 
-/* plain zero fill of absolute indices [from, to) (any alignment) by the group */
+/* plain zero fill of absolute indices [from, to) (any alignment) by the group; 64-bit, as the zeros past
+ * the end of a row may lie beyond 2^32 */
 template <int G>
 __device__ __forceinline__ void ring_zero(const Ring rg, unsigned pos, unsigned pos_off,
-	unsigned from, unsigned to, unsigned g)
+	unsigned long long from, unsigned long long to, unsigned g)
 {
-    for (unsigned i = from + g; i < to; i += G) {
-	int off0 = (int)pos_off + (int)(i - pos);
+    for (unsigned long long i = from + g; i < to; i += G) {
+	int off0 = (int)pos_off + (int)(i - pos);	/* i - pos >= -3, below two ring lengths */
 	if (off0 < 0)
 	    off0 += (int)rg.R;
 	unsigned off = (unsigned)off0;

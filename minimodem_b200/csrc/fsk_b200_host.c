@@ -606,6 +606,15 @@ static int check_layout(const float *samples, size_t stride)
     return 0;
 }
 
+/* positions inside a row are 32-bit: the rx kernels take at most FSK_B200_MAX_ROW_SAMPLES per row */
+static int check_row_limit(const char *what, uint32_t nsamples_all)
+{
+    if (nsamples_all > FSK_B200_MAX_ROW_SAMPLES) {
+	fsk_b200_set_error("%s: nsamples_all (%u) exceeds the row limit of 2^32 - 4 samples", what, nsamples_all);
+	return -EINVAL;
+    }
+    return 0;
+}
 int fsk_b200_find_frame_batch(fsk_b200_engine *e, const float *samples, size_t nstreams,
 	size_t stride, const uint32_t *offset, const uint32_t *nvalid,
 	const uint32_t *try_first, const uint32_t *try_max, const uint32_t *try_step,
@@ -656,6 +665,8 @@ int fsk_b200_rx_batch(fsk_b200_engine *e, const float *samples, size_t nstreams,
 	fsk_b200_set_error("rx_batch: NULL argument");
 	return -EINVAL;
     }
+    if ((rc = check_row_limit("rx_batch", nsamples_all)))
+	return rc;
     if (!nsamples && (size_t)nsamples_all > stride) {
 	fsk_b200_set_error("rx_batch: nsamples_all (%u) exceeds the row stride (%zu)", nsamples_all, stride);
 	return -EINVAL;
@@ -682,6 +693,8 @@ int fsk_b200_rx_batch_s16(fsk_b200_engine *e, const int16_t *samples, size_t nst
 	fsk_b200_set_error("rx_batch_s16: NULL argument");
 	return -EINVAL;
     }
+    if (check_row_limit("rx_batch_s16", nsamples_all))
+	return -EINVAL;
     if ((!nsamples && (size_t)nsamples_all > stride) || nstreams > 0x7fffffffu) {
 	fsk_b200_set_error("rx_batch_s16: nsamples_all (%u) exceeds the row stride (%zu), or too many streams",
 		nsamples_all, stride);
@@ -795,6 +808,8 @@ static int rx_batch_auto_any(fsk_b200_engine *e, const void *samples, int elem, 
 	fsk_b200_set_error("rx_batch_auto: NULL argument");
 	return -EINVAL;
     }
+    if (check_row_limit("rx_batch_auto", nsamples_all))
+	return -EINVAL;
     if ((!nsamples && (size_t)nsamples_all > stride) || nstreams > 0x7fffffffu) {
 	fsk_b200_set_error("rx_batch_auto: nsamples_all (%u) exceeds the row stride (%zu), or too many streams",
 		nsamples_all, stride);
@@ -872,6 +887,8 @@ static int rx_batch_tones_any(fsk_b200_engine *e, const void *samples, int elem,
 	fsk_b200_set_error("rx_batch_tones: NULL argument");
 	return -EINVAL;
     }
+    if (check_row_limit("rx_batch_tones", nsamples_all))
+	return -EINVAL;
     if (!nsamples && (size_t)nsamples_all > stride) {
 	fsk_b200_set_error("rx_batch_tones: nsamples_all (%u) exceeds the row stride (%zu)", nsamples_all, stride);
 	return -EINVAL;
@@ -985,6 +1002,8 @@ int fsk_b200_rx_batch_host(fsk_b200_engine *e, const float *host_samples, size_t
 	fsk_b200_set_error("rx_batch_host: bad argument (stride must be a multiple of 4)");
 	return -EINVAL;
     }
+    if (check_row_limit("rx_batch_host", nsamples_all))
+	return -EINVAL;
     if ((size_t)nsamples_all > stride || nstreams > 0x7fffffffu) {
 	fsk_b200_set_error("rx_batch_host: nsamples_all (%u) exceeds the row stride (%zu), or too many streams",
 		nsamples_all, stride);
@@ -1057,6 +1076,8 @@ int fsk_b200_rx_batch_host_s16(fsk_b200_engine *e, const int16_t *host_samples, 
 	fsk_b200_set_error("rx_batch_host_s16: bad argument (stride must be a multiple of 4)");
 	return -EINVAL;
     }
+    if (check_row_limit("rx_batch_host_s16", nsamples_all))
+	return -EINVAL;
     return fsk_b200_cuda_rx_batch_host_s16(e->ce, &e->geom, &e->loopc, host_samples, nstreams,
 	    stride, nsamples_all, host_frames, max_frames, host_states);
 }

@@ -258,11 +258,12 @@ k_find_frame(const __grid_constant__ fsk_b200_geom geo, const float4 *__restrict
 	float ampl = 0.f, conf = 0.f;
 	unsigned start = 0;
 	if (tmax) {
+	    /* indexed from the 16-byte chunk of `off`: an absolute end index could pass 2^32 - 1 */
 	    const unsigned from = off & ~3u;
-	    const unsigned to = (off + tmax - 1u + geo.span + 3u) & ~3u;
-	    if (MODE == 0 && to - from <= ring_floats) {
+	    const unsigned len = ((off & 3u) + tmax - 1u + geo.span + 3u) & ~3u;
+	    if (MODE == 0 && len <= ring_floats) {
 		__syncwarp(gmask);
-		ring_issue<G>(rg, x, n, off, off & 3u, from, to, g);
+		ring_issue<G>(rg, x + from, n > from ? n - from : 0u, off & 3u, off & 3u, 0u, len, g);
 		cp_async_commit();
 		cp_async_wait<0>();
 		__syncwarp(gmask);
@@ -285,13 +286,13 @@ k_find_frame(const __grid_constant__ fsk_b200_geom geo, const float4 *__restrict
 			    g, gmask, lo, hi, am, nopend, a.bit_mags + (size_t)s * geo.n_bits);
 		}
 	    } else {
-		const GlobalSrc src = { x, n };
-		conf = find_frame<G, GlobalSrc>(src, off, geo, sel, sm.tw, sm.scr, g, gmask,
+		const GlobalSrc src = { x + off, n > off ? n - off : 0u };	/* indexed from `off` */
+		conf = find_frame<G, GlobalSrc>(src, 0u, geo, sel, sm.tw, sm.scr, g, gmask,
 			a.try_first[s], tmax, tstep, a.limit[s], bits, ampl, start);
 		if (a.bit_mags) {
 		    unsigned long long b2;
 		    float am;
-		    (void)frame_analyze<G, GlobalSrc>(src, off + start, geo, sel, sm.tw, sm.scr, g, gmask, b2, am,
+		    (void)frame_analyze<G, GlobalSrc>(src, start, geo, sel, sm.tw, sm.scr, g, gmask, b2, am,
 			    a.bit_mags + (size_t)s * geo.n_bits);
 		}
 	    }
@@ -371,8 +372,9 @@ k_rx(const __grid_constant__ fsk_b200_geom geo, const __grid_constant__ fsk_b200
 	const unsigned row = AUTO == 2 ? s / au.k : s;
 	const float *x = SRC ? (const float *)nullptr : a.samples + (size_t)row * a.stride;
 	const int16_t *x16 = SRC ? a.samples16 + (size_t)row * a.stride : (const int16_t *)nullptr;
-	/* a row never extends past its stride (per-row lengths are caller data) */
-	const unsigned n = (unsigned)min((size_t)(a.nsamples ? a.nsamples[row] : a.nsamples_all), a.stride);
+	/* a row never extends past its stride or the 32-bit position limit (per-row lengths are caller data) */
+	const unsigned n = (unsigned)min(min((size_t)(a.nsamples ? a.nsamples[row] : a.nsamples_all), a.stride),
+		(size_t)FSK_B200_MAX_ROW_SAMPLES);
 	fsk_b200_frame *out = a.frames + (size_t)s * a.max_frames;
 	/* 16-byte chunks of the source line up with 16-byte chunks of the ring: 4 floats, or 8 int16 */
 	constexpr unsigned AL = SRC ? 7u : 3u;
@@ -410,12 +412,20 @@ k_rx(const __grid_constant__ fsk_b200_geom geo, const __grid_constant__ fsk_b200
 	}
 
 	/* ring bookkeeping (MODE 0): ring offset of `pos`, and the absolute index up to
-	 * which the ring content has been REQUESTED (copies issued or zeros stored) */
+	 * which the ring content has been REQUESTED (copies issued or zeros stored).  The
+	 * requests run past the end of the row (zeros), and a row may end just below 2^32:
+	 * the absolute indices of the requests are 64-bit; pos < n <= 2^32 - 4 stays 32-bit */
 	unsigned pos_off = pos & AL;
-	unsigned filled = pos & ~AL;
-	unsigned conv = filled, coff = 0;		/* SRC 1: blocks up to `conv` (ring offset coff) are widened */
+	unsigned long long filled = pos & ~AL;
+	unsigned long long conv = filled;		/* SRC 1: blocks up to `conv` (ring offset coff) are widened */
+	unsigned coff = 0;
 	const unsigned need_max = lc.try_max_nocarrier - 1u + geo.span;
-	const unsigned n4 = (n + 3u) & ~3u;		/* rows are readable up to a multiple of 4 */
+	const unsigned n4 = (n + 3u) & ~3u;		/* rows are readable up to a multiple of 4 (n <= 2^32 - 4) */
+	/* the request limit of an iteration at p: its largest window `extra` samples further on, and no
+	 * more than the ring holds */
+	auto reach = [&](unsigned p, unsigned extra) {
+	    return min(((unsigned long long)p + extra + need_max + 3u) & ~3ull, (unsigned long long)(p & ~AL) + R);
+	};
 	const unsigned bar0 = smem_u32(sm.bars), bar1 = bar0 + 8u;
 	unsigned kphase = 0;				/* bulk fill: number of barrier phases armed */
 	bool tail_fix = false;				/* bulk fill: [n, n4) holds row padding, not zeros */
@@ -428,10 +438,10 @@ k_rx(const __grid_constant__ fsk_b200_geom geo, const __grid_constant__ fsk_b200
 	unsigned fdst = dst0;
 	const float *fsrc = SRC ? x : x + filled + 4u * g;
 	/* request the ring content up to absolute index `to` (rounded up to whole blocks) */
-	auto request_at = [&](unsigned to, unsigned base) {
+	auto request_at = [&](unsigned long long to, unsigned base) {
 	    /* FILL 0 only: whole blocks while they start below `to` and still fit in a ring
 	     * whose oldest live sample is `base` */
-	    const unsigned lim = min(to, (base & ~AL) + R - (RING_BLOCK - 1u));
+	    const unsigned long long lim = min(to, (unsigned long long)(base & ~AL) + R - (RING_BLOCK - 1u));
 	    while (filled < lim) {
 		if (SRC) {				/* int16 rows: landing zone = upper half of the block */
 		    if (filled + RING_BLOCK <= n)
@@ -450,19 +460,19 @@ k_rx(const __grid_constant__ fsk_b200_geom geo, const __grid_constant__ fsk_b200
 	    }
 	    cp_async_commit();
 	};
-	auto request = [&](unsigned to) {
+	auto request = [&](unsigned long long to) {
 	    if (FILL == 0) {
 		request_at(to, pos);
 	    } else {
-		const unsigned to_b = min(to, n4);
-		const unsigned from_b = min(filled, to_b);
+		const unsigned to_b = (unsigned)min(to, (unsigned long long)n4);
+		const unsigned from_b = (unsigned)min(filled, (unsigned long long)to_b);
 		if (g == 0)
 		    ring_issue_bulk(rg, x, pos, pos_off, from_b, to_b, (kphase & 1u) ? bar1 : bar0);
 		if (n < n4 && from_b < n4 && to_b == n4 && to_b > from_b)
 		    tail_fix = true;
 		kphase++;
-		if (to > max(filled, n4))		/* past the end of the stream: zeros */
-		    ring_zero<G>(rg, pos, pos_off, max(filled, n4), to, g);
+		if (to > max(filled, (unsigned long long)n4))	/* past the end of the stream: zeros */
+		    ring_zero<G>(rg, pos, pos_off, max(filled, (unsigned long long)n4), to, g);
 		if (to > filled)
 		    filled = to;
 	    }
@@ -511,7 +521,7 @@ k_rx(const __grid_constant__ fsk_b200_geom geo, const __grid_constant__ fsk_b200
 		}
 	    }
 	    __syncwarp(gmask);
-	    request(min((pos + need_max + 3u) & ~3u, (pos & ~AL) + R));
+	    request(reach(pos, 0u));
 	}
 
 	for (;;) {
@@ -576,10 +586,10 @@ k_rx(const __grid_constant__ fsk_b200_geom geo, const __grid_constant__ fsk_b200
 		 * below); whatever is missing -- first iteration of a launch, a restarted ring, the
 		 * bulk fill -- is requested here together with what the next iteration can need
 		 * (it starts at most `lookahead` samples further) */
-		const unsigned need_now = (pos + try_max - 1u + geo.span + 3u) & ~3u;
+		const unsigned long long need_now = ((unsigned long long)pos + try_max - 1u + geo.span + 3u) & ~3ull;
 		const bool late = filled < need_now;	/* part of this window is only now requested */
 		if (FILL != 0 || late)
-		    request(min((pos + lookahead + need_max + 3u) & ~3u, (pos & ~AL) + R));
+		    request(reach(pos, lookahead));
 		if (SRC) {
 		    /* int16 rows: everything requested so far has to land and be widened in place
 		     * before the search reads it (the float fill lets the search itself wait) */
@@ -599,8 +609,9 @@ k_rx(const __grid_constant__ fsk_b200_geom geo, const __grid_constant__ fsk_b200
 		} else
 		    settle(late);
 	    }
-	    const GlobalSrc gsrc = { x, n };
-	    const GlobalSrc16 gsrc16 = { x16, n };
+	    /* MODE 1 reads from `pos` on (pos < n here), so that its indices stay small */
+	    const GlobalSrc gsrc = { SRC ? x : x + pos, n - pos };
+	    const GlobalSrc16 gsrc16 = { SRC ? x16 + pos : x16, n - pos };
 
 	    unsigned long long bits;
 	    float amplitude, confidence;
@@ -718,18 +729,18 @@ k_rx(const __grid_constant__ fsk_b200_geom geo, const __grid_constant__ fsk_b200
 		    const unsigned npos = pos + adv;
 		    if (adv <= remaining && filled >= (npos & ~AL)) {
 			__syncwarp(gmask);	/* every read of this window precedes the copies */
-			request_at(min((npos + lookahead + need_max + 3u) & ~3u, (npos & ~AL) + R), npos);
+			request_at(reach(npos, lookahead), npos);
 		    }
 		    /* (The bulk fill of MODE 3 asks at the top of the next iteration.  Asking here as well
 		     * costs one more barrier phase per iteration, and the state machine below is too short
 		     * to hide a copy; the other warps of the SM do that already.) */
 		}
 	    } else if (SRC)
-		confidence = find_frame<G, GlobalSrc16>(gsrc16, pos, geo, sel, sm.tw, sm.scr, g, gmask,
+		confidence = find_frame<G, GlobalSrc16>(gsrc16, 0u, geo, sel, sm.tw, sm.scr, g, gmask,
 			try_first, try_max, try_step, lc.confidence_search_limit,
 			bits, amplitude, frame_start);
 	    else
-		confidence = find_frame<G, GlobalSrc>(gsrc, pos, geo, sel, sm.tw, sm.scr, g, gmask,
+		confidence = find_frame<G, GlobalSrc>(gsrc, 0u, geo, sel, sm.tw, sm.scr, g, gmask,
 			try_first, try_max, try_step, lc.confidence_search_limit,
 			bits, amplitude, frame_start);
 
@@ -788,11 +799,11 @@ k_rx(const __grid_constant__ fsk_b200_geom geo, const __grid_constant__ fsk_b200
 			frame_start2 = refined.start;
 			bits2 = ((unsigned long long)refined.bits_hi << 32) | refined.bits_lo;
 		    } else if (SRC)
-			confidence2 = find_frame<G, GlobalSrc16>(gsrc16, pos, geo, 0, sm.tw, sm.scr, g,
+			confidence2 = find_frame<G, GlobalSrc16>(gsrc16, 0u, geo, 0, sm.tw, sm.scr, g,
 				gmask, try_first, try_max, try_step, INFINITY,
 				bits2, amplitude2, frame_start2);
 		    else
-			confidence2 = find_frame<G, GlobalSrc>(gsrc, pos, geo, 0, sm.tw, sm.scr, g,
+			confidence2 = find_frame<G, GlobalSrc>(gsrc, 0u, geo, 0, sm.tw, sm.scr, g,
 				gmask, try_first, try_max, try_step, INFINITY,
 				bits2, amplitude2, frame_start2);
 		    if (confidence2 > confidence) {
@@ -1450,8 +1461,9 @@ __global__ void k_stream_push(float *__restrict__ samples, unsigned nrows, size_
     const unsigned tail = have - m;
     /* forward move in tiles of 32: a tile is read completely before it is written, and the
      * destination of tile k ends below the source of tile k+1 (dst = src - m, m >= 0) */
+    /* (64-bit counters: a 32-bit one stepping by 32 never passes a length above 2^32 - 32) */
     if (m)
-	for (unsigned t = 0; t < tail; t += 32) {
+	for (size_t t = 0; t < tail; t += 32) {
 	    const float v = t + lane < tail ? row[m + t + lane] : 0.f;
 	    __syncwarp();
 	    if (t + lane < tail)
@@ -1459,11 +1471,13 @@ __global__ void k_stream_push(float *__restrict__ samples, unsigned nrows, size_
 	    __syncwarp();
 	}
     unsigned len = chunk_len ? chunk_len[r] : chunk_len_all;
-    const unsigned room = (unsigned)min((size_t)0xffffffffu, stride) - tail;
+    /* a row holds at most min(stride, the rx calls' row limit); the rest is dropped */
+    const unsigned cap = (unsigned)min((size_t)FSK_B200_MAX_ROW_SAMPLES, stride);
+    const unsigned room = tail < cap ? cap - tail : 0u;
     const unsigned drop = len > room ? len - room : 0u;
     len -= drop;
     const float *src = chunk + (size_t)r * chunk_stride;
-    for (unsigned i = lane; i < len; i += 32)
+    for (size_t i = lane; i < len; i += 32)
 	row[tail + i] = src[i];
     __syncwarp();		/* every lane has read fill[r] and the states before any lane rewrites them */
     for (unsigned j = lane; j < k; j += 32) {

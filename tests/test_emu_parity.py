@@ -68,6 +68,15 @@ def test_launch_shapes_on_the_emulated_kernels(async_mode):
     assert " passed" in tail and "failed" not in tail
 
 
+@pytest.mark.parametrize("async_mode", ["eager", "late"])
+def test_long_rows_on_the_emulated_kernels(async_mode):
+    """tests/test_gpu_long_rows.py: a stream at the end of a row of up to 2^32 - 4 samples (a memfd aliased
+    over the whole range) decodes as at the start of a small row, in every rx family (the TMA bulk fill
+    excepted: not emulated); the row-limit refusals, the live push at the cap and the transmitter's bounds."""
+    tail = run_emulated("", async_mode, 900, module="test_gpu_long_rows.py")
+    assert " passed" in tail and "failed" not in tail
+
+
 def test_the_emulator_itself():
     """tests/emu/selftest.cpp: hand-verifiable kernels.  Group-masked shuffles / votes with
     divergent trip counts, block barriers and dynamic shared memory give CUDA's results; cp.async
