@@ -183,7 +183,8 @@ typedef struct fsk_b200_stream_state {
     uint32_t	noconfidence;	/* :1087 */
     float	track_amplitude;	/* :1132 */
     float	peak_confidence;	/* :1133 */
-    uint32_t	done;		/* loop ended: fewer than expect_nsamples remain (:1229) */
+    uint32_t	done;		/* loop ended: fewer than expect_nsamples remain (:1229); bit
+				 * FSK_B200_STREAM_ENDED: the stream's input has ended (live streams) */
     /* statistics of the open carrier session (:1082-1085) */
     uint64_t	carrier_nsamples;
     float	confidence_total;
@@ -196,6 +197,13 @@ typedef struct fsk_b200_stream_state {
     uint32_t	stat_searches;
     uint32_t	reserved;	/* engine-private search hint (part of the resumable state; keep it with the rest) */
 } fsk_b200_stream_state;
+/* A flag bit of fsk_b200_stream_state.done: this stream's input has ended.  Every rx call skips a stream
+ * whose done has any OTHER bit set, so the values the loop writes (0, 1) keep their meaning; a stream with
+ * only this bit runs, and stops by the loop's own rule (fewer than expect_nsamples left, src/minimodem.c:1229)
+ * whatever holdback the engine has -- the end-of-input pass of set_holdback(e, 0), for this stream alone.  The
+ * rx calls write the state back as done | FSK_B200_STREAM_ENDED: a flagged stream that fills max_frames stops
+ * with done == FSK_B200_STREAM_ENDED and resumes like any other overflowed stream. */
+#define FSK_B200_STREAM_ENDED 2u
 
 typedef struct fsk_b200_engine fsk_b200_engine;
 
@@ -289,6 +297,10 @@ int fsk_b200_rx_batch_host(fsk_b200_engine *e, const float *host_samples, size_t
  *       ... consume states[s].nframes records of each stream ...
  *   at the end of a stream: fsk_b200_engine_set_holdback(e, 0) and one more rx_batch (the reference's
  *   end-of-input rule: it analyses what is left as long as expect_nsamples remain, src/minimodem.c:1229)
+ *
+ * Streams that end and start on their own: fsk_b200_stream_push_events with FSK_B200_ROW_END on a row's last
+ * chunk sets FSK_B200_STREAM_ENDED in the states of the row, and the rx call that follows decodes that row to
+ * its end by the rule above while the other rows stay held back; FSK_B200_ROW_OPEN starts a new stream in a row.
  *
  * With the holdback at fsk_b200_stream_window() a search starts only when every sample it can touch
  * has arrived, so the records do not depend on how the stream was cut into chunks.
@@ -404,7 +416,26 @@ int fsk_b200_rx_batch_tones_s16(fsk_b200_engine *e, const int16_t *samples, size
  * gets pos = min(pos, old fill) - min(min(pos, old fill), m), nframes = 0, done = 0 (carrier, squelch and
  * session fields untouched).  A disabled channel therefore never pins its row's tail, and a channel
  * enabled later starts at the oldest sample the row still holds.  fsk_b200_stream_push is the k = 1,
- * tone_bands = NULL case.  -EINVAL for channels_per_row == 0 and nrows * channels_per_row > 2^31 - 1. */
+ * tone_bands = NULL case.  -EINVAL for channels_per_row == 0 and nrows * channels_per_row > 2^31 - 1.
+ *
+ * fsk_b200_stream_push_events: fsk_b200_stream_push_channels with row_events (device, uint8 [nrows]).  NULL is
+ * fsk_b200_stream_push_channels exactly (and fsk_b200_stream_push), done = 0 included.  With row_events every
+ * push keeps the flag, done &= FSK_B200_STREAM_ENDED in place of done = 0, so a caller that uses events passes
+ * them (zeros where nothing happens) at every push.  Per row r:
+ * - FSK_B200_ROW_OPEN: a new stream starts in row r.  The old content is discarded first (the old fill
+ *   counts as 0) and every channel state of the row is zeroed (a fresh stream, the flag clear); then the chunk
+ *   is appended as usual.  The push owns neither decoder states nor auto states: for an opened row the caller
+ *   zeroes the row's fsk_b200_decoder_state and fsk_b200_auto_state as well (all zeros = fresh).
+ * - FSK_B200_ROW_END: this chunk is the row's last.  After the append, every channel of the row (disabled
+ *   ones included) gets FSK_B200_STREAM_ENDED, and the next rx call decodes it to its end.
+ * - OPEN | END: a whole stream in one chunk.
+ * - A row whose channels all carry FSK_B200_STREAM_ENDED, without OPEN: the chunk is not appended and its
+ *   length is counted in dropped[r].  An ended stream's records and state (with the carrier session still
+ *   open at its end, which the reference prints at exit, :1469-1474) therefore stay as they are until the
+ *   row is reopened.
+ * Other bits of row_events are ignored.  Validation and refusals are fsk_b200_stream_push_channels'. */
+#define FSK_B200_ROW_OPEN 1u
+#define FSK_B200_ROW_END  2u
 int fsk_b200_rx_batch_channels(fsk_b200_engine *e, const float *samples, size_t nrows, size_t stride,
 	const uint32_t *nsamples, uint32_t nsamples_all, uint32_t channels_per_row, const uint32_t *tone_bands,
 	fsk_b200_frame *frames, uint32_t max_frames, fsk_b200_stream_state *states, void *stream);
@@ -415,6 +446,10 @@ int fsk_b200_stream_push_channels(float *samples, size_t nrows, size_t stride, u
 	uint32_t channels_per_row, const uint32_t *tone_bands, uint32_t nbands, fsk_b200_stream_state *states,
 	const float *chunk, size_t chunk_stride, const uint32_t *chunk_len, uint32_t chunk_len_all, uint32_t *dropped,
 	void *stream);
+int fsk_b200_stream_push_events(float *samples, size_t nrows, size_t stride, uint32_t *fill,
+	uint32_t channels_per_row, const uint32_t *tone_bands, uint32_t nbands, fsk_b200_stream_state *states,
+	const float *chunk, size_t chunk_stride, const uint32_t *chunk_len, uint32_t chunk_len_all, uint32_t *dropped,
+	const uint8_t *row_events, void *stream);
 
 /* N2 -- 16-bit PCM ingest (the reference transmitter's default sample format, read back by
  * its rx as float = short / 32768: src/simpleaudio-sndfile.c:43-57, src/minimodem.c:786-788).

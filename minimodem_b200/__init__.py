@@ -15,6 +15,6 @@ from .api import (  # noqa: F401
     DECODE_ASCII, DECODE_BINARY, DECODE_BAUDOT, DECODE_CALLERID, DECODE_UIC_GROUND, DECODE_UIC_TRAIN,
     DECODER_STATE_BYTES, DecoderState, decoder_for_mode, decode_max_bytes_per_frame, decode_max_bytes, detect_carrier_batch, stream_push, wav_locate,
     TxEngine, TxSignal, TxState, TX_STATE_BYTES, AUTO_STATE_BYTES, TX_IDLE_IF_EMPTY, TX_FINAL, ENCODE_ASCII8, ENCODE_BAUDOT,
-    encoder_for_mode, tx_max_samples, tone_bands,
+    encoder_for_mode, tx_max_samples, tone_bands, STREAM_ENDED, ROW_OPEN, ROW_END,
 )
 from .serving import LiveReceiver, LiveTransmitter  # noqa: F401,E402

@@ -74,6 +74,9 @@ STATE_DTYPE = np.dtype([("pos", "<u8"), ("nframes", "<u4"), ("carrier", "<u4"),
                         ("amplitude_total", "<f4"), ("nframes_decoded", "<u4"),
                         ("stat_candidates", "<u4"), ("stat_searches", "<u4"), ("reserved", "<u4")])
 STATE_WORDS = STATE_DTYPE.itemsize // 4
+# include/fsk_b200.h: the end-of-input flag of StreamState.done, and the row events of stream_push
+STREAM_ENDED = 2
+ROW_OPEN, ROW_END = 1, 2
 
 
 class TxConfig(C.Structure):
@@ -127,6 +130,7 @@ EXPORTS = [
     "fsk_b200_rx_batch_auto_s16", "fsk_b200_auto_stream_window",
     "fsk_b200_tone_bands", "fsk_b200_rx_batch_tones", "fsk_b200_rx_batch_tones_s16",
     "fsk_b200_rx_batch_channels", "fsk_b200_rx_batch_channels_s16", "fsk_b200_stream_push_channels",
+    "fsk_b200_stream_push_events",
 ]
 
 _lib = None
@@ -286,6 +290,8 @@ def lib():
                                                 C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_size_t,
                                                 C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p]
     L.fsk_b200_stream_push_channels.restype = C.c_int
+    L.fsk_b200_stream_push_events.argtypes = L.fsk_b200_stream_push_channels.argtypes[:-1] + [C.c_void_p, C.c_void_p]
+    L.fsk_b200_stream_push_events.restype = C.c_int
     L.fsk_b200_version.restype = C.c_char_p
     L.fsk_b200_launch_count.restype = C.c_ulonglong
     L.fsk_b200_last_error.restype = C.c_char_p
@@ -748,12 +754,18 @@ def detect_carrier_batch(fftsize, samples, nsamples, min_mag_threshold, offset=N
 
 
 def stream_push(rows, fill, states, chunk, chunk_len=None, dropped=None, stream=None, channels_per_row=1,
-                tone_bands=None, nbands=0):
+                tone_bands=None, nbands=0, row_events=None):
     """fsk_b200_stream_push on CUDA tensors: rows [n, stride] float32, fill [n] int32 (in/out), states
     [n, STATE_WORDS] int32 (in/out), chunk [n, chunk_stride] float32, chunk_len [n] int32 or an int.
     channels_per_row=k or tone_bands given (fsk_b200_stream_push_channels): states are per channel,
     [n*k, STATE_WORDS]; tone_bands (int32 [n*k, 2] or None) marks which channels are active (both bands
-    < nbands), and only those keep a row's tail."""
+    < nbands), and only those keep a row's tail.
+    row_events (fsk_b200_stream_push_events): uint8 CUDA tensor [n] of ROW_OPEN / ROW_END bits per row; with
+    it the push keeps the STREAM_ENDED flag of a state (without it, done = 0 as before).
+    ROW_OPEN starts a new stream in the row (old content discarded, its channel states zeroed; the caller
+    zeroes its decoder and auto states); ROW_END flags the row's channels STREAM_ENDED after the append, so
+    the next rx call decodes it to its end.  A row whose channels are all ended and not opened takes no
+    chunk: its length goes to dropped."""
     torch = _torch()
     # the C call takes raw pointers and row strides: the tensors must be what it assumes
     assert rows.is_contiguous() and rows.dtype == torch.float32 and chunk.is_contiguous() and chunk.dtype == torch.float32
@@ -764,6 +776,17 @@ def stream_push(rows, fill, states, chunk, chunk_len=None, dropped=None, stream=
     per = chunk_len if hasattr(chunk_len, "data_ptr") else None
     assert per is None or (per.dtype == torch.int32 and per.is_contiguous())
     common = 0 if per is not None else int(chunk.shape[1] if chunk_len is None else chunk_len)
+    if row_events is not None:
+        assert (row_events.dtype == torch.uint8 and row_events.is_contiguous()
+                and tuple(row_events.shape) == (n,))
+        assert tone_bands is None or (tone_bands.dtype == torch.int32 and tone_bands.is_contiguous()
+                                      and tuple(tone_bands.shape) == (n * k, 2))
+        rc = lib().fsk_b200_stream_push_events(_ptr(rows), n, stride, _ptr(fill), k, _ptr(tone_bands), int(nbands),
+                                               _ptr(states), _ptr(chunk), chunk.shape[1], _ptr(per), common,
+                                               _ptr(dropped), _ptr(row_events), _stream_handle(stream))
+        if rc:
+            _err("fsk_b200_stream_push_events", rc)
+        return
     if k == 1 and tone_bands is None:
         rc = lib().fsk_b200_stream_push(_ptr(rows), n, stride, _ptr(fill), _ptr(states), _ptr(chunk),
                                         chunk.shape[1], _ptr(per), common, _ptr(dropped), _stream_handle(stream))
@@ -800,11 +823,11 @@ def frames_to_numpy(frames):
 
 
 def check_not_truncated(states, max_frames):
-    """Raises if a stream stopped because its record buffer was full (done == 0 and nframes == max_frames,
-    include/fsk_b200.h): its decode is incomplete until the caller consumes the records, resets nframes and
-    calls rx_batch again.  Synchronises (reads the states back)."""
+    """Raises if a stream stopped because its record buffer was full (done == 0, bar the STREAM_ENDED flag,
+    and nframes == max_frames, include/fsk_b200.h): its decode is incomplete until the caller consumes the
+    records, resets nframes and calls rx_batch again.  Synchronises (reads the states back)."""
     st = states_to_numpy(states)
-    bad = np.nonzero((st["done"] == 0) & (st["nframes"] >= int(max_frames)))[0]
+    bad = np.nonzero(((st["done"] & ~np.uint32(STREAM_ENDED)) == 0) & (st["nframes"] >= int(max_frames)))[0]
     if bad.size:
         raise RuntimeError("rx_batch: %d stream(s) filled their %d-record buffer before the end of their samples "
                            "(first: stream %d); use RxEngine.max_frames(nsamples) or resume them" % (

@@ -550,6 +550,7 @@ fsk_b200_engine *fsk_b200_engine_new(const fsk_b200_rx_params *params)
     }
     e->loopc.frame_nsamples = params->frame_nsamples;
     e->loopc.expect_nsamples = params->expect_nsamples;
+    e->loopc.end_expect_nsamples = params->expect_nsamples;
     e->loopc.nsamples_overscan = params->nsamples_overscan;
     e->loopc.try_max_nocarrier = params->try_max_nocarrier;
     e->loopc.try_max_carrier = params->try_max_carrier;
@@ -957,10 +958,10 @@ int fsk_b200_engine_set_holdback(fsk_b200_engine *e, uint32_t nsamples)
     return 0;
 }
 
-int fsk_b200_stream_push_channels(float *samples, size_t nrows, size_t stride, uint32_t *fill,
+int fsk_b200_stream_push_events(float *samples, size_t nrows, size_t stride, uint32_t *fill,
 	uint32_t channels_per_row, const uint32_t *tone_bands, uint32_t nbands, fsk_b200_stream_state *states,
 	const float *chunk, size_t chunk_stride, const uint32_t *chunk_len, uint32_t chunk_len_all, uint32_t *dropped,
-	void *stream)
+	const uint8_t *row_events, void *stream)
 {
     if (channels_per_row == 0 || nrows > 0x7fffffffu / channels_per_row) {
 	fsk_b200_set_error("stream_push: channels_per_row (%u) is 0, or more than 2^31 - 1 channels",
@@ -981,7 +982,16 @@ int fsk_b200_stream_push_channels(float *samples, size_t nrows, size_t stride, u
 	return -ENODEV;
     }
     return fsk_b200_cuda_stream_push(samples, nrows, stride, fill, channels_per_row, tone_bands, nbands, states,
-	    chunk, chunk_stride, chunk_len, chunk_len_all, dropped, stream);
+	    chunk, chunk_stride, chunk_len, chunk_len_all, dropped, row_events, stream);
+}
+
+int fsk_b200_stream_push_channels(float *samples, size_t nrows, size_t stride, uint32_t *fill,
+	uint32_t channels_per_row, const uint32_t *tone_bands, uint32_t nbands, fsk_b200_stream_state *states,
+	const float *chunk, size_t chunk_stride, const uint32_t *chunk_len, uint32_t chunk_len_all, uint32_t *dropped,
+	void *stream)
+{
+    return fsk_b200_stream_push_events(samples, nrows, stride, fill, channels_per_row, tone_bands, nbands, states,
+	    chunk, chunk_stride, chunk_len, chunk_len_all, dropped, NULL, stream);
 }
 
 int fsk_b200_stream_push(float *samples, size_t nstreams, size_t stride, uint32_t *fill,

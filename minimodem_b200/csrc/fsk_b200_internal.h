@@ -37,6 +37,8 @@ typedef struct fsk_b200_loopc {
     unsigned int try_max_nocarrier, try_max_carrier;
     float	confidence_threshold, confidence_search_limit;
     unsigned int slide;			/* 1: the per-candidate rx kernel runs its fine searches by sliding (geom.tw_entries covers it) */
+    unsigned int end_expect_nsamples;	/* the loop's own stop rule (:1229), never raised: the bound of a stream
+					 * whose state carries FSK_B200_STREAM_ENDED */
 } fsk_b200_loopc;
 
 /* ---- shared-segment search plan (the "multi" rx kernel) --------------------------------------
@@ -213,7 +215,8 @@ int  fsk_b200_cuda_rx_batch_tones(void *ce, const fsk_b200_geom *g, const fsk_b2
 /* live rows: k channels (states) per row, tone_bands (device, optional) [nrows * k][2] */
 int  fsk_b200_cuda_stream_push(float *samples, size_t nrows, size_t stride, uint32_t *fill, unsigned int k,
 	const uint32_t *tone_bands, unsigned int nbands, fsk_b200_stream_state *states, const float *chunk,
-	size_t chunk_stride, const uint32_t *chunk_len, uint32_t chunk_len_all, uint32_t *dropped, void *stream);
+	size_t chunk_stride, const uint32_t *chunk_len, uint32_t chunk_len_all, uint32_t *dropped,
+	const uint8_t *row_events, void *stream);
 /* the synthesis kernel; lut: device table of plan->lut_len float or int16 entries */
 int  fsk_b200_cuda_tx_synth(const fsk_b200_tx_plan *plan, const void *lut, const fsk_b200_tx_io *io,
 	void *stream);

@@ -366,8 +366,12 @@ k_rx(const __grid_constant__ fsk_b200_geom geo, const __grid_constant__ fsk_b200
     for (unsigned s = (blockIdx.x * wpb + warp) * spw + sidx; s < a.nstreams;
 	    s += gridDim.x * wpb * spw) {
 	fsk_b200_stream_state st = a.states[s];
-	if (st.done)
+	if (st.done & ~FSK_B200_STREAM_ENDED)
 	    continue;
+	/* an ended stream stops by the loop's own rule (:1229), the others by the engine's holdback (raised for
+	 * live streams, never below the rule).  The flag is read where the two differ, once a stream is within
+	 * the holdback of its end, so nothing of it is live across the search */
+	auto ended = [&]() { return (a.states[s].done & FSK_B200_STREAM_ENDED) != 0u; };
 	/* AUTO 2: the k channels of a row are consecutive streams; records, states and pairs stay per stream */
 	const unsigned row = AUTO == 2 ? s / au.k : s;
 	const float *x = SRC ? (const float *)nullptr : a.samples + (size_t)row * a.stride;
@@ -528,9 +532,11 @@ k_rx(const __grid_constant__ fsk_b200_geom geo, const __grid_constant__ fsk_b200
 	    if (pos >= n) { done = 1; break; }			/* :1176 */
 	    const unsigned remaining = n - pos;
 	    if (AUTO == 1) {
-		/* a live stream's holdback (lc.expect_nsamples raised above the loop's own rule) stops the
-		 * loop before the scan: the refill below must not see where the stream was cut */
-		if (lc.expect_nsamples > au.expect_nsamples && remaining < lc.expect_nsamples) { done = 1; break; }
+		/* a live stream's holdback (raised above the loop's own rule) stops the loop before the scan:
+		 * the refill below must not see where the stream was cut */
+		/* (the flag of the state loaded above: the re-read costs a spill in one int16 instance) */
+		if (lc.expect_nsamples > au.expect_nsamples && remaining < lc.expect_nsamples
+			&& !(st.done & FSK_B200_STREAM_ENDED)) { done = 1; break; }
 		if (vring > remaining)				/* (a state that does not fit this row) */
 		    vring = remaining;
 		if (vring < au.half_ring)			/* :1158-1174, the refill */
@@ -569,7 +575,7 @@ k_rx(const __grid_constant__ fsk_b200_geom geo, const __grid_constant__ fsk_b200
 		    }
 		}
 	    }
-	    if (remaining < lc.expect_nsamples) { done = 1; break; }	/* :1229 */
+	    if (remaining < lc.expect_nsamples && (remaining < lc.end_expect_nsamples || !ended())) { done = 1; break; }	/* :1229 */
 	    if (nframes >= a.max_frames)
 		break;						/* output full: resumable */
 
@@ -859,7 +865,7 @@ k_rx(const __grid_constant__ fsk_b200_geom geo, const __grid_constant__ fsk_b200
 	    st.confidence_total = confidence_total;
 	    st.amplitude_total = amplitude_total;
 	    st.nframes_decoded = nframes_decoded;
-	    st.done = done;
+	    st.done = done | (ended() ? FSK_B200_STREAM_ENDED : 0u);
 	    st.stat_candidates += ncand;
 	    st.stat_searches += nsearch;
 	    st.reserved = mhint ? 1u : 0u;
@@ -1433,20 +1439,37 @@ __global__ void k_s16_to_f32_scalar(const short *__restrict__ src, float *__rest
 /* ------------------------------------------------------------------------ */
 /* Row r carries the k channels (streams) r*k .. r*k + k-1.  The tail starts at m, the smallest
  * min(pos, fill) over the row's active channels (all of them when bands is NULL, else those with both
- * bands < nbands), or at fill when none is active; every channel is then rewound by m. */
+ * bands < nbands), or at fill when none is active; every channel is then rewound by m.
+ * Row events (events[r]; events NULL: the push as it was before them, done = 0): ROW_OPEN discards the
+ * row (old fill 0) and zeroes its channel states before the append; ROW_END flags every channel of the row
+ * FSK_B200_STREAM_ENDED after it; the flag survives the pushes that follow (done &= ENDED).  A row whose
+ * channels are all flagged takes no chunk unless it is opened: the chunk is counted in dropped[r] and the
+ * row, its fill and its states are left as they are. */
 __global__ void k_stream_push(float *__restrict__ samples, unsigned nrows, size_t stride,
 	uint32_t *__restrict__ fill, unsigned k, const uint32_t *__restrict__ bands, unsigned nbands,
 	fsk_b200_stream_state *__restrict__ states,
 	const float *__restrict__ chunk, size_t chunk_stride, const uint32_t *__restrict__ chunk_len,
-	uint32_t chunk_len_all, uint32_t *__restrict__ dropped)
+	uint32_t chunk_len_all, uint32_t *__restrict__ dropped, const uint8_t *__restrict__ events)
 {
     const unsigned lane = threadIdx.x & 31;
     const unsigned r = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     if (r >= nrows)
 	return;						/* whole warps leave together */
     float *row = samples + (size_t)r * stride;
-    const unsigned have = fill[r];
+    const unsigned ev = events ? events[r] : 0u;
+    const bool open = (ev & FSK_B200_ROW_OPEN) != 0u, end = (ev & FSK_B200_ROW_END) != 0u;
     fsk_b200_stream_state *const st = states + (size_t)r * k;
+    if (events && !open) {
+	bool live = false;
+	for (unsigned j = lane; j < k; j += 32)
+	    live = live || (st[j].done & FSK_B200_STREAM_ENDED) == 0u;
+	if (!__any_sync(0xffffffffu, live)) {		/* an ended stream's records are final */
+	    if (lane == 0 && dropped)
+		dropped[r] = chunk_len ? chunk_len[r] : chunk_len_all;
+	    return;
+	}
+    }
+    const unsigned have = open ? 0u : fill[r];		/* an opened row starts empty */
     const uint32_t *const bd = bands ? bands + 2u * (size_t)r * k : nullptr;
     unsigned m = 0xffffffffu;
     for (unsigned j = lane; j < k; j += 32) {
@@ -1481,11 +1504,17 @@ __global__ void k_stream_push(float *__restrict__ samples, unsigned nrows, size_
 	row[tail + i] = src[i];
     __syncwarp();		/* every lane has read fill[r] and the states before any lane rewrites them */
     for (unsigned j = lane; j < k; j += 32) {
-	const unsigned long long pos64 = st[j].pos;
-	const unsigned pos = pos64 < have ? (unsigned)pos64 : have;
-	st[j].pos = pos - min(pos, m);
-	st[j].nframes = 0;				/* the record buffer starts over */
-	st[j].done = 0;
+	if (open) {
+	    st[j] = fsk_b200_stream_state{};		/* a fresh stream */
+	} else {
+	    const unsigned long long pos64 = st[j].pos;
+	    const unsigned pos = pos64 < have ? (unsigned)pos64 : have;
+	    st[j].pos = pos - min(pos, m);
+	    st[j].nframes = 0;				/* the record buffer starts over */
+	    st[j].done = events ? st[j].done & FSK_B200_STREAM_ENDED : 0u;	/* the end of input stays */
+	}
+	if (end)
+	    st[j].done |= FSK_B200_STREAM_ENDED;
     }
     if (lane == 0) {
 	fill[r] = tail + len;
@@ -2603,17 +2632,20 @@ extern "C" int fsk_b200_cuda_s16_to_f32(const int16_t *src, float *dst, size_t n
     return 0;
 }
 
-/* one warp per row; k channels (states) per row, tone_bands optional ([nrows * k][2]) */
+/* one warp per row; k channels (states) per row, tone_bands optional ([nrows * k][2]), row_events optional
+ * ([nrows]) */
 extern "C" int fsk_b200_cuda_stream_push(float *samples, size_t nrows, size_t stride, uint32_t *fill,
 	unsigned k, const uint32_t *tone_bands, unsigned nbands, fsk_b200_stream_state *states, const float *chunk,
-	size_t chunk_stride, const uint32_t *chunk_len, uint32_t chunk_len_all, uint32_t *dropped, void *stream)
+	size_t chunk_stride, const uint32_t *chunk_len, uint32_t chunk_len_all, uint32_t *dropped,
+	const uint8_t *row_events, void *stream)
 {
     if (nrows == 0)
 	return 0;
     const unsigned threads = 128;
     const size_t blocks = (nrows * 32 + threads - 1) / threads;
     FSK_LAUNCH(k_stream_push, (unsigned)blocks, threads, 0, (cudaStream_t)stream, samples, (unsigned)nrows,
-	    stride, fill, k, tone_bands, nbands, states, chunk, chunk_stride, chunk_len, chunk_len_all, dropped);
+	    stride, fill, k, tone_bands, nbands, states, chunk, chunk_stride, chunk_len, chunk_len_all, dropped,
+	    row_events);
     g_launches++;
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) {

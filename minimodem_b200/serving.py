@@ -21,6 +21,16 @@ each fed row carries k channels (both directions of a duplex line, k signals of 
 (fsk_b200_stream_push_channels, where a disabled channel does not hold the row back), one
 fsk_b200_rx_batch_channels, and text and decoder state per channel, [nstreams*k, ...].
 
+Streams with lifetimes of their own (calls on a modem bank, a Caller-ID front end):
+
+    text, counts = rx.feed(chunk, lengths, opened=opened, ended=ended)   # bool CUDA tensors [nstreams]
+
+In one feed the opened rows start a new stream (their decoder and auto states zeroed on the device), every
+row's chunk is pushed with the row events of fsk_b200_stream_push_events, and an ended row (this chunk is its
+last) comes back decoded to its end by the reference's end-of-input rule while the other rows stay held back.
+A row that ended in an earlier feed and is not reopened returns count 0; its chunk is counted in rx.dropped,
+and its final state (with the carrier session still open at its end) stays in rx.states until it is reopened.
+
     tx = LiveTransmitter("rtty", sample_rate=8000, nstreams=4096, max_text=64)
     for text, lengths in source:                  # uint8 CUDA tensor [nstreams, <= max_text], int32 [nstreams]
         audio, counts = tx.feed(text, lengths)    # int16 (or float32) CUDA tensor [nstreams, row], int32 [nstreams]
@@ -73,11 +83,16 @@ class LiveReceiver:
         if tones is not None:
             assert tuple(tones.shape) == (nchannels, 2)
             self.tones = tones.to(device=dev, dtype=torch.int32).contiguous()
+        self._ended = None          # bool [nstreams]: rows whose stream has ended, once events are in use
 
-    def _step(self, chunk, lengths):
-        if self.k > 1:
+    def _step(self, chunk, lengths, events=None):
+        if events is None and self._ended is not None:
+            # once rows have ended, every push carries events, so that their flag survives
+            events = self._no_events
+        if self.k > 1 or events is not None:
             api.stream_push(self.rows, self.fill, self.states, chunk, lengths, dropped=self.dropped,
-                            channels_per_row=self.k, tone_bands=self.tones, nbands=self.engine.params.nbands)
+                            channels_per_row=self.k, tone_bands=self.tones, nbands=self.engine.params.nbands,
+                            row_events=events)
         else:
             api.stream_push(self.rows, self.fill, self.states, chunk, lengths, dropped=self.dropped)
         if self.tones is not None:
@@ -91,14 +106,43 @@ class LiveReceiver:
         else:
             frames, self.states = self.engine.rx_batch(self.rows, nsamples=self.stride, nsamples_each=self.fill,
                                                        max_frames=self.max_frames, states=self.states)
-        return self.engine.decode_batch(self.kind, frames, self.states, dstates=self.dstates,
+        states = self.states
+        if self._ended is not None:
+            # rows that ended in an earlier feed: the rx call skipped them, and their records were decoded then
+            torch = api._torch()
+            stale = self._ended.repeat_interleave(self.k)
+            states = torch.where(stale[:, None] & self._nframes_word, 0, self.states)
+        return self.engine.decode_batch(self.kind, frames, states, dstates=self.dstates,
                                         out_stride=self.row_bytes)
 
-    def feed(self, chunk, lengths=None):
+    def feed(self, chunk, lengths=None, opened=None, ended=None):
         """chunk: float32 CUDA tensor [nstreams, width <= max_chunk]; lengths: int32 CUDA tensor [nstreams]
-        (samples valid in each row of the chunk) or None = the whole width.  Returns (text, counts)."""
+        (samples valid in each row of the chunk) or None = the whole width.  opened / ended: bool CUDA tensors
+        [nstreams] or None: rows where a new stream starts with this chunk, rows whose stream ends with it
+        (both: a whole stream in one chunk).  Returns (text, counts)."""
         assert chunk.shape[0] == self.nstreams and chunk.shape[1] <= self.max_chunk
-        return self._step(chunk, lengths)
+        if opened is None and ended is None:
+            return self._step(chunk, lengths)
+        torch = api._torch()
+        dev = self.rows.device
+        no = torch.zeros((self.nstreams,), dtype=torch.bool, device=dev)
+        opened = no if opened is None else opened.to(device=dev, dtype=torch.bool)
+        ended = no if ended is None else ended.to(device=dev, dtype=torch.bool)
+        assert tuple(opened.shape) == (self.nstreams,) and tuple(ended.shape) == (self.nstreams,)
+        if self._ended is None:
+            self._ended = no.clone()
+            self._nframes_word = torch.zeros((1, api.STATE_WORDS), dtype=torch.bool, device=dev)
+            self._nframes_word[0, 2] = True         # StreamState.nframes
+            self._no_events = torch.zeros((self.nstreams,), dtype=torch.uint8, device=dev)
+        # the push owns the stream states of an opened row; the decoder and auto states are zeroed here
+        self.dstates.masked_fill_(opened.repeat_interleave(self.k)[:, None], 0)
+        if self.auto:
+            self.auto_states.masked_fill_(opened[:, None], 0)
+        self._ended &= ~opened
+        events = opened.to(torch.uint8) * api.ROW_OPEN + ended.to(torch.uint8) * api.ROW_END
+        out = self._step(chunk, lengths, events)
+        self._ended |= ended
+        return out
 
     def finish(self):
         """End of input: the reference's rule (it analyses what is left while expect_nsamples remain,
