@@ -486,13 +486,15 @@ class RxEngine:
             _err("fsk_b200_find_frame_batch", rc)
         return frames
 
-    def rx_batch(self, samples, nsamples=None, max_frames=None, frames=None, states=None,
-                 nsamples_each=None, stream=None):
-        """The rx loop over every row of `samples` ([nstreams, stride] float32 CUDA tensor).
-        Returns (frames [nstreams, max_frames, 5] int32, states [nstreams, STATE_WORDS] int32)."""
+    def _rx(self, name, samples, nstreams, nsamples, max_frames, frames, states, nsamples_each, stream,
+            before=(), after=None):
+        """The device rx calls: fsk_b200_<name>, or its _s16 form for int16 rows, with the records of the
+        longest row (max_frames) and fresh frames and states unless given.  before: the arguments between the
+        row lengths and the records; after(max_frames): those between the states and the stream.  Returns
+        (frames, states, after's tensors)."""
         torch = _torch()
         assert samples.is_cuda and samples.dtype in (torch.float32, torch.int16) and samples.is_contiguous()
-        nstreams, stride = samples.shape
+        nrows, stride = samples.shape
         n_all = int(nsamples if nsamples is not None else stride)
         if max_frames is None:
             max_frames = self.max_frames(n_all)
@@ -500,13 +502,21 @@ class RxEngine:
             frames = torch.empty((nstreams, max_frames, 5), dtype=torch.int32, device=samples.device)
         if states is None:
             states = torch.zeros((nstreams, STATE_WORDS), dtype=torch.int32, device=samples.device)
-        # int16 rows: fsk_b200_rx_batch_s16 (the PCM samples are widened inside the kernel's ring fill)
-        fn = lib().fsk_b200_rx_batch if samples.dtype == torch.float32 else lib().fsk_b200_rx_batch_s16
-        rc = fn(self._e, _ptr(samples), nstreams, stride, _ptr(nsamples_each), n_all,
-                _ptr(frames), max_frames, _ptr(states), _stream_handle(stream))
+        tail = after(max_frames) if after else ()
+        fn = getattr(lib(), "fsk_b200_" + name + ("" if samples.dtype == torch.float32 else "_s16"))
+        rc = fn(self._e, _ptr(samples), nrows, stride, _ptr(nsamples_each), n_all, *before, _ptr(frames), max_frames,
+                _ptr(states), *map(_ptr, tail), _stream_handle(stream))
         if rc:
-            _err("fsk_b200_rx_batch", rc)
-        return frames, states
+            _err("fsk_b200_" + name, rc)
+        return frames, states, tail
+
+    def rx_batch(self, samples, nsamples=None, max_frames=None, frames=None, states=None,
+                 nsamples_each=None, stream=None):
+        """The rx loop over every row of `samples` ([nstreams, stride] float32 CUDA tensor; int16 rows go
+        through fsk_b200_rx_batch_s16, widened inside the kernel's ring fill).
+        Returns (frames [nstreams, max_frames, 5] int32, states [nstreams, STATE_WORDS] int32)."""
+        return self._rx("rx_batch", samples, samples.shape[0], nsamples, max_frames, frames, states, nsamples_each,
+                        stream)[:2]
 
     def rx_batch_host(self, samples, nsamples=None, max_frames=None, frames_out=None, states_out=None):
         """Host arrays in, host records out (copies overlap demodulation inside the library).
@@ -588,28 +598,17 @@ class RxEngine:
         Returns (frames, states, auto_states), and with rec_band=True (or a [nstreams, max_frames] int32
         CUDA tensor) also the mark band of every record."""
         torch = _torch()
-        assert samples.is_cuda and samples.dtype in (torch.float32, torch.int16) and samples.is_contiguous()
-        nstreams, stride = samples.shape
-        n_all = int(nsamples if nsamples is not None else stride)
-        if max_frames is None:
-            max_frames = self.max_frames(n_all)
-        if frames is None:
-            frames = torch.empty((nstreams, max_frames, 5), dtype=torch.int32, device=samples.device)
-        if states is None:
-            states = torch.zeros((nstreams, STATE_WORDS), dtype=torch.int32, device=samples.device)
+        nstreams = samples.shape[0]
         if auto_states is None:
             auto_states = torch.zeros((nstreams, AUTO_STATE_BYTES), dtype=torch.uint8, device=samples.device)
         assert auto_states.dtype == torch.uint8 and tuple(auto_states.shape) == (nstreams, AUTO_STATE_BYTES)
-        bands = None
-        if rec_band is True:
-            bands = torch.zeros((nstreams, max_frames), dtype=torch.int32, device=samples.device)
-        elif rec_band is not False and rec_band is not None:
-            bands = rec_band
-        fn = lib().fsk_b200_rx_batch_auto if samples.dtype == torch.float32 else lib().fsk_b200_rx_batch_auto_s16
-        rc = fn(self._e, _ptr(samples), nstreams, stride, _ptr(nsamples_each), n_all, _ptr(frames), max_frames,
-                _ptr(states), _ptr(auto_states), _ptr(bands), _stream_handle(stream))
-        if rc:
-            _err("fsk_b200_rx_batch_auto", rc)
+
+        def after(max_frames):
+            if rec_band is True:
+                return auto_states, torch.zeros((nstreams, max_frames), dtype=torch.int32, device=samples.device)
+            return auto_states, (None if rec_band is False else rec_band)
+        frames, states, (_, bands) = self._rx("rx_batch_auto", samples, nstreams, nsamples, max_frames, frames, states,
+                                              nsamples_each, stream, after=after)
         if bands is None:
             return frames, states, auto_states
         return frames, states, auto_states, bands
@@ -647,33 +646,15 @@ class RxEngine:
         each, channel c = r*k + j reads row r with pair tone_bands[c] ([nrows*k, 2]); nsamples_each is per
         row, frames and states are per channel ([nrows*k, ...])."""
         torch = _torch()
-        assert samples.is_cuda and samples.dtype in (torch.float32, torch.int16) and samples.is_contiguous()
-        nrows, stride = samples.shape
         k = int(channels_per_row)
-        nstreams = nrows * k
+        nstreams = samples.shape[0] * k
         assert (tone_bands.is_cuda and tone_bands.dtype == torch.int32 and tone_bands.is_contiguous()
                 and tuple(tone_bands.shape) == (nstreams, 2))
-        n_all = int(nsamples if nsamples is not None else stride)
-        if max_frames is None:
-            max_frames = self.max_frames(n_all)
-        if frames is None:
-            frames = torch.empty((nstreams, max_frames, 5), dtype=torch.int32, device=samples.device)
-        if states is None:
-            states = torch.zeros((nstreams, STATE_WORDS), dtype=torch.int32, device=samples.device)
         if k == 1:
-            fn = lib().fsk_b200_rx_batch_tones if samples.dtype == torch.float32 else lib().fsk_b200_rx_batch_tones_s16
-            rc = fn(self._e, _ptr(samples), nrows, stride, _ptr(nsamples_each), n_all, _ptr(tone_bands),
-                    _ptr(frames), max_frames, _ptr(states), _stream_handle(stream))
-            if rc:
-                _err("fsk_b200_rx_batch_tones", rc)
-            return frames, states
-        fn = (lib().fsk_b200_rx_batch_channels if samples.dtype == torch.float32
-              else lib().fsk_b200_rx_batch_channels_s16)
-        rc = fn(self._e, _ptr(samples), nrows, stride, _ptr(nsamples_each), n_all, k, _ptr(tone_bands),
-                _ptr(frames), max_frames, _ptr(states), _stream_handle(stream))
-        if rc:
-            _err("fsk_b200_rx_batch_channels", rc)
-        return frames, states
+            return self._rx("rx_batch_tones", samples, nstreams, nsamples, max_frames, frames, states, nsamples_each,
+                            stream, before=(_ptr(tone_bands),))[:2]
+        return self._rx("rx_batch_channels", samples, nstreams, nsamples, max_frames, frames, states, nsamples_each,
+                        stream, before=(k, _ptr(tone_bands)))[:2]
 
     def set_holdback(self, nsamples):
         """fsk_b200_engine_set_holdback: searches start only with this many samples left (0 = the

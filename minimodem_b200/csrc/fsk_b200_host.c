@@ -548,6 +548,8 @@ fsk_b200_engine *fsk_b200_engine_new(const fsk_b200_rx_params *params)
 	e->geom.rot[2] = (float)cos(as);
 	e->geom.rot[3] = (float)-sin(as);
     }
+    e->autoc.fftsize = params->fftsize;		/* the tone calls read these two as well */
+    e->autoc.nbands = params->nbands;
     e->loopc.frame_nsamples = params->frame_nsamples;
     e->loopc.expect_nsamples = params->expect_nsamples;
     e->loopc.end_expect_nsamples = params->expect_nsamples;
@@ -607,15 +609,6 @@ static int check_layout(const float *samples, size_t stride)
     return 0;
 }
 
-/* positions inside a row are 32-bit: the rx kernels take at most FSK_B200_MAX_ROW_SAMPLES per row */
-static int check_row_limit(const char *what, uint32_t nsamples_all)
-{
-    if (nsamples_all > FSK_B200_MAX_ROW_SAMPLES) {
-	fsk_b200_set_error("%s: nsamples_all (%u) exceeds the row limit of 2^32 - 4 samples", what, nsamples_all);
-	return -EINVAL;
-    }
-    return 0;
-}
 int fsk_b200_find_frame_batch(fsk_b200_engine *e, const float *samples, size_t nstreams,
 	size_t stride, const uint32_t *offset, const uint32_t *nvalid,
 	const uint32_t *try_first, const uint32_t *try_max, const uint32_t *try_step,
@@ -653,60 +646,76 @@ int fsk_b200_find_frame_batch_bits(fsk_b200_engine *e, const float *samples, siz
 	    nvalid, try_first, try_max, try_step, limit, expect_sel, frames, bit_mags, stream);
 }
 
+/* Every batched rx call: the checks in the order callers see them, then the launch.  `what` names the call's
+ * family in the error messages; host: the rows, records and states are in host memory. */
+static int rx_call(fsk_b200_engine *e, const char *what, int host, const fsk_b200_rx_call *c)
+{
+    if (c->kind == FSK_B200_RX_AUTO && (!e || !e->auto_on)) {
+	fsk_b200_set_error("%s: call fsk_b200_engine_set_auto_carrier first", what);
+	return -EINVAL;
+    }
+    if (c->kind == FSK_B200_RX_TONES) {
+	if (!e || !c->tone_bands) {
+	    fsk_b200_set_error("%s: NULL engine or tone_bands", what);
+	    return -EINVAL;
+	}
+	if (c->k == 0 || c->nrows > 0x7fffffffu / c->k) {
+	    fsk_b200_set_error("%s: channels_per_row (%u) is 0, or more than 2^31 - 1 streams", what, c->k);
+	    return -EINVAL;
+	}
+    }
+    if (c->nrows == 0)
+	return 0;
+    if (!e) {
+	fsk_b200_set_error("%s: NULL engine", what);
+	return -EINVAL;
+    }
+    const size_t align = !host && c->elem == 2 ? 8 : 4;
+    if (!c->samples || (!host && ((uintptr_t)c->samples & 15)) || (c->stride & (align - 1))) {
+	fsk_b200_set_error(host ? "%s: NULL samples, or a stride that is not a multiple of %zu samples"
+		: "%s: samples must be 16-byte aligned and the stride a multiple of %zu samples", what, align);
+	return -EINVAL;
+    }
+    if (!c->frames || !c->states || (c->kind == FSK_B200_RX_AUTO && !c->auto_states) || c->max_frames == 0) {
+	fsk_b200_set_error("%s: NULL argument", what);
+	return -EINVAL;
+    }
+    /* positions inside a row are 32-bit: the rx kernels take at most FSK_B200_MAX_ROW_SAMPLES per row */
+    if (c->nsamples_all > FSK_B200_MAX_ROW_SAMPLES) {
+	fsk_b200_set_error("%s: nsamples_all (%u) exceeds the row limit of 2^32 - 4 samples", what, c->nsamples_all);
+	return -EINVAL;
+    }
+    if (!c->nsamples && (size_t)c->nsamples_all > c->stride) {
+	fsk_b200_set_error("%s: nsamples_all (%u) exceeds the row stride (%zu)", what, c->nsamples_all, c->stride);
+	return -EINVAL;
+    }
+    if (c->nrows > 0x7fffffffu) {
+	fsk_b200_set_error("%s: at most 2^31-1 streams per call", what);
+	return -EINVAL;
+    }
+    const int rc = (host ? fsk_b200_cuda_rx_host : fsk_b200_cuda_rx)(e->ce, &e->geom, &e->loopc, &e->autoc, c);
+    if (rc == -ENOTSUP && c->kind == FSK_B200_RX_FIXED && c->elem == 2)
+	fsk_b200_set_error("rx_batch_s16: this mode's launch shape has no int16 build; widen with fsk_b200_s16_to_f32 "
+		"and call fsk_b200_rx_batch (fsk_b200_rx_batch_host_s16 does that by itself)");
+    return rc;
+}
+
 int fsk_b200_rx_batch(fsk_b200_engine *e, const float *samples, size_t nstreams, size_t stride,
 	const uint32_t *nsamples, uint32_t nsamples_all, fsk_b200_frame *frames,
 	uint32_t max_frames, fsk_b200_stream_state *states, void *stream)
 {
-    if (nstreams == 0)
-	return 0;
-    int rc = check_layout(samples, stride);
-    if (rc)
-	return rc;
-    if (!frames || !states || max_frames == 0) {
-	fsk_b200_set_error("rx_batch: NULL argument");
-	return -EINVAL;
-    }
-    if ((rc = check_row_limit("rx_batch", nsamples_all)))
-	return rc;
-    if (!nsamples && (size_t)nsamples_all > stride) {
-	fsk_b200_set_error("rx_batch: nsamples_all (%u) exceeds the row stride (%zu)", nsamples_all, stride);
-	return -EINVAL;
-    }
-    if (nstreams > 0x7fffffffu) {
-	fsk_b200_set_error("rx_batch: at most 2^31-1 streams per call");
-	return -EINVAL;
-    }
-    return fsk_b200_cuda_rx_batch(e->ce, &e->geom, &e->loopc, samples, nstreams, stride,
-	    nsamples, nsamples_all, frames, max_frames, states, stream);
+    return rx_call(e, "rx_batch", 0, &(fsk_b200_rx_call){ .kind = FSK_B200_RX_FIXED, .elem = 4, .samples = samples,
+	    .nrows = nstreams, .k = 1, .stride = stride, .nsamples = nsamples, .nsamples_all = nsamples_all,
+	    .frames = frames, .max_frames = max_frames, .states = states, .stream = stream });
 }
 
 int fsk_b200_rx_batch_s16(fsk_b200_engine *e, const int16_t *samples, size_t nstreams, size_t stride,
 	const uint32_t *nsamples, uint32_t nsamples_all, fsk_b200_frame *frames,
 	uint32_t max_frames, fsk_b200_stream_state *states, void *stream)
 {
-    if (nstreams == 0)
-	return 0;
-    if (!samples || ((uintptr_t)samples & 15) || (stride & 7)) {
-	fsk_b200_set_error("rx_batch_s16: samples must be 16-byte aligned and stride a multiple of 8 samples");
-	return -EINVAL;
-    }
-    if (!frames || !states || max_frames == 0) {
-	fsk_b200_set_error("rx_batch_s16: NULL argument");
-	return -EINVAL;
-    }
-    if (check_row_limit("rx_batch_s16", nsamples_all))
-	return -EINVAL;
-    if ((!nsamples && (size_t)nsamples_all > stride) || nstreams > 0x7fffffffu) {
-	fsk_b200_set_error("rx_batch_s16: nsamples_all (%u) exceeds the row stride (%zu), or too many streams",
-		nsamples_all, stride);
-	return -EINVAL;
-    }
-    int rc = fsk_b200_cuda_rx_batch_s16(e->ce, &e->geom, &e->loopc, samples, nstreams, stride,
-	    nsamples, nsamples_all, frames, max_frames, states, stream);
-    if (rc == -ENOTSUP)
-	fsk_b200_set_error("rx_batch_s16: this mode's launch shape has no int16 build; widen with fsk_b200_s16_to_f32 "
-		"and call fsk_b200_rx_batch (fsk_b200_rx_batch_host_s16 does that by itself)");
-    return rc;
+    return rx_call(e, "rx_batch_s16", 0, &(fsk_b200_rx_call){ .kind = FSK_B200_RX_FIXED, .elem = 2, .samples = samples,
+	    .nrows = nstreams, .k = 1, .stride = stride, .nsamples = nsamples, .nsamples_all = nsamples_all,
+	    .frames = frames, .max_frames = max_frames, .states = states, .stream = stream });
 }
 
 /* ---- --auto-carrier ------------------------------------------------------------ */
@@ -781,59 +790,30 @@ int fsk_b200_engine_set_auto_carrier(fsk_b200_engine *e, float threshold, int au
     e->autoc.threshold = threshold;
     e->autoc.scan_n = scan_n;
     e->autoc.b_shift = b_shift;
-    e->autoc.fftsize = p->fftsize;
-    e->autoc.nbands = p->nbands;
     e->autoc.half_ring = (unsigned)half_ring;
     e->autoc.expect_nsamples = p->expect_nsamples;
     e->auto_on = 1;
     return 0;
 }
 
-static int rx_batch_auto_any(fsk_b200_engine *e, const void *samples, int elem, size_t nstreams, size_t stride,
-	const uint32_t *nsamples, uint32_t nsamples_all, fsk_b200_frame *frames, uint32_t max_frames,
-	fsk_b200_stream_state *states, fsk_b200_auto_state *auto_states, uint32_t *rec_band, void *stream)
-{
-    if (!e || !e->auto_on) {
-	fsk_b200_set_error("rx_batch_auto: call fsk_b200_engine_set_auto_carrier first");
-	return -EINVAL;
-    }
-    if (nstreams == 0)
-	return 0;
-    const size_t align = elem == 2 ? 7 : 3;
-    if (!samples || ((uintptr_t)samples & 15) || (stride & align)) {
-	fsk_b200_set_error("rx_batch_auto: samples must be 16-byte aligned and the stride a multiple of %zu samples",
-		align + 1);
-	return -EINVAL;
-    }
-    if (!frames || !states || !auto_states || max_frames == 0) {
-	fsk_b200_set_error("rx_batch_auto: NULL argument");
-	return -EINVAL;
-    }
-    if (check_row_limit("rx_batch_auto", nsamples_all))
-	return -EINVAL;
-    if ((!nsamples && (size_t)nsamples_all > stride) || nstreams > 0x7fffffffu) {
-	fsk_b200_set_error("rx_batch_auto: nsamples_all (%u) exceeds the row stride (%zu), or too many streams",
-		nsamples_all, stride);
-	return -EINVAL;
-    }
-    return fsk_b200_cuda_rx_batch_auto(e->ce, &e->geom, &e->loopc, &e->autoc, samples, elem, nstreams, stride,
-	    nsamples, nsamples_all, frames, max_frames, states, auto_states, rec_band, stream);
-}
-
 int fsk_b200_rx_batch_auto(fsk_b200_engine *e, const float *samples, size_t nstreams, size_t stride,
 	const uint32_t *nsamples, uint32_t nsamples_all, fsk_b200_frame *frames, uint32_t max_frames,
 	fsk_b200_stream_state *states, fsk_b200_auto_state *auto_states, uint32_t *rec_band, void *stream)
 {
-    return rx_batch_auto_any(e, samples, 4, nstreams, stride, nsamples, nsamples_all, frames, max_frames, states,
-	    auto_states, rec_band, stream);
+    return rx_call(e, "rx_batch_auto", 0, &(fsk_b200_rx_call){ .kind = FSK_B200_RX_AUTO, .elem = 4, .samples = samples,
+	    .nrows = nstreams, .k = 1, .stride = stride, .nsamples = nsamples, .nsamples_all = nsamples_all,
+	    .frames = frames, .max_frames = max_frames, .states = states, .auto_states = auto_states,
+	    .rec_band = rec_band, .stream = stream });
 }
 
 int fsk_b200_rx_batch_auto_s16(fsk_b200_engine *e, const int16_t *samples, size_t nstreams, size_t stride,
 	const uint32_t *nsamples, uint32_t nsamples_all, fsk_b200_frame *frames, uint32_t max_frames,
 	fsk_b200_stream_state *states, fsk_b200_auto_state *auto_states, uint32_t *rec_band, void *stream)
 {
-    return rx_batch_auto_any(e, samples, 2, nstreams, stride, nsamples, nsamples_all, frames, max_frames, states,
-	    auto_states, rec_band, stream);
+    return rx_call(e, "rx_batch_auto", 0, &(fsk_b200_rx_call){ .kind = FSK_B200_RX_AUTO, .elem = 2, .samples = samples,
+	    .nrows = nstreams, .k = 1, .stride = stride, .nsamples = nsamples, .nsamples_all = nsamples_all,
+	    .frames = frames, .max_frames = max_frames, .states = states, .auto_states = auto_states,
+	    .rec_band = rec_band, .stream = stream });
 }
 
 /* ---- -M / -S per stream ------------------------------------------------------------ */
@@ -864,70 +844,40 @@ int fsk_b200_tone_bands(const fsk_b200_rx_params *p, float f_mark, float f_space
 }
 
 /* k channels per row (k = 1: the tone calls); pairs, records and states per channel */
-static int rx_batch_tones_any(fsk_b200_engine *e, const void *samples, int elem, size_t nrows, uint32_t k,
-	size_t stride, const uint32_t *nsamples, uint32_t nsamples_all, const uint32_t *tone_bands,
-	fsk_b200_frame *frames, uint32_t max_frames, fsk_b200_stream_state *states, void *stream)
-{
-    if (!e || !tone_bands) {
-	fsk_b200_set_error("rx_batch_tones: NULL engine or tone_bands");
-	return -EINVAL;
-    }
-    if (k == 0 || nrows > 0x7fffffffu / k) {
-	fsk_b200_set_error("rx_batch_tones: channels_per_row (%u) is 0, or more than 2^31 - 1 streams", k);
-	return -EINVAL;
-    }
-    if (nrows == 0)
-	return 0;
-    const size_t align = elem == 2 ? 7 : 3;
-    if (!samples || ((uintptr_t)samples & 15) || (stride & align)) {
-	fsk_b200_set_error("rx_batch_tones: samples must be 16-byte aligned and the stride a multiple of %zu samples",
-		align + 1);
-	return -EINVAL;
-    }
-    if (!frames || !states || max_frames == 0) {
-	fsk_b200_set_error("rx_batch_tones: NULL argument");
-	return -EINVAL;
-    }
-    if (check_row_limit("rx_batch_tones", nsamples_all))
-	return -EINVAL;
-    if (!nsamples && (size_t)nsamples_all > stride) {
-	fsk_b200_set_error("rx_batch_tones: nsamples_all (%u) exceeds the row stride (%zu)", nsamples_all, stride);
-	return -EINVAL;
-    }
-    return fsk_b200_cuda_rx_batch_tones(e->ce, &e->geom, &e->loopc, e->params.fftsize, e->params.nbands, samples,
-	    elem, nrows, k, stride, nsamples, nsamples_all, tone_bands, frames, max_frames, states, stream);
-}
-
 int fsk_b200_rx_batch_tones(fsk_b200_engine *e, const float *samples, size_t nstreams, size_t stride,
 	const uint32_t *nsamples, uint32_t nsamples_all, const uint32_t *tone_bands, fsk_b200_frame *frames,
 	uint32_t max_frames, fsk_b200_stream_state *states, void *stream)
 {
-    return rx_batch_tones_any(e, samples, 4, nstreams, 1, stride, nsamples, nsamples_all, tone_bands, frames,
-	    max_frames, states, stream);
+    return rx_call(e, "rx_batch_tones", 0, &(fsk_b200_rx_call){ .kind = FSK_B200_RX_TONES, .elem = 4, .samples = samples,
+	    .nrows = nstreams, .k = 1, .stride = stride, .nsamples = nsamples, .nsamples_all = nsamples_all,
+	    .frames = frames, .max_frames = max_frames, .states = states, .tone_bands = tone_bands, .stream = stream });
 }
 
 int fsk_b200_rx_batch_tones_s16(fsk_b200_engine *e, const int16_t *samples, size_t nstreams, size_t stride,
 	const uint32_t *nsamples, uint32_t nsamples_all, const uint32_t *tone_bands, fsk_b200_frame *frames,
 	uint32_t max_frames, fsk_b200_stream_state *states, void *stream)
 {
-    return rx_batch_tones_any(e, samples, 2, nstreams, 1, stride, nsamples, nsamples_all, tone_bands, frames,
-	    max_frames, states, stream);
+    return rx_call(e, "rx_batch_tones", 0, &(fsk_b200_rx_call){ .kind = FSK_B200_RX_TONES, .elem = 2, .samples = samples,
+	    .nrows = nstreams, .k = 1, .stride = stride, .nsamples = nsamples, .nsamples_all = nsamples_all,
+	    .frames = frames, .max_frames = max_frames, .states = states, .tone_bands = tone_bands, .stream = stream });
 }
 
 int fsk_b200_rx_batch_channels(fsk_b200_engine *e, const float *samples, size_t nrows, size_t stride,
 	const uint32_t *nsamples, uint32_t nsamples_all, uint32_t channels_per_row, const uint32_t *tone_bands,
 	fsk_b200_frame *frames, uint32_t max_frames, fsk_b200_stream_state *states, void *stream)
 {
-    return rx_batch_tones_any(e, samples, 4, nrows, channels_per_row, stride, nsamples, nsamples_all, tone_bands,
-	    frames, max_frames, states, stream);
+    return rx_call(e, "rx_batch_tones", 0, &(fsk_b200_rx_call){ .kind = FSK_B200_RX_TONES, .elem = 4, .samples = samples,
+	    .nrows = nrows, .k = channels_per_row, .stride = stride, .nsamples = nsamples, .nsamples_all = nsamples_all,
+	    .frames = frames, .max_frames = max_frames, .states = states, .tone_bands = tone_bands, .stream = stream });
 }
 
 int fsk_b200_rx_batch_channels_s16(fsk_b200_engine *e, const int16_t *samples, size_t nrows, size_t stride,
 	const uint32_t *nsamples, uint32_t nsamples_all, uint32_t channels_per_row, const uint32_t *tone_bands,
 	fsk_b200_frame *frames, uint32_t max_frames, fsk_b200_stream_state *states, void *stream)
 {
-    return rx_batch_tones_any(e, samples, 2, nrows, channels_per_row, stride, nsamples, nsamples_all, tone_bands,
-	    frames, max_frames, states, stream);
+    return rx_call(e, "rx_batch_tones", 0, &(fsk_b200_rx_call){ .kind = FSK_B200_RX_TONES, .elem = 2, .samples = samples,
+	    .nrows = nrows, .k = channels_per_row, .stride = stride, .nsamples = nsamples, .nsamples_all = nsamples_all,
+	    .frames = frames, .max_frames = max_frames, .states = states, .tone_bands = tone_bands, .stream = stream });
 }
 
 /* ---- live streams ------------------------------------------------------------ */
@@ -1006,21 +956,9 @@ int fsk_b200_rx_batch_host(fsk_b200_engine *e, const float *host_samples, size_t
 	size_t stride, uint32_t nsamples_all, fsk_b200_frame *host_frames, uint32_t max_frames,
 	fsk_b200_stream_state *host_states)
 {
-    if (nstreams == 0)
-	return 0;
-    if (!host_samples || !host_frames || !host_states || (stride & 3) || max_frames == 0) {
-	fsk_b200_set_error("rx_batch_host: bad argument (stride must be a multiple of 4)");
-	return -EINVAL;
-    }
-    if (check_row_limit("rx_batch_host", nsamples_all))
-	return -EINVAL;
-    if ((size_t)nsamples_all > stride || nstreams > 0x7fffffffu) {
-	fsk_b200_set_error("rx_batch_host: nsamples_all (%u) exceeds the row stride (%zu), or too many streams",
-		nsamples_all, stride);
-	return -EINVAL;
-    }
-    return fsk_b200_cuda_rx_batch_host(e->ce, &e->geom, &e->loopc, host_samples, nstreams,
-	    stride, nsamples_all, host_frames, max_frames, host_states);
+    return rx_call(e, "rx_batch_host", 1, &(fsk_b200_rx_call){ .kind = FSK_B200_RX_FIXED, .elem = 4,
+	    .samples = host_samples, .nrows = nstreams, .k = 1, .stride = stride, .nsamples_all = nsamples_all,
+	    .frames = host_frames, .max_frames = max_frames, .states = host_states });
 }
 
 int fsk_b200_s16_to_f32(const int16_t *src, float *dst, size_t nstreams, size_t stride, void *stream)
@@ -1080,16 +1018,9 @@ int fsk_b200_rx_batch_host_s16(fsk_b200_engine *e, const int16_t *host_samples, 
 	size_t stride, uint32_t nsamples_all, fsk_b200_frame *host_frames, uint32_t max_frames,
 	fsk_b200_stream_state *host_states)
 {
-    if (nstreams == 0)
-	return 0;
-    if (!host_samples || !host_frames || !host_states || (stride & 3) || max_frames == 0) {
-	fsk_b200_set_error("rx_batch_host_s16: bad argument (stride must be a multiple of 4)");
-	return -EINVAL;
-    }
-    if (check_row_limit("rx_batch_host_s16", nsamples_all))
-	return -EINVAL;
-    return fsk_b200_cuda_rx_batch_host_s16(e->ce, &e->geom, &e->loopc, host_samples, nstreams,
-	    stride, nsamples_all, host_frames, max_frames, host_states);
+    return rx_call(e, "rx_batch_host_s16", 1, &(fsk_b200_rx_call){ .kind = FSK_B200_RX_FIXED, .elem = 2,
+	    .samples = host_samples, .nrows = nstreams, .k = 1, .stride = stride, .nsamples_all = nsamples_all,
+	    .frames = host_frames, .max_frames = max_frames, .states = host_states });
 }
 
 int fsk_b200_decoder_for_mode(const char *baudmode, unsigned int n_data_bits, int binary_output)

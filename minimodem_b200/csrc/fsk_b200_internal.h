@@ -73,10 +73,6 @@ typedef struct fsk_b200_mplan {
     fsk_b200_mkind kind[4];
     uint32_t	always;		/* 1: every coarse search goes through the shared segments (no single-candidate fast path) */
 } fsk_b200_mplan;
-/* 0 and the plan if every search kind of this mode can run on `slots` period slots, else -1 */
-int fsk_b200_mplan_build(const fsk_b200_geom *g, const struct fsk_b200_loopc *lc, unsigned int slots,
-	fsk_b200_mplan *out);
-
 
 /* ---- chunk-prefix table search (the "prefix" rx kernel, k_rx MODE 3) ------------------------------
  * Once per rx-loop iteration the 32 lanes of a stream's warp demodulate the whole search span
@@ -152,6 +148,37 @@ typedef struct fsk_b200_tx_io {
     size_t	acc_stride;
 } fsk_b200_tx_io;
 
+/* --auto-carrier constants of an engine (fsk_b200_engine_set_auto_carrier) */
+typedef struct fsk_b200_auto_args {
+    float	threshold;		/* carrier_autodetect_threshold, > 0 */
+    float	scan_n;			/* min(nsamples_per_bit, fftsize), src/minimodem.c:1183-1185 */
+    int		b_shift;		/* :1200-1203 */
+    int		fftsize;		/* fftsize and nbands: the engine's, set without auto-carrier too */
+    unsigned int nbands;
+    unsigned int half_ring;		/* samplebuf_size / 2 */
+    unsigned int expect_nsamples;	/* the loop's own stop rule (:1229), below any holdback */
+} fsk_b200_auto_args;
+/* one batched rx call (fsk_b200_rx_batch and its siblings), checked by the host layer */
+enum { FSK_B200_RX_FIXED, FSK_B200_RX_AUTO, FSK_B200_RX_TONES };	/* the engine's pair, --auto-carrier, a pair per stream */
+typedef struct fsk_b200_rx_call {
+    int		kind, elem;		/* FSK_B200_RX_*; bytes per sample: 4 float32, 2 int16 */
+    const void	*samples;		/* [nrows][stride] */
+    size_t	nrows, stride;
+    unsigned int k;			/* channels (streams) per row: nrows * k streams */
+    const uint32_t *nsamples;		/* [nrows], or NULL: nsamples_all */
+    uint32_t	nsamples_all, max_frames;
+    fsk_b200_frame *frames;		/* [nrows * k][max_frames] */
+    fsk_b200_stream_state *states;	/* [nrows * k] */
+    const uint32_t *tone_bands;		/* TONES: [nrows * k][2] (mark band, space band) */
+    fsk_b200_auto_state *auto_states;	/* AUTO: [nrows] */
+    uint32_t	*rec_band;		/* AUTO, optional: [nrows][max_frames] */
+    void	*stream;
+} fsk_b200_rx_call;
+/* nothing below leaves the library: its exported functions are those of include/fsk_b200.h */
+#pragma GCC visibility push(hidden)
+/* 0 and the plan if every search kind of this mode can run on `slots` period slots, else -1 */
+int fsk_b200_mplan_build(const fsk_b200_geom *g, const struct fsk_b200_loopc *lc, unsigned int slots,
+	fsk_b200_mplan *out);
 void fsk_b200_set_error(const char *fmt, ...);
 
 /* host-side pure derivations (fsk_b200_host.c) */
@@ -171,17 +198,6 @@ int  fsk_b200_cuda_find_frame_batch(void *ce, const fsk_b200_geom *g, const floa
 	size_t nstreams, size_t stride, const uint32_t *offset, const uint32_t *nvalid,
 	const uint32_t *try_first, const uint32_t *try_max, const uint32_t *try_step,
 	const float *limit, const uint8_t *expect_sel, fsk_b200_frame *frames, float *bit_mags, void *stream);
-int  fsk_b200_cuda_rx_batch(void *ce, const fsk_b200_geom *g, const fsk_b200_loopc *lc,
-	const float *samples, size_t nstreams, size_t stride, const uint32_t *nsamples,
-	uint32_t nsamples_all, fsk_b200_frame *frames, uint32_t max_frames,
-	fsk_b200_stream_state *states, void *stream);
-int  fsk_b200_cuda_rx_batch_s16(void *ce, const fsk_b200_geom *g, const fsk_b200_loopc *lc,
-	const int16_t *samples, size_t nstreams, size_t stride, const uint32_t *nsamples,
-	uint32_t nsamples_all, fsk_b200_frame *frames, uint32_t max_frames,
-	fsk_b200_stream_state *states, void *stream);
-int  fsk_b200_cuda_rx_batch_host(void *ce, const fsk_b200_geom *g, const fsk_b200_loopc *lc,
-	const float *host_samples, size_t nstreams, size_t stride, uint32_t nsamples_all,
-	fsk_b200_frame *host_frames, uint32_t max_frames, fsk_b200_stream_state *host_states);
 /* single-stream helpers behind the drop-in API: host buffers in, host results out */
 int  fsk_b200_cuda_find_frame_one(void *ce, const fsk_b200_geom *g, const float *host_samples,
 	unsigned int nfloats, unsigned int try_first, unsigned int try_max, unsigned int try_step,
@@ -190,28 +206,13 @@ int  fsk_b200_cuda_band_mags(void *ce, int fftsize, const float *host_samples,
 	unsigned int nsamples, unsigned int nbands, float *host_mags);
 int  fsk_b200_cuda_detect_carrier_batch(int fftsize, const float *samples, size_t nstreams, size_t stride,
 	const uint32_t *offset, uint32_t nsamples, float min_mag_threshold, int32_t *out_band, void *stream);
-
-/* --auto-carrier constants of an engine (fsk_b200_engine_set_auto_carrier) */
-typedef struct fsk_b200_auto_args {
-    float	threshold;		/* carrier_autodetect_threshold, > 0 */
-    float	scan_n;			/* min(nsamples_per_bit, fftsize), src/minimodem.c:1183-1185 */
-    int		b_shift;		/* :1200-1203 */
-    int		fftsize;
-    unsigned int nbands;
-    unsigned int half_ring;		/* samplebuf_size / 2 */
-    unsigned int expect_nsamples;	/* the loop's own stop rule (:1229), below any holdback */
-} fsk_b200_auto_args;
 int  fsk_b200_cuda_set_unit_table(void *ce, int fftsize);
-int  fsk_b200_cuda_rx_batch_auto(void *ce, const fsk_b200_geom *g, const fsk_b200_loopc *lc,
-	const fsk_b200_auto_args *aa, const void *samples, int elem, size_t nstreams, size_t stride,
-	const uint32_t *nsamples, uint32_t nsamples_all, fsk_b200_frame *frames, uint32_t max_frames,
-	fsk_b200_stream_state *states, fsk_b200_auto_state *auto_states, uint32_t *rec_band, void *stream);
-/* -M / -S per channel: k channels per row, tone_bands (device) [nrows * k][2] (mark band, space band);
- * nsamples (device, optional) [nrows], frames and states per channel */
-int  fsk_b200_cuda_rx_batch_tones(void *ce, const fsk_b200_geom *g, const fsk_b200_loopc *lc, int fftsize,
-	unsigned int nbands, const void *samples, int elem, size_t nrows, unsigned int k, size_t stride,
-	const uint32_t *nsamples, uint32_t nsamples_all, const uint32_t *tone_bands, fsk_b200_frame *frames,
-	uint32_t max_frames, fsk_b200_stream_state *states, void *stream);
+/* a checked rx call on device buffers; -ENOTSUP, with nothing launched, where the shape has no such build */
+int  fsk_b200_cuda_rx(void *ce, const fsk_b200_geom *g, const fsk_b200_loopc *lc, const fsk_b200_auto_args *aa,
+	const fsk_b200_rx_call *c);
+/* the same over host buffers (fixed tones, nsamples NULL): slabs of rows through fsk_b200_cuda_rx */
+int  fsk_b200_cuda_rx_host(void *ce, const fsk_b200_geom *g, const fsk_b200_loopc *lc, const fsk_b200_auto_args *aa,
+	const fsk_b200_rx_call *c);
 /* live rows: k channels (states) per row, tone_bands (device, optional) [nrows * k][2] */
 int  fsk_b200_cuda_stream_push(float *samples, size_t nrows, size_t stride, uint32_t *fill, unsigned int k,
 	const uint32_t *tone_bands, unsigned int nbands, fsk_b200_stream_state *states, const float *chunk,
@@ -224,14 +225,12 @@ int  fsk_b200_cuda_tx_synth(const fsk_b200_tx_plan *plan, const void *lut, const
 void *fsk_b200_cuda_upload(const void *host, size_t bytes);
 void fsk_b200_cuda_free(void *dev);
 int  fsk_b200_cuda_s16_to_f32(const int16_t *src, float *dst, size_t nstreams, size_t stride, void *stream);
-int  fsk_b200_cuda_rx_batch_host_s16(void *ce, const fsk_b200_geom *g, const fsk_b200_loopc *lc,
-	const int16_t *host_samples, size_t nstreams, size_t stride, uint32_t nsamples_all,
-	fsk_b200_frame *host_frames, uint32_t max_frames, fsk_b200_stream_state *host_states);
 int  fsk_b200_cuda_decode(int kind, unsigned shift, unsigned n_data_bits, int msb_first, int do_rx_sync,
 	unsigned long long sync_byte, const fsk_b200_frame *frames, const fsk_b200_stream_state *states,
 	size_t nstreams, uint32_t max_frames, fsk_b200_decoder_state *dstates, uint8_t *out,
 	uint32_t out_stride, uint32_t *out_count, void *stream);
 unsigned long long fsk_b200_cuda_launch_count(void);
+#pragma GCC visibility pop
 
 #ifdef __cplusplus
 }

@@ -2185,7 +2185,7 @@ extern "C" int fsk_b200_cuda_find_frame_batch(void *p, const fsk_b200_geom *g, c
 
 template <int G, int W, int L, int MODE, int FILL, int SRC = 0, int AUTO = 0>
 static cudaError_t launch_rx_t(const Shape &sh, const CudaEngine *ce, const fsk_b200_loopc *lc,
-	const RxArgs &a, cudaStream_t st, const AutoArgs &au = AutoArgs())
+	const RxArgs &a, cudaStream_t st, const AutoArgs &au)
 {
     cudaError_t e = cudaFuncSetAttribute(k_rx<G, W, L, MODE, FILL, SRC, AUTO>,
 	    cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sh.smem);
@@ -2197,105 +2197,6 @@ static cudaError_t launch_rx_t(const Shape &sh, const CudaEngine *ce, const fsk_
 	    au);
     g_launches++;
     return cudaGetLastError();
-}
-
-/* elem 4: float32 rows; elem 2: int16 PCM rows, widened inside the kernel's ring fill.  -ENOTSUP when
- * the launch shape of this mode has no int16 build (the caller widens with fsk_b200_cuda_s16_to_f32). */
-static int rx_batch_any(CudaEngine *ce, const fsk_b200_geom *g, const fsk_b200_loopc *lc,
-	const void *samples, int elem, size_t nstreams, size_t stride, const uint32_t *nsamples,
-	uint32_t nsamples_all, fsk_b200_frame *frames, uint32_t max_frames,
-	fsk_b200_stream_state *states, void *stream)
-{
-    if (!ce->d_tw || ce->tw_n < g->tw_entries) {
-	fsk_b200_set_error("rx_batch: twiddle table not set");
-	return -EINVAL;
-    }
-    if (engine_device_check(ce, "rx_batch"))
-	return -EINVAL;
-    Shape sh;
-    const unsigned tmax = lc->try_max_nocarrier > lc->try_max_carrier
-	? lc->try_max_nocarrier : lc->try_max_carrier;
-    const unsigned max_advance = tmax - 1u + lc->frame_nsamples;	/* :1407, overscan >= 0 */
-    pick_shape(ce, g, tmax - 1u + g->span, max_advance, nstreams, &sh, lc);
-    fsk_b200_loopc lc_launch = *lc;
-    lc_launch.slide = sh.slide;
-    lc = &lc_launch;
-    const RxArgs a = { elem == 4 ? (const float *)samples : NULL, elem == 2 ? (const int16_t *)samples : NULL,
-	(unsigned)nstreams, stride, nsamples, nsamples_all, frames, max_frames, states };
-    cudaStream_t st = (cudaStream_t)stream;
-    cudaError_t e = cudaErrorInvalidValue;
-    bool launched = false;
-    if (elem == 2) {
-	if (sh.mode == 3) {
-#define X(WW) if (sh.W == WW) { e = launch_rx_t<32, WW, 1, 3, 0, 1>(sh, ce, lc, a, st); launched = true; }
-	    PFX_SLOTS(X)
-#undef X
-	} else if (sh.mode == 2) {
-#define X(GG, WW, LL) if (sh.G == GG && sh.W == WW && sh.L == LL) { e = launch_rx_t<GG, WW, LL, 2, 0, 1>(sh, ce, lc, a, st); launched = true; }
-	    MULTI_COMBOS(X)
-#undef X
-	} else if (sh.mode == 0) {
-#define X(GG, WW, LL) if (sh.G == GG && sh.W == WW && sh.L == LL) { e = launch_rx_t<GG, WW, LL, 0, 0, 1>(sh, ce, lc, a, st); launched = true; }
-	    S16_FAST_COMBOS(X)
-#undef X
-	} else {
-	    e = launch_rx_t<32, 1, 1, 1, 0, 1>(sh, ce, lc, a, st);
-	    launched = true;
-	}
-	if (!launched)
-	    return -ENOTSUP;
-    } else if (sh.mode == 3) {
-	/* one stream per warp: the ring is filled by bulk copies of the TMA engine (one elected lane, two to
-	 * four copies per iteration) unless FSK_B200_PFX_FILL=0 asks for the per-lane cp.async fill */
-	if (ce->pfx_fill) {
-#define X(WW) if (sh.W == WW) e = launch_rx_t<32, WW, 1, 3, 1>(sh, ce, lc, a, st);
-	    PFX_SLOTS(X)
-#undef X
-	} else {
-#define X(WW) if (sh.W == WW) e = launch_rx_t<32, WW, 1, 3, 0>(sh, ce, lc, a, st);
-	    PFX_SLOTS(X)
-#undef X
-	}
-    } else if (sh.mode == 2) {
-#define X(GG, WW, LL) if (sh.G == GG && sh.W == WW && sh.L == LL) e = launch_rx_t<GG, WW, LL, 2, 0>(sh, ce, lc, a, st);
-	MULTI_COMBOS(X)
-#undef X
-    } else if (sh.mode == 0) {
-#define X(GG, WW, LL) if (sh.G == GG && sh.W == WW && sh.L == LL) e = launch_rx_t<GG, WW, LL, 0, 0>(sh, ce, lc, a, st);
-	FAST_COMBOS(X)
-#undef X
-    } else {
-	e = launch_rx_t<32, 1, 1, 1, 0>(sh, ce, lc, a, st);
-    }
-    snprintf(ce->last_kernel, sizeof(ce->last_kernel),
-	    "k_rx<G=%d,W=%d,L=%d,mode=%d(%s),fill=%d,src=%s> threads=%d ring=%u smem=%zu blocks=%d lookahead=%u",
-	    sh.G, sh.W, sh.L, sh.mode, sh.mode == 3 ? "prefix-table" : sh.mode == 2 ? "shared-segment" : sh.mode == 0 ? "per-candidate" : "generic",
-	    (sh.mode == 3 && elem == 4) ? ce->pfx_fill : 0, elem == 2 ? (sh.slide ? "s16,slide" : "s16") : (sh.slide ? "f32,slide" : "f32"),
-	    sh.wpb * 32, sh.ring, sh.smem, sh.blocks, sh.lookahead);
-    if (e != cudaSuccess) {
-	fsk_b200_set_error("rx_batch launch (G=%d W=%d L=%d mode=%d ring=%u smem=%zu): %s", sh.G, sh.W,
-		sh.L, sh.mode, sh.ring, sh.smem, cudaGetErrorString(e));
-	return -EIO;
-    }
-    return 0;
-}
-
-extern "C" int fsk_b200_cuda_rx_batch(void *p, const fsk_b200_geom *g, const fsk_b200_loopc *lc,
-	const float *samples, size_t nstreams, size_t stride, const uint32_t *nsamples,
-	uint32_t nsamples_all, fsk_b200_frame *frames, uint32_t max_frames,
-	fsk_b200_stream_state *states, void *stream)
-{
-    return rx_batch_any((CudaEngine *)p, g, lc, samples, 4, nstreams, stride, nsamples, nsamples_all, frames,
-	    max_frames, states, stream);
-}
-
-extern "C" int fsk_b200_cuda_rx_batch_s16(void *p, const fsk_b200_geom *g, const fsk_b200_loopc *lc,
-	const int16_t *samples, size_t nstreams, size_t stride, const uint32_t *nsamples,
-	uint32_t nsamples_all, fsk_b200_frame *frames, uint32_t max_frames,
-	fsk_b200_stream_state *states, void *stream)
-{
-    return rx_batch_any((CudaEngine *)p, g, lc, samples, 2, nstreams, stride, nsamples, nsamples_all, frames,
-	    max_frames, states, stream);
 }
 
 /* --auto-carrier: the shapes of the per-candidate kernel with a tone table per stream (AUTO 1), in float
@@ -2338,125 +2239,110 @@ extern "C" int fsk_b200_cuda_set_unit_table(void *p, int fftsize)
     return 0;
 }
 
-/* elem 4: float32 rows, elem 2: int16 rows.  -ENOTSUP (nothing launched) where the per-candidate kernel
- * cannot take the mode or the shape has no auto build. */
-extern "C" int fsk_b200_cuda_rx_batch_auto(void *p, const fsk_b200_geom *g, const fsk_b200_loopc *lc,
-	const fsk_b200_auto_args *aa, const void *samples, int elem, size_t nstreams, size_t stride,
-	const uint32_t *nsamples, uint32_t nsamples_all, fsk_b200_frame *frames, uint32_t max_frames,
-	fsk_b200_stream_state *states, fsk_b200_auto_state *auto_states, uint32_t *rec_band, void *stream)
+/* the k_rx instance a launch shape runs for rows of SRC (0 float32, 1 int16) and tones AUTO (0 the engine's pair,
+ * 1 --auto-carrier, 2 a pair per stream); NULL where it is not built */
+typedef cudaError_t (*RxLaunch)(const Shape &, const CudaEngine *, const fsk_b200_loopc *, const RxArgs &,
+	cudaStream_t, const AutoArgs &);
+template <int SRC, int AUTO>
+static RxLaunch rx_instance(const Shape &sh, const CudaEngine *ce)
 {
+    if constexpr (AUTO != 0) {
+	if (sh.mode == 0) {
+#define X(GG, WW, LL) if (sh.G == GG && sh.W == WW && sh.L == LL) return launch_rx_t<GG, WW, LL, 0, 0, SRC, AUTO>;
+	    AUTO_COMBOS(X)
+	}
+    } else if (sh.mode == 0) {
+	if constexpr (SRC == 0) {
+	    FAST_COMBOS(X)
+	} else {
+	    S16_FAST_COMBOS(X)
+	}
+#undef X
+    } else if (sh.mode == 2) {
+#define X(GG, WW, LL) if (sh.G == GG && sh.W == WW && sh.L == LL) return launch_rx_t<GG, WW, LL, 2, 0, SRC, 0>;
+	MULTI_COMBOS(X)
+#undef X
+    } else if (sh.mode == 3) {
+	/* one stream per warp: float rows are filled by bulk copies of the TMA engine (one elected lane, two to
+	 * four copies per iteration) unless FSK_B200_PFX_FILL=0 asks for the per-lane cp.async fill */
+	if constexpr (SRC == 0) {
+	    if (ce->pfx_fill) {
+#define X(WW) if (sh.W == WW) return launch_rx_t<32, WW, 1, 3, 1, 0, 0>;
+		PFX_SLOTS(X)
+#undef X
+		return NULL;
+	    }
+	}
+#define X(WW) if (sh.W == WW) return launch_rx_t<32, WW, 1, 3, 0, SRC, 0>;
+	PFX_SLOTS(X)
+#undef X
+    } else {
+	return launch_rx_t<32, 1, 1, 1, 0, SRC, 0>;
+    }
+    return NULL;
+}
+
+/* Every batched rx call, checked by the host layer.  The streams are nrows * k channels, k per row; the launch
+ * shape is the one of nrows * k streams.  -ENOTSUP, with nothing launched or built, where the launch shape has
+ * no build for the call's kind and rows (the int16 rows of the fixed tones are then widened by the caller).
+ * The per-stream tone calls build the engine's unit-circle table on first use (synchronous). */
+extern "C" int fsk_b200_cuda_rx(void *p, const fsk_b200_geom *g, const fsk_b200_loopc *lc,
+	const fsk_b200_auto_args *aa, const fsk_b200_rx_call *c)
+{
+    static const char *const what[] = { "rx_batch", "rx_batch_auto", "rx_batch_tones" };
+    static const char *const name[] = { "k_rx", "k_rx_auto", "k_rx_tones" };
     CudaEngine *ce = (CudaEngine *)p;
-    if (!ce->d_unit || ce->unit_f != aa->fftsize) {
+    if (c->kind == FSK_B200_RX_FIXED && (!ce->d_tw || ce->tw_n < g->tw_entries)) {
+	fsk_b200_set_error("rx_batch: twiddle table not set");
+	return -EINVAL;
+    }
+    if (c->kind == FSK_B200_RX_AUTO && (!ce->d_unit || ce->unit_f != aa->fftsize)) {
 	fsk_b200_set_error("rx_batch_auto: auto-carrier not set");
 	return -EINVAL;
     }
-    if (engine_device_check(ce, "rx_batch_auto"))
+    if (engine_device_check(ce, what[c->kind]))
 	return -EINVAL;
+    const size_t nstreams = c->nrows * c->k;
     Shape sh;
     const unsigned tmax = lc->try_max_nocarrier > lc->try_max_carrier ? lc->try_max_nocarrier : lc->try_max_carrier;
-    const unsigned max_advance = tmax - 1u + lc->frame_nsamples;
-    pick_shape(ce, g, tmax - 1u + g->span, max_advance, nstreams, &sh, lc, true);
+    const unsigned max_advance = tmax - 1u + lc->frame_nsamples;	/* :1407, overscan >= 0 */
+    pick_shape(ce, g, tmax - 1u + g->span, max_advance, nstreams, &sh, lc, c->kind != FSK_B200_RX_FIXED);
     fsk_b200_loopc lc_launch = *lc;
     lc_launch.slide = sh.slide;
-    bool launched = false;
-    cudaError_t e = cudaErrorInvalidValue;
-    if (sh.mode == 0) {
-	const RxArgs a = { elem == 4 ? (const float *)samples : NULL, elem == 2 ? (const int16_t *)samples : NULL,
-	    (unsigned)nstreams, stride, nsamples, nsamples_all, frames, max_frames, states };
-	const AutoArgs au = { auto_states, rec_band, ce->d_unit, aa->threshold, aa->scan_n, aa->b_shift,
-	    (unsigned)aa->fftsize, aa->nbands, aa->half_ring, aa->expect_nsamples };
-	cudaStream_t st = (cudaStream_t)stream;
-	if (elem == 2) {
-#define X(GG, WW, LL) if (sh.G == GG && sh.W == WW && sh.L == LL) { e = launch_rx_t<GG, WW, LL, 0, 0, 1, 1>(sh, ce, &lc_launch, a, st, au); launched = true; }
-	    AUTO_COMBOS(X)
-#undef X
-	} else {
-#define X(GG, WW, LL) if (sh.G == GG && sh.W == WW && sh.L == LL) { e = launch_rx_t<GG, WW, LL, 0, 0, 0, 1>(sh, ce, &lc_launch, a, st, au); launched = true; }
-	    AUTO_COMBOS(X)
-#undef X
-	}
-    }
-    if (!launched) {
-	fsk_b200_set_error("rx_batch_auto: no auto-carrier build of the per-candidate kernel for this mode "
-		"(launch shape G=%d W=%d L=%d mode=%d)", sh.G, sh.W, sh.L, sh.mode);
+    const bool s16 = c->elem == 2;
+    const RxLaunch launch = c->kind == FSK_B200_RX_AUTO ? (s16 ? rx_instance<1, 1>(sh, ce) : rx_instance<0, 1>(sh, ce))
+	: c->kind == FSK_B200_RX_TONES ? (s16 ? rx_instance<1, 2>(sh, ce) : rx_instance<0, 2>(sh, ce))
+	: s16 ? rx_instance<1, 0>(sh, ce) : rx_instance<0, 0>(sh, ce);
+    if (!launch) {
+	if (c->kind != FSK_B200_RX_FIXED)
+	    fsk_b200_set_error("%s: no %s build of the per-candidate kernel for this mode (launch shape G=%d W=%d "
+		    "L=%d mode=%d)", what[c->kind], c->kind == FSK_B200_RX_AUTO ? "auto-carrier" : "per-stream tone",
+		    sh.G, sh.W, sh.L, sh.mode);
 	return -ENOTSUP;
     }
+    if (c->kind == FSK_B200_RX_TONES) {
+	const int rc = fsk_b200_cuda_set_unit_table(ce, aa->fftsize);
+	if (rc)
+	    return rc;
+    }
+    const RxArgs a = { s16 ? NULL : (const float *)c->samples, s16 ? (const int16_t *)c->samples : NULL,
+	(unsigned)nstreams, c->stride, c->nsamples, c->nsamples_all, c->frames, c->max_frames, c->states };
+    const AutoArgs au = { c->auto_states, c->rec_band, ce->d_unit, aa->threshold, aa->scan_n, aa->b_shift,
+	(unsigned)aa->fftsize, aa->nbands, aa->half_ring, aa->expect_nsamples, c->tone_bands, c->k };
+    const cudaError_t e = launch(sh, ce, &lc_launch, a, (cudaStream_t)c->stream, au);
+    const int fill = sh.mode == 3 && !s16 ? ce->pfx_fill : 0;
     snprintf(ce->last_kernel, sizeof(ce->last_kernel),
-	    "k_rx_auto<G=%d,W=%d,L=%d,mode=0(per-candidate),fill=0,src=%s> threads=%d ring=%u smem=%zu blocks=%d lookahead=%u",
-	    sh.G, sh.W, sh.L, elem == 2 ? (sh.slide ? "s16,slide" : "s16") : (sh.slide ? "f32,slide" : "f32"),
+	    "%s<G=%d,W=%d,L=%d,mode=%d(%s),fill=%d,src=%s%s> threads=%d ring=%u smem=%zu blocks=%d lookahead=%u",
+	    name[c->kind], sh.G, sh.W, sh.L, sh.mode, sh.mode == 3 ? "prefix-table" : sh.mode == 2 ? "shared-segment"
+	    : sh.mode == 0 ? "per-candidate" : "generic", fill, s16 ? "s16" : "f32", sh.slide ? ",slide" : "",
 	    sh.wpb * 32, sh.ring, sh.smem, sh.blocks, sh.lookahead);
-    if (e != cudaSuccess) {
-	fsk_b200_set_error("rx_batch_auto launch (G=%d W=%d L=%d ring=%u smem=%zu): %s", sh.G, sh.W, sh.L, sh.ring,
-		sh.smem, cudaGetErrorString(e));
-	return -EIO;
-    }
-    return 0;
-}
-
-/* -M / -S per stream: the AUTO_COMBOS shapes with AUTO 2, elem 4: float32 rows, elem 2: int16 rows.  The
- * streams are nrows * k channels, k per row (k = 1: a stream per row); the launch shape is the one of
- * nrows * k streams.  The engine's unit-circle table is built on first use (synchronous).  -ENOTSUP, with
- * nothing launched or built, where the per-candidate kernel cannot take the mode or the shape has no build
- * of it. */
-extern "C" int fsk_b200_cuda_rx_batch_tones(void *p, const fsk_b200_geom *g, const fsk_b200_loopc *lc, int fftsize,
-	unsigned nbands, const void *samples, int elem, size_t nrows, unsigned k, size_t stride,
-	const uint32_t *nsamples, uint32_t nsamples_all, const uint32_t *tone_bands, fsk_b200_frame *frames,
-	uint32_t max_frames, fsk_b200_stream_state *states, void *stream)
-{
-    CudaEngine *ce = (CudaEngine *)p;
-    if (engine_device_check(ce, "rx_batch_tones"))
-	return -EINVAL;
-    const size_t nstreams = nrows * k;
-    Shape sh;
-    const unsigned tmax = lc->try_max_nocarrier > lc->try_max_carrier ? lc->try_max_nocarrier : lc->try_max_carrier;
-    const unsigned max_advance = tmax - 1u + lc->frame_nsamples;
-    pick_shape(ce, g, tmax - 1u + g->span, max_advance, nstreams, &sh, lc, true);
-    fsk_b200_loopc lc_launch = *lc;
-    lc_launch.slide = sh.slide;
-    bool built = false;
-    if (sh.mode == 0) {
-#define X(GG, WW, LL) if (sh.G == GG && sh.W == WW && sh.L == LL) built = true;
-	AUTO_COMBOS(X)
-#undef X
-    }
-    if (!built) {
-	fsk_b200_set_error("rx_batch_tones: no per-stream tone build of the per-candidate kernel for this mode "
-		"(launch shape G=%d W=%d L=%d mode=%d)", sh.G, sh.W, sh.L, sh.mode);
-	return -ENOTSUP;
-    }
-    const int rc = fsk_b200_cuda_set_unit_table(ce, fftsize);
-    if (rc)
-	return rc;
-    const RxArgs a = { elem == 4 ? (const float *)samples : NULL, elem == 2 ? (const int16_t *)samples : NULL,
-	(unsigned)nstreams, stride, nsamples, nsamples_all, frames, max_frames, states };
-    AutoArgs au = AutoArgs();
-    au.unit = ce->d_unit;
-    au.fftsize = (unsigned)fftsize;
-    au.nbands = nbands;
-    au.tones = tone_bands;
-    au.k = k;
-    cudaStream_t st = (cudaStream_t)stream;
-    cudaError_t e = cudaErrorInvalidValue;
-    if (elem == 2) {
-#define X(GG, WW, LL) if (sh.G == GG && sh.W == WW && sh.L == LL) e = launch_rx_t<GG, WW, LL, 0, 0, 1, 2>(sh, ce, &lc_launch, a, st, au);
-	AUTO_COMBOS(X)
-#undef X
-    } else {
-#define X(GG, WW, LL) if (sh.G == GG && sh.W == WW && sh.L == LL) e = launch_rx_t<GG, WW, LL, 0, 0, 0, 2>(sh, ce, &lc_launch, a, st, au);
-	AUTO_COMBOS(X)
-#undef X
-    }
-    snprintf(ce->last_kernel, sizeof(ce->last_kernel),
-	    "k_rx_tones<G=%d,W=%d,L=%d,mode=0(per-candidate),fill=0,src=%s> threads=%d ring=%u smem=%zu blocks=%d lookahead=%u",
-	    sh.G, sh.W, sh.L, elem == 2 ? (sh.slide ? "s16,slide" : "s16") : (sh.slide ? "f32,slide" : "f32"),
-	    sh.wpb * 32, sh.ring, sh.smem, sh.blocks, sh.lookahead);
-    if (k > 1) {
+    if (c->k > 1) {
 	const size_t used = strlen(ce->last_kernel);
-	snprintf(ce->last_kernel + used, sizeof(ce->last_kernel) - used, " channels=%u", k);
+	snprintf(ce->last_kernel + used, sizeof(ce->last_kernel) - used, " channels=%u", c->k);
     }
     if (e != cudaSuccess) {
-	fsk_b200_set_error("rx_batch_tones launch (G=%d W=%d L=%d ring=%u smem=%zu): %s", sh.G, sh.W, sh.L, sh.ring,
-		sh.smem, cudaGetErrorString(e));
+	fsk_b200_set_error("%s launch (G=%d W=%d L=%d mode=%d ring=%u smem=%zu): %s", what[c->kind], sh.G, sh.W,
+		sh.L, sh.mode, sh.ring, sh.smem, cudaGetErrorString(e));
 	return -EIO;
     }
     return 0;
@@ -2467,10 +2353,16 @@ extern "C" int fsk_b200_cuda_rx_batch_tones(void *p, const fsk_b200_geom *g, con
  * inside the rx kernel's ring fill (rows 16-byte aligned, i.e. stride % 8 == 0, and a launch shape
  * with an int16 build; otherwise a separate widening pass runs first).
  * FSK_B200_TRACE=1 prints, per call, where the time went (CUDA events around every step). */
-static int rx_batch_host_common(CudaEngine *ce, const fsk_b200_geom *g, const fsk_b200_loopc *lc,
-	const void *host_samples, int elem, size_t nstreams, size_t stride, uint32_t nsamples_all,
-	fsk_b200_frame *host_frames, uint32_t max_frames, fsk_b200_stream_state *host_states)
+extern "C" int fsk_b200_cuda_rx_host(void *p, const fsk_b200_geom *g, const fsk_b200_loopc *lc,
+	const fsk_b200_auto_args *aa, const fsk_b200_rx_call *c)
 {
+    CudaEngine *ce = (CudaEngine *)p;
+    const void *host_samples = c->samples;
+    const int elem = c->elem;
+    const size_t nstreams = c->nrows, stride = c->stride;
+    fsk_b200_frame *host_frames = c->frames;
+    const uint32_t max_frames = c->max_frames;
+    fsk_b200_stream_state *host_states = c->states;
     if (engine_device_check(ce, "rx_batch_host"))
 	return -EINVAL;
     /* slab = as many streams as make slab_bytes on the wire (two slabs in flight) */
@@ -2525,28 +2417,29 @@ static int rx_batch_host_common(CudaEngine *ce, const fsk_b200_geom *g, const fs
 	    HOST_TRY(cudaMemcpyAsync(ce->d_slab_states[k], host_states + s0, ns * sizeof(fsk_b200_stream_state),
 			cudaMemcpyHostToDevice, st));
 	    if (ev) cudaEventRecord(ev[4 * si + 1], st);
-	    if (elem == 4) {
-		rc = rx_batch_any(ce, g, lc, ce->d_slab_in[k], 4, ns, stride, NULL, nsamples_all,
-			ce->d_slab_frames[k], max_frames, ce->d_slab_states[k], st);
-	    } else {
-		rc = fused ? rx_batch_any(ce, g, lc, ce->d_slab_in[k], 2, ns, stride, NULL, nsamples_all,
-			ce->d_slab_frames[k], max_frames, ce->d_slab_states[k], st) : -ENOTSUP;
-		if (rc == -ENOTSUP) {		/* no int16 build for this mode's launch shape: widen first */
-		    fused = false;
-		    if (ce->slab_f32_floats < slab * stride) {
-			for (int i = 0; i < 2; i++) {
-			    cudaFree(ce->d_slab[i]); ce->d_slab[i] = NULL;
-			}
-			ce->slab_f32_floats = 0;
-			for (int i = 0; i < 2; i++)
-			    HOST_TRY(cudaMalloc(&ce->d_slab[i], slab * stride * sizeof(float)));
-			ce->slab_f32_floats = slab * stride;
+	    fsk_b200_rx_call sc = *c;		/* the slab, on the device */
+	    sc.samples = ce->d_slab_in[k];
+	    sc.nrows = ns;
+	    sc.frames = ce->d_slab_frames[k];
+	    sc.states = ce->d_slab_states[k];
+	    sc.stream = st;
+	    rc = elem == 4 || fused ? fsk_b200_cuda_rx(ce, g, lc, aa, &sc) : -ENOTSUP;
+	    if (rc == -ENOTSUP && elem == 2) {	/* no int16 build for this mode's launch shape: widen first */
+		fused = false;
+		if (ce->slab_f32_floats < slab * stride) {
+		    for (int i = 0; i < 2; i++) {
+			cudaFree(ce->d_slab[i]); ce->d_slab[i] = NULL;
 		    }
-		    rc = fsk_b200_cuda_s16_to_f32((const int16_t *)ce->d_slab_in[k], ce->d_slab[k], ns, stride, st);
-		    if (!rc)
-			rc = rx_batch_any(ce, g, lc, ce->d_slab[k], 4, ns, stride, NULL, nsamples_all,
-				ce->d_slab_frames[k], max_frames, ce->d_slab_states[k], st);
+		    ce->slab_f32_floats = 0;
+		    for (int i = 0; i < 2; i++)
+			HOST_TRY(cudaMalloc(&ce->d_slab[i], slab * stride * sizeof(float)));
+		    ce->slab_f32_floats = slab * stride;
 		}
+		rc = fsk_b200_cuda_s16_to_f32((const int16_t *)ce->d_slab_in[k], ce->d_slab[k], ns, stride, st);
+		sc.samples = ce->d_slab[k];
+		sc.elem = 4;
+		if (!rc)
+		    rc = fsk_b200_cuda_rx(ce, g, lc, aa, &sc);
 	    }
 	    if (rc)
 		goto fail;
@@ -2592,22 +2485,6 @@ fail:
     (void)cudaGetLastError();
     return rc;
 #undef HOST_TRY
-}
-
-extern "C" int fsk_b200_cuda_rx_batch_host(void *p, const fsk_b200_geom *g, const fsk_b200_loopc *lc,
-	const float *host_samples, size_t nstreams, size_t stride, uint32_t nsamples_all,
-	fsk_b200_frame *host_frames, uint32_t max_frames, fsk_b200_stream_state *host_states)
-{
-    return rx_batch_host_common((CudaEngine *)p, g, lc, host_samples, 4, nstreams, stride, nsamples_all,
-	    host_frames, max_frames, host_states);
-}
-
-extern "C" int fsk_b200_cuda_rx_batch_host_s16(void *p, const fsk_b200_geom *g, const fsk_b200_loopc *lc,
-	const int16_t *host_samples, size_t nstreams, size_t stride, uint32_t nsamples_all,
-	fsk_b200_frame *host_frames, uint32_t max_frames, fsk_b200_stream_state *host_states)
-{
-    return rx_batch_host_common((CudaEngine *)p, g, lc, host_samples, 2, nstreams, stride, nsamples_all,
-	    host_frames, max_frames, host_states);
 }
 
 extern "C" int fsk_b200_cuda_s16_to_f32(const int16_t *src, float *dst, size_t nstreams, size_t stride,

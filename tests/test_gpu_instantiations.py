@@ -1,7 +1,7 @@
 """Every rx, find-frame and transmitter kernel instantiation the launchers can dispatch, on random
 framings, against the oracle.
 
-The rest of the `gpu` suite drives the kernels through a few fixed geometries; `rx_batch_any` and
+The rest of the `gpu` suite drives the kernels through a few fixed geometries; `fsk_b200_cuda_rx` and
 `fsk_b200_find_frame_batch` (minimodem_b200/csrc/fsk_b200_kernels.cu) can launch some 140 distinct
 template instances, and `tx_launch` eight.  The tables below map each launchable instance to a framing
 and an environment that reach it, each test asserts that `last_kernel()` names the instance its row
@@ -165,7 +165,7 @@ def launchable():
 
 
 def test_the_tables_cover_every_instantiation():
-    """CPU: the tables = what rx_batch_any / the find-frame launcher / tx_launch can dispatch, minus
+    """CPU: the tables = what fsk_b200_cuda_rx / the find-frame launcher / tx_launch can dispatch, minus
     UNREACHABLE (each with its reason)."""
     rx, ff, tx = launchable()
     assert set(UNREACHABLE) <= rx

@@ -1,11 +1,12 @@
 """CPU-only checks of the product's host layer (no compute calls): the C-ABI
-library loads and exports every symbol include/fsk_b200.h declares; the mode
+library loads and exports exactly the functions include/fsk_b200.h declares; the mode
 presets and frame geometry it derives equal the oracle's restatement of
 src/minimodem.c:819-1131 for every mode the reference tests use; without a CUDA
 device the engine refuses to start (no CPU fallback)."""
 import ctypes as C
 import os
 import re
+import subprocess
 
 import numpy as np
 import pytest
@@ -32,6 +33,11 @@ def test_library_exports_every_declared_symbol():
     for name in sorted(declared):
         assert hasattr(L, name), name
     assert declared == set(mm.EXPORTS)
+    # and nothing else: the library's internal interface stays out of its dynamic symbol table
+    nm = subprocess.run(["nm", "-D", "--defined-only", mm.LIB_PATH], stdout=subprocess.PIPE, check=True)
+    exported = {f[2] for f in (line.split() for line in nm.stdout.decode().splitlines())
+                if len(f) == 3 and f[1] in "TtWi" and f[2].startswith("fsk_")}
+    assert exported == declared, (exported - declared, declared - exported)
     assert "sm_90a" in mm.version()
 
 
