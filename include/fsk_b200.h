@@ -305,6 +305,10 @@ int fsk_b200_rx_batch_host(fsk_b200_engine *e, const float *host_samples, size_t
  * With the holdback at fsk_b200_stream_window() a search starts only when every sample it can touch
  * has arrived, so the records do not depend on how the stream was cut into chunks.
  *
+ * 16-bit PCM: fsk_b200_stream_push_s16 keeps int16 rows, fed int16 chunks, for the _s16 rx calls, at half the
+ * bytes of float rows; where fsk_b200_rx_batch_s16_runs says the plain call has no int16 build, keep float rows
+ * and widen each chunk (fsk_b200_s16_to_f32) before fsk_b200_stream_push.
+ *
  * fsk_b200_stream_push: per stream s, the unconsumed tail [states[s].pos, fill[s]) of row s moves to
  * the front, chunk_len[s] (or chunk_len_all when chunk_len is NULL) floats of chunk row s are
  * appended (what does not fit in min(stride, FSK_B200_MAX_ROW_SAMPLES) is dropped and counted in
@@ -450,6 +454,15 @@ int fsk_b200_stream_push_events(float *samples, size_t nrows, size_t stride, uin
 	uint32_t channels_per_row, const uint32_t *tone_bands, uint32_t nbands, fsk_b200_stream_state *states,
 	const float *chunk, size_t chunk_stride, const uint32_t *chunk_len, uint32_t chunk_len_all, uint32_t *dropped,
 	const uint8_t *row_events, void *stream);
+/* fsk_b200_stream_push_s16: fsk_b200_stream_push_events on int16 rows with an int16 chunk, the samples copied
+ * bit for bit (no widening): the same rule, fill, states and dropped, with row_events NULL exactly
+ * fsk_b200_stream_push_channels (and, k = 1 with tone_bands NULL, fsk_b200_stream_push).  The same validation
+ * and refusals, with the row layout of the _s16 rx calls: samples 16-byte aligned and stride a multiple of 8
+ * samples (-EINVAL otherwise), so rows the push accepts are rows those calls accept. */
+int fsk_b200_stream_push_s16(int16_t *samples, size_t nrows, size_t stride, uint32_t *fill,
+	uint32_t channels_per_row, const uint32_t *tone_bands, uint32_t nbands, fsk_b200_stream_state *states,
+	const int16_t *chunk, size_t chunk_stride, const uint32_t *chunk_len, uint32_t chunk_len_all, uint32_t *dropped,
+	const uint8_t *row_events, void *stream);
 
 /* N2 -- 16-bit PCM ingest (the reference transmitter's default sample format, read back by
  * its rx as float = short / 32768: src/simpleaudio-sndfile.c:43-57, src/minimodem.c:786-788).
@@ -469,6 +482,11 @@ int fsk_b200_rx_batch_s16(fsk_b200_engine *e, const int16_t *samples, size_t nst
 	size_t stride, const uint32_t *nsamples, uint32_t nsamples_all,
 	fsk_b200_frame *frames, uint32_t max_frames,
 	fsk_b200_stream_state *states, void *stream);
+/* Whether fsk_b200_rx_batch_s16 on nstreams (> 0) valid rows launches at the engine's current tuning (1) or
+ * returns -ENOTSUP (0): the launch shape and the int16 build lookup of that call, on the host, with nothing
+ * launched and no synchronisation.  -EINVAL for a NULL engine.  The auto-carrier and tone calls have their int16
+ * builds wherever they have float ones, so only this call needs asking. */
+int fsk_b200_rx_batch_s16_runs(const fsk_b200_engine *e, size_t nstreams);
 
 /* N2, the file side: where the samples of a RIFF/WAVE image are (the container the reference's
  * tests and its default `--file` output use; the reference itself goes through libsndfile,

@@ -130,7 +130,7 @@ EXPORTS = [
     "fsk_b200_rx_batch_auto_s16", "fsk_b200_auto_stream_window",
     "fsk_b200_tone_bands", "fsk_b200_rx_batch_tones", "fsk_b200_rx_batch_tones_s16",
     "fsk_b200_rx_batch_channels", "fsk_b200_rx_batch_channels_s16", "fsk_b200_stream_push_channels",
-    "fsk_b200_stream_push_events",
+    "fsk_b200_stream_push_events", "fsk_b200_stream_push_s16", "fsk_b200_rx_batch_s16_runs",
 ]
 
 _lib = None
@@ -292,6 +292,10 @@ def lib():
     L.fsk_b200_stream_push_channels.restype = C.c_int
     L.fsk_b200_stream_push_events.argtypes = L.fsk_b200_stream_push_channels.argtypes[:-1] + [C.c_void_p, C.c_void_p]
     L.fsk_b200_stream_push_events.restype = C.c_int
+    L.fsk_b200_stream_push_s16.argtypes = list(L.fsk_b200_stream_push_events.argtypes)
+    L.fsk_b200_stream_push_s16.restype = C.c_int
+    L.fsk_b200_rx_batch_s16_runs.argtypes = [C.c_void_p, C.c_size_t]
+    L.fsk_b200_rx_batch_s16_runs.restype = C.c_int
     L.fsk_b200_version.restype = C.c_char_p
     L.fsk_b200_launch_count.restype = C.c_ulonglong
     L.fsk_b200_last_error.restype = C.c_char_p
@@ -518,6 +522,15 @@ class RxEngine:
         return self._rx("rx_batch", samples, samples.shape[0], nsamples, max_frames, frames, states, nsamples_each,
                         stream)[:2]
 
+    def rx_batch_s16_runs(self, nstreams):
+        """fsk_b200_rx_batch_s16_runs: whether rx_batch on int16 rows of nstreams streams launches at the
+        engine's current tuning (True), or has no int16 build for its launch shape (False: widen the rows).
+        Host only."""
+        rc = lib().fsk_b200_rx_batch_s16_runs(self._e, int(nstreams))
+        if rc < 0:
+            _err("fsk_b200_rx_batch_s16_runs", rc)
+        return bool(rc)
+
     def rx_batch_host(self, samples, nsamples=None, max_frames=None, frames_out=None, states_out=None):
         """Host arrays in, host records out (copies overlap demodulation inside the library).
         samples: [nstreams, stride] float32 numpy array or (pinned) CPU torch tensor;
@@ -738,6 +751,8 @@ def stream_push(rows, fill, states, chunk, chunk_len=None, dropped=None, stream=
                 tone_bands=None, nbands=0, row_events=None):
     """fsk_b200_stream_push on CUDA tensors: rows [n, stride] float32, fill [n] int32 (in/out), states
     [n, STATE_WORDS] int32 (in/out), chunk [n, chunk_stride] float32, chunk_len [n] int32 or an int.
+    int16 rows with an int16 chunk go to fsk_b200_stream_push_s16 (the same rule, the samples copied as they
+    are; stride a multiple of 8), whatever the other arguments; rows and chunk of different types are refused.
     channels_per_row=k or tone_bands given (fsk_b200_stream_push_channels): states are per channel,
     [n*k, STATE_WORDS]; tone_bands (int32 [n*k, 2] or None) marks which channels are active (both bands
     < nbands), and only those keep a row's tail.
@@ -749,7 +764,10 @@ def stream_push(rows, fill, states, chunk, chunk_len=None, dropped=None, stream=
     chunk: its length goes to dropped."""
     torch = _torch()
     # the C call takes raw pointers and row strides: the tensors must be what it assumes
-    assert rows.is_contiguous() and rows.dtype == torch.float32 and chunk.is_contiguous() and chunk.dtype == torch.float32
+    assert rows.is_contiguous() and chunk.is_contiguous()
+    if rows.dtype not in (torch.float32, torch.int16) or chunk.dtype != rows.dtype:
+        raise TypeError("stream_push: rows and chunk must both be float32 or both int16 (got %s and %s)"
+                        % (rows.dtype, chunk.dtype))
     assert fill.is_contiguous() and fill.dtype == torch.int32 and states.is_contiguous() and states.dtype == torch.int32
     k = int(channels_per_row)
     assert chunk.shape[0] == rows.shape[0] and states.shape == (rows.shape[0] * k, STATE_WORDS)
@@ -757,16 +775,18 @@ def stream_push(rows, fill, states, chunk, chunk_len=None, dropped=None, stream=
     per = chunk_len if hasattr(chunk_len, "data_ptr") else None
     assert per is None or (per.dtype == torch.int32 and per.is_contiguous())
     common = 0 if per is not None else int(chunk.shape[1] if chunk_len is None else chunk_len)
-    if row_events is not None:
-        assert (row_events.dtype == torch.uint8 and row_events.is_contiguous()
-                and tuple(row_events.shape) == (n,))
+    s16 = rows.dtype == torch.int16
+    if row_events is not None or s16:
+        assert row_events is None or (row_events.dtype == torch.uint8 and row_events.is_contiguous()
+                                      and tuple(row_events.shape) == (n,))
         assert tone_bands is None or (tone_bands.dtype == torch.int32 and tone_bands.is_contiguous()
                                       and tuple(tone_bands.shape) == (n * k, 2))
-        rc = lib().fsk_b200_stream_push_events(_ptr(rows), n, stride, _ptr(fill), k, _ptr(tone_bands), int(nbands),
-                                               _ptr(states), _ptr(chunk), chunk.shape[1], _ptr(per), common,
-                                               _ptr(dropped), _ptr(row_events), _stream_handle(stream))
+        name = "fsk_b200_stream_push_s16" if s16 else "fsk_b200_stream_push_events"
+        rc = getattr(lib(), name)(_ptr(rows), n, stride, _ptr(fill), k, _ptr(tone_bands), int(nbands),
+                                  _ptr(states), _ptr(chunk), chunk.shape[1], _ptr(per), common,
+                                  _ptr(dropped), _ptr(row_events), _stream_handle(stream))
         if rc:
-            _err("fsk_b200_stream_push_events", rc)
+            _err(name, rc)
         return
     if k == 1 and tone_bands is None:
         rc = lib().fsk_b200_stream_push(_ptr(rows), n, stride, _ptr(fill), _ptr(states), _ptr(chunk),

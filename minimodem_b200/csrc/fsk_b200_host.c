@@ -600,10 +600,14 @@ int fsk_b200_engine_tune(fsk_b200_engine *e, int lanes_per_stream, int warps_per
     return fsk_b200_cuda_tune(e->ce, lanes_per_stream, warps_per_block, ring_floats);
 }
 
-static int check_layout(const float *samples, size_t stride)
+/* device rows of elem bytes per sample (4 float32, 2 int16): 16-byte aligned, and so is every row start
+ * (for int16 rows the layout the _s16 rx calls take) */
+static int check_layout(const void *samples, size_t stride, int elem)
 {
-    if (!samples || ((uintptr_t)samples & 15) || (stride & 3)) {
-	fsk_b200_set_error("samples must be 16-byte aligned and stride a multiple of 4 floats");
+    const size_t align = elem == 2 ? 8 : 4;
+    if (!samples || ((uintptr_t)samples & 15) || (stride & (align - 1))) {
+	fsk_b200_set_error("samples must be 16-byte aligned and stride a multiple of %zu %s", align,
+		elem == 2 ? "int16 samples" : "floats");
 	return -EINVAL;
     }
     return 0;
@@ -616,7 +620,7 @@ int fsk_b200_find_frame_batch(fsk_b200_engine *e, const float *samples, size_t n
 {
     if (nstreams == 0)
 	return 0;
-    int rc = check_layout(samples, stride);
+    int rc = check_layout(samples, stride, 4);
     if (rc)
 	return rc;
     if (!nvalid || !try_first || !try_max || !try_step || !limit || !frames) {
@@ -634,7 +638,7 @@ int fsk_b200_find_frame_batch_bits(fsk_b200_engine *e, const float *samples, siz
 {
     if (nstreams == 0)
 	return 0;
-    int rc = check_layout(samples, stride);
+    int rc = check_layout(samples, stride, 4);
     if (rc)
 	return rc;
     if (!nvalid || !try_first || !try_max || !try_step || !limit || !frames || !bit_mags
@@ -707,6 +711,15 @@ int fsk_b200_rx_batch(fsk_b200_engine *e, const float *samples, size_t nstreams,
     return rx_call(e, "rx_batch", 0, &(fsk_b200_rx_call){ .kind = FSK_B200_RX_FIXED, .elem = 4, .samples = samples,
 	    .nrows = nstreams, .k = 1, .stride = stride, .nsamples = nsamples, .nsamples_all = nsamples_all,
 	    .frames = frames, .max_frames = max_frames, .states = states, .stream = stream });
+}
+
+int fsk_b200_rx_batch_s16_runs(const fsk_b200_engine *e, size_t nstreams)
+{
+    if (!e) {
+	fsk_b200_set_error("rx_batch_s16_runs: NULL engine");
+	return -EINVAL;
+    }
+    return fsk_b200_cuda_rx_s16_runs(e->ce, &e->geom, &e->loopc, nstreams);
 }
 
 int fsk_b200_rx_batch_s16(fsk_b200_engine *e, const int16_t *samples, size_t nstreams, size_t stride,
@@ -908,9 +921,10 @@ int fsk_b200_engine_set_holdback(fsk_b200_engine *e, uint32_t nsamples)
     return 0;
 }
 
-int fsk_b200_stream_push_events(float *samples, size_t nrows, size_t stride, uint32_t *fill,
+/* Every live push: rows and chunk of elem bytes per sample (4 float32, 2 int16) */
+static int stream_push(int elem, void *samples, size_t nrows, size_t stride, uint32_t *fill,
 	uint32_t channels_per_row, const uint32_t *tone_bands, uint32_t nbands, fsk_b200_stream_state *states,
-	const float *chunk, size_t chunk_stride, const uint32_t *chunk_len, uint32_t chunk_len_all, uint32_t *dropped,
+	const void *chunk, size_t chunk_stride, const uint32_t *chunk_len, uint32_t chunk_len_all, uint32_t *dropped,
 	const uint8_t *row_events, void *stream)
 {
     if (channels_per_row == 0 || nrows > 0x7fffffffu / channels_per_row) {
@@ -920,7 +934,7 @@ int fsk_b200_stream_push_events(float *samples, size_t nrows, size_t stride, uin
     }
     if (nrows == 0)
 	return 0;
-    int rc = check_layout(samples, stride);
+    int rc = check_layout(samples, stride, elem);
     if (rc)
 	return rc;
     if (!fill || !states || (!chunk && (chunk_len || chunk_len_all))) {
@@ -931,8 +945,26 @@ int fsk_b200_stream_push_events(float *samples, size_t nrows, size_t stride, uin
 	fsk_b200_set_error("no usable CUDA device (there is no CPU fallback)");
 	return -ENODEV;
     }
-    return fsk_b200_cuda_stream_push(samples, nrows, stride, fill, channels_per_row, tone_bands, nbands, states,
-	    chunk, chunk_stride, chunk_len, chunk_len_all, dropped, row_events, stream);
+    return fsk_b200_cuda_stream_push(elem, samples, nrows, stride, fill, channels_per_row, tone_bands, nbands,
+	    states, chunk, chunk_stride, chunk_len, chunk_len_all, dropped, row_events, stream);
+}
+
+int fsk_b200_stream_push_events(float *samples, size_t nrows, size_t stride, uint32_t *fill,
+	uint32_t channels_per_row, const uint32_t *tone_bands, uint32_t nbands, fsk_b200_stream_state *states,
+	const float *chunk, size_t chunk_stride, const uint32_t *chunk_len, uint32_t chunk_len_all, uint32_t *dropped,
+	const uint8_t *row_events, void *stream)
+{
+    return stream_push(4, samples, nrows, stride, fill, channels_per_row, tone_bands, nbands, states, chunk,
+	    chunk_stride, chunk_len, chunk_len_all, dropped, row_events, stream);
+}
+
+int fsk_b200_stream_push_s16(int16_t *samples, size_t nrows, size_t stride, uint32_t *fill,
+	uint32_t channels_per_row, const uint32_t *tone_bands, uint32_t nbands, fsk_b200_stream_state *states,
+	const int16_t *chunk, size_t chunk_stride, const uint32_t *chunk_len, uint32_t chunk_len_all, uint32_t *dropped,
+	const uint8_t *row_events, void *stream)
+{
+    return stream_push(2, samples, nrows, stride, fill, channels_per_row, tone_bands, nbands, states, chunk,
+	    chunk_stride, chunk_len, chunk_len_all, dropped, row_events, stream);
 }
 
 int fsk_b200_stream_push_channels(float *samples, size_t nrows, size_t stride, uint32_t *fill,

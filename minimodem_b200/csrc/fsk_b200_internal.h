@@ -213,9 +213,13 @@ int  fsk_b200_cuda_rx(void *ce, const fsk_b200_geom *g, const fsk_b200_loopc *lc
 /* the same over host buffers (fixed tones, nsamples NULL): slabs of rows through fsk_b200_cuda_rx */
 int  fsk_b200_cuda_rx_host(void *ce, const fsk_b200_geom *g, const fsk_b200_loopc *lc, const fsk_b200_auto_args *aa,
 	const fsk_b200_rx_call *c);
-/* live rows: k channels (states) per row, tone_bands (device, optional) [nrows * k][2] */
-int  fsk_b200_cuda_stream_push(float *samples, size_t nrows, size_t stride, uint32_t *fill, unsigned int k,
-	const uint32_t *tone_bands, unsigned int nbands, fsk_b200_stream_state *states, const float *chunk,
+/* 1 if fsk_b200_cuda_rx launches a FIXED call on int16 rows of nstreams streams, 0 if it returns -ENOTSUP
+ * (host only: the launch shape and the instance lookup of that call, nothing launched) */
+int  fsk_b200_cuda_rx_s16_runs(void *ce, const fsk_b200_geom *g, const fsk_b200_loopc *lc, size_t nstreams);
+/* live rows of elem bytes per sample (4 float32, 2 int16; the chunk alike): k channels (states) per row,
+ * tone_bands (device, optional) [nrows * k][2] */
+int  fsk_b200_cuda_stream_push(int elem, void *samples, size_t nrows, size_t stride, uint32_t *fill, unsigned int k,
+	const uint32_t *tone_bands, unsigned int nbands, fsk_b200_stream_state *states, const void *chunk,
 	size_t chunk_stride, const uint32_t *chunk_len, uint32_t chunk_len_all, uint32_t *dropped,
 	const uint8_t *row_events, void *stream);
 /* the synthesis kernel; lut: device table of plan->lut_len float or int16 entries */

@@ -1445,17 +1445,18 @@ __global__ void k_s16_to_f32_scalar(const short *__restrict__ src, float *__rest
  * FSK_B200_STREAM_ENDED after it; the flag survives the pushes that follow (done &= ENDED).  A row whose
  * channels are all flagged takes no chunk unless it is opened: the chunk is counted in dropped[r] and the
  * row, its fill and its states are left as they are. */
-__global__ void k_stream_push(float *__restrict__ samples, unsigned nrows, size_t stride,
+template <typename T>		/* float or int16_t rows; the chunk is of the same type and copied bit for bit */
+__global__ void k_stream_push(T *__restrict__ samples, unsigned nrows, size_t stride,
 	uint32_t *__restrict__ fill, unsigned k, const uint32_t *__restrict__ bands, unsigned nbands,
 	fsk_b200_stream_state *__restrict__ states,
-	const float *__restrict__ chunk, size_t chunk_stride, const uint32_t *__restrict__ chunk_len,
+	const T *__restrict__ chunk, size_t chunk_stride, const uint32_t *__restrict__ chunk_len,
 	uint32_t chunk_len_all, uint32_t *__restrict__ dropped, const uint8_t *__restrict__ events)
 {
     const unsigned lane = threadIdx.x & 31;
     const unsigned r = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     if (r >= nrows)
 	return;						/* whole warps leave together */
-    float *row = samples + (size_t)r * stride;
+    T *row = samples + (size_t)r * stride;
     const unsigned ev = events ? events[r] : 0u;
     const bool open = (ev & FSK_B200_ROW_OPEN) != 0u, end = (ev & FSK_B200_ROW_END) != 0u;
     fsk_b200_stream_state *const st = states + (size_t)r * k;
@@ -1487,7 +1488,7 @@ __global__ void k_stream_push(float *__restrict__ samples, unsigned nrows, size_
     /* (64-bit counters: a 32-bit one stepping by 32 never passes a length above 2^32 - 32) */
     if (m)
 	for (size_t t = 0; t < tail; t += 32) {
-	    const float v = t + lane < tail ? row[m + t + lane] : 0.f;
+	    const T v = t + lane < tail ? row[m + t + lane] : T(0);
 	    __syncwarp();
 	    if (t + lane < tail)
 		row[t + lane] = v;
@@ -1499,7 +1500,7 @@ __global__ void k_stream_push(float *__restrict__ samples, unsigned nrows, size_
     const unsigned room = tail < cap ? cap - tail : 0u;
     const unsigned drop = len > room ? len - room : 0u;
     len -= drop;
-    const float *src = chunk + (size_t)r * chunk_stride;
+    const T *src = chunk + (size_t)r * chunk_stride;
     for (size_t i = lane; i < len; i += 32)
 	row[tail + i] = src[i];
     __syncwarp();		/* every lane has read fill[r] and the states before any lane rewrites them */
@@ -2282,6 +2283,23 @@ static RxLaunch rx_instance(const Shape &sh, const CudaEngine *ce)
     return NULL;
 }
 
+/* the launch shape of an rx call over nstreams streams */
+static void rx_shape(const CudaEngine *ce, const fsk_b200_geom *g, const fsk_b200_loopc *lc, size_t nstreams,
+	bool per_stream_tw, Shape *sh)
+{
+    const unsigned tmax = lc->try_max_nocarrier > lc->try_max_carrier ? lc->try_max_nocarrier : lc->try_max_carrier;
+    const unsigned max_advance = tmax - 1u + lc->frame_nsamples;	/* :1407, overscan >= 0 */
+    pick_shape(ce, g, tmax - 1u + g->span, max_advance, nstreams, sh, lc, per_stream_tw);
+}
+
+extern "C" int fsk_b200_cuda_rx_s16_runs(void *p, const fsk_b200_geom *g, const fsk_b200_loopc *lc, size_t nstreams)
+{
+    const CudaEngine *ce = (const CudaEngine *)p;
+    Shape sh;
+    rx_shape(ce, g, lc, nstreams, false, &sh);
+    return rx_instance<1, 0>(sh, ce) != NULL;
+}
+
 /* Every batched rx call, checked by the host layer.  The streams are nrows * k channels, k per row; the launch
  * shape is the one of nrows * k streams.  -ENOTSUP, with nothing launched or built, where the launch shape has
  * no build for the call's kind and rows (the int16 rows of the fixed tones are then widened by the caller).
@@ -2304,9 +2322,7 @@ extern "C" int fsk_b200_cuda_rx(void *p, const fsk_b200_geom *g, const fsk_b200_
 	return -EINVAL;
     const size_t nstreams = c->nrows * c->k;
     Shape sh;
-    const unsigned tmax = lc->try_max_nocarrier > lc->try_max_carrier ? lc->try_max_nocarrier : lc->try_max_carrier;
-    const unsigned max_advance = tmax - 1u + lc->frame_nsamples;	/* :1407, overscan >= 0 */
-    pick_shape(ce, g, tmax - 1u + g->span, max_advance, nstreams, &sh, lc, c->kind != FSK_B200_RX_FIXED);
+    rx_shape(ce, g, lc, nstreams, c->kind != FSK_B200_RX_FIXED, &sh);
     fsk_b200_loopc lc_launch = *lc;
     lc_launch.slide = sh.slide;
     const bool s16 = c->elem == 2;
@@ -2510,9 +2526,9 @@ extern "C" int fsk_b200_cuda_s16_to_f32(const int16_t *src, float *dst, size_t n
 }
 
 /* one warp per row; k channels (states) per row, tone_bands optional ([nrows * k][2]), row_events optional
- * ([nrows]) */
-extern "C" int fsk_b200_cuda_stream_push(float *samples, size_t nrows, size_t stride, uint32_t *fill,
-	unsigned k, const uint32_t *tone_bands, unsigned nbands, fsk_b200_stream_state *states, const float *chunk,
+ * ([nrows]); elem: bytes per sample of the rows and the chunk, 4 float32, 2 int16 */
+extern "C" int fsk_b200_cuda_stream_push(int elem, void *samples, size_t nrows, size_t stride, uint32_t *fill,
+	unsigned k, const uint32_t *tone_bands, unsigned nbands, fsk_b200_stream_state *states, const void *chunk,
 	size_t chunk_stride, const uint32_t *chunk_len, uint32_t chunk_len_all, uint32_t *dropped,
 	const uint8_t *row_events, void *stream)
 {
@@ -2520,9 +2536,14 @@ extern "C" int fsk_b200_cuda_stream_push(float *samples, size_t nrows, size_t st
 	return 0;
     const unsigned threads = 128;
     const size_t blocks = (nrows * 32 + threads - 1) / threads;
-    FSK_LAUNCH(k_stream_push, (unsigned)blocks, threads, 0, (cudaStream_t)stream, samples, (unsigned)nrows,
-	    stride, fill, k, tone_bands, nbands, states, chunk, chunk_stride, chunk_len, chunk_len_all, dropped,
-	    row_events);
+    if (elem == 2)
+	FSK_LAUNCH(k_stream_push<int16_t>, (unsigned)blocks, threads, 0, (cudaStream_t)stream, (int16_t *)samples,
+		(unsigned)nrows, stride, fill, k, tone_bands, nbands, states, (const int16_t *)chunk, chunk_stride,
+		chunk_len, chunk_len_all, dropped, row_events);
+    else
+	FSK_LAUNCH(k_stream_push<float>, (unsigned)blocks, threads, 0, (cudaStream_t)stream, (float *)samples,
+		(unsigned)nrows, stride, fill, k, tone_bands, nbands, states, (const float *)chunk, chunk_stride,
+		chunk_len, chunk_len_all, dropped, row_events);
     g_launches++;
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) {

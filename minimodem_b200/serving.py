@@ -21,6 +21,12 @@ each fed row carries k channels (both directions of a duplex line, k signals of 
 (fsk_b200_stream_push_channels, where a disabled channel does not hold the row back), one
 fsk_b200_rx_batch_channels, and text and decoder state per channel, [nstreams*k, ...].
 
+With pcm16=True the receiver takes int16 CUDA chunks (16-bit PCM, LiveTransmitter's default output) in every form above:
+the rows stay int16 (stride a multiple of 8), the push is fsk_b200_stream_push_s16 and the rx call its _s16 form, widened
+(x / 32768, exact) inside the kernel's ring fill; the text is the float receiver's on the widened chunks.  Where
+fsk_b200_rx_batch_s16_runs says the plain int16 call has no build for the mode, the rows are float32 and every chunk is
+widened into a preallocated buffer before the float push; rx.rows.dtype shows which.
+
 Streams with lifetimes of their own (calls on a modem bank, a Caller-ID front end):
 
     text, counts = rx.feed(chunk, lengths, opened=opened, ended=ended)   # bool CUDA tensors [nstreams]
@@ -49,7 +55,7 @@ from . import api
 
 class LiveReceiver:
     def __init__(self, baudmode, sample_rate=48000, nstreams=1, max_chunk=4800, device=None,
-                 binary_output=False, auto_carrier=None, tones=None, channels_per_row=1, **overrides):
+                 binary_output=False, auto_carrier=None, tones=None, channels_per_row=1, pcm16=False, **overrides):
         torch = api._torch()
         if auto_carrier is not None and tones is not None:
             raise ValueError("LiveReceiver: auto_carrier and tones exclude each other")
@@ -66,18 +72,30 @@ class LiveReceiver:
         self.nstreams, self.max_chunk = int(nstreams), int(max_chunk)
         # a row holds the longest tail the loop can leave behind plus one chunk
         tail_max = self.window + self.engine.params.frame_nsamples
-        self.stride = (tail_max + self.max_chunk + 3) & ~3
+        self.pcm16 = bool(pcm16)
+        align = 8 if self.pcm16 else 4         # int16 rows: the row layout of the _s16 calls
+        self.stride = (tail_max + self.max_chunk + align - 1) & ~(align - 1)
         self.max_frames = self.engine.max_frames(self.stride)
         self.row_bytes = api.decode_max_bytes(self.kind, self.engine.params.n_data_bits, self.max_frames)
         dev = device if device is not None else torch.device("cuda:0")
         z = lambda shape, dt: torch.zeros(shape, dtype=dt, device=dev)
         nchannels = self.nstreams * self.k
-        self.rows = z((self.nstreams, self.stride), torch.float32)
+        # pcm16: int16 rows wherever the rx call has an int16 build (the tone and auto-carrier calls always do);
+        # elsewhere float32 rows, and every chunk is widened exactly (x / 32768) before the push
+        s16_rows = self.pcm16 and (tones is not None or self.auto or self.engine.rx_batch_s16_runs(self.nstreams))
+        row_type = torch.int16 if s16_rows else torch.float32
+        self.rows = z((self.nstreams, self.stride), row_type)
         self.fill = z((self.nstreams,), torch.int32)
         self.states = z((nchannels, api.STATE_WORDS), torch.int32)
         self.dstates = z((nchannels, api.DECODER_STATE_BYTES), torch.uint8)
         self.dropped = z((self.nstreams,), torch.int32)
-        self._empty = z((self.nstreams, 4), torch.float32)
+        self._empty = z((self.nstreams, align), row_type)
+        self._wide = self._stage = None
+        if self.pcm16 and not s16_rows:
+            # flat buffers, viewed [nstreams, width] per chunk: 16-byte aligned, contiguous at every width
+            wide = (self.max_chunk + 3) & ~3
+            self._wide = z((self.nstreams * wide,), torch.float32)
+            self._stage = z((self.nstreams * wide,), torch.int16)
         self.auto_states = z((self.nstreams, api.AUTO_STATE_BYTES), torch.uint8) if self.auto else None
         self.tones = None
         if tones is not None:
@@ -115,15 +133,34 @@ class LiveReceiver:
         return self.engine.decode_batch(self.kind, frames, states, dstates=self.dstates,
                                         out_stride=self.row_bytes)
 
+    def _widened(self, chunk):
+        """the int16 chunk as float32 (x / 32768, exact) in the preallocated buffer, for float rows"""
+        n, w = chunk.shape
+        w4 = (w + 3) & ~3
+        src = chunk
+        if w4 != w or not chunk.is_contiguous() or chunk.data_ptr() % 8:
+            src = self._stage[:n * w4].view(n, w4)     # fsk_b200_s16_to_f32 takes strides of 4 samples
+            src[:, :w].copy_(chunk)
+        out = self._wide[:n * w4].view(n, w4)
+        api.s16_to_f32(src, out=out)
+        return out
+
     def feed(self, chunk, lengths=None, opened=None, ended=None):
-        """chunk: float32 CUDA tensor [nstreams, width <= max_chunk]; lengths: int32 CUDA tensor [nstreams]
-        (samples valid in each row of the chunk) or None = the whole width.  opened / ended: bool CUDA tensors
-        [nstreams] or None: rows where a new stream starts with this chunk, rows whose stream ends with it
-        (both: a whole stream in one chunk).  Returns (text, counts)."""
+        """chunk: float32 CUDA tensor [nstreams, width <= max_chunk] (int16 with pcm16=True); lengths: int32 CUDA
+        tensor [nstreams] (samples valid in each row of the chunk) or None = the whole width.  opened / ended:
+        bool CUDA tensors [nstreams] or None: rows where a new stream starts with this chunk, rows whose stream
+        ends with it (both: a whole stream in one chunk).  Returns (text, counts)."""
         assert chunk.shape[0] == self.nstreams and chunk.shape[1] <= self.max_chunk
+        torch = api._torch()
+        want = torch.int16 if self.pcm16 else torch.float32
+        if chunk.dtype != want:
+            raise TypeError("LiveReceiver.feed: a %s chunk, this receiver takes %s" % (chunk.dtype, want))
+        if lengths is None:
+            lengths = chunk.shape[1]
+        if self._wide is not None:
+            chunk = self._widened(chunk)
         if opened is None and ended is None:
             return self._step(chunk, lengths)
-        torch = api._torch()
         dev = self.rows.device
         no = torch.zeros((self.nstreams,), dtype=torch.bool, device=dev)
         opened = no if opened is None else opened.to(device=dev, dtype=torch.bool)
