@@ -660,6 +660,11 @@ __device__ __forceinline__ Found find_frame_slide(const Ring rg, unsigned pos_of
 	acc[j][0] = acc[j][1] = acc[j][2] = acc[j][3] = 0.f;
     }
     corr_pass<W, L>(acc, p, tw + t, part, N);	/* the lowest candidate: a full correlation, phase index t + n */
+    /* the largest sample that has left each window since its last full correlation (see below) */
+    float gone[W];
+#pragma unroll
+    for (int j = 0; j < W; j++)
+	gone[j] = 0.f;
 
     Found best = { 0.f, 0.f, 0u, 0u, 0u };
     unsigned best_order = 0;
@@ -700,6 +705,7 @@ __device__ __forceinline__ Found find_frame_slide(const Ring rg, unsigned pos_of
 #pragma unroll
 	    for (int j = 0; j < W; j++) {
 		const float xr = pr[j][n], xa = pa[j][n];
+		gone[j] = fmaxf(gone[j], fabsf(xr));
 		acc[j][0] = fmaf(xa, ca.x, fmaf(-xr, cr.x, acc[j][0]));
 		acc[j][1] = fmaf(xa, ca.y, fmaf(-xr, cr.y, acc[j][1]));
 		acc[j][2] = fmaf(xa, ca.z, fmaf(-xr, cr.z, acc[j][2]));
@@ -707,9 +713,27 @@ __device__ __forceinline__ Found find_frame_slide(const Ring rg, unsigned pos_of
 	    }
 	}
 	t += step;
+	/* A sum that kept a loud sample (a click) carries a few ulp of it after the sample has left: past 16x
+	 * this lane's share of the window that is beyond the error the slide is allowed, and far past it the
+	 * window cancels to nothing.  A NaN or inf that left turned the sums into NaN (the unordered test).
+	 * Either way the windows are correlated afresh, as the lowest candidate was. */
+	bool stale = false;
 #pragma unroll
-	for (int j = 0; j < W; j++)
+	for (int j = 0; j < W; j++) {
 	    p[j] = ring + ring_wrap(ring_wrap(pos_off + t, R) + lw.beg[j], R);	/* window starts (fp64 re-sum) */
+	    const float amax = fmaxf(fmaxf(fabsf(acc[j][0]), fabsf(acc[j][1])), fmaxf(fabsf(acc[j][2]), fabsf(acc[j][3])));
+	    stale |= !(gone[j] <= 16.f * amax);
+	}
+	/* the lanes of a window hold shares of its sums that only add up together: all lanes of the group start
+	 * afresh, each with its samples n = part (mod L) as at the lowest candidate */
+	if (__any_sync(gmask, stale)) {
+#pragma unroll
+	    for (int j = 0; j < W; j++) {
+		acc[j][0] = acc[j][1] = acc[j][2] = acc[j][3] = 0.f;
+		gone[j] = 0.f;
+	    }
+	    corr_pass<W, L>(acc, p, tw + t, part, N);
+	}
     }
     return best;
 }
@@ -1253,9 +1277,16 @@ __device__ __forceinline__ float pfx_round(const float *ring, unsigned R, unsign
     float mag_mark = fast_sqrt(S.x * S.x + S.y * S.y);
     float mag_space = fast_sqrt(S.z * S.z + S.w * S.w);
     const float mag_hi = fmaxf(mag_mark, mag_space);
-    if (own && mag_hi != 0.f && fminf(mag_mark, mag_space) < eps_u + 2e-6f * mag_hi) {
-	/* too close to the :279 threshold for fp32 sums (see needs_resum): the window again, in fp64, phase
-	 * counted from its first sample (the per-sample table, from global memory: rare) */
+    /* The window is a difference of prefix values, so its fp32 error is a few ulp of the prefix at its
+     * boundary, not of the window.  A loud sample earlier in the lane-run (a click) leaves the prefix far above
+     * the window, and the difference cancels: past 16x the error exceeds the 2e-6 budget of needs_resum, and
+     * far past it the window reads as silence.  A NaN or inf there makes the difference NaN (the unordered
+     * test below).  Either way the window does not hold the sample, and the raw samples give it exactly. */
+    const float pmax = fmaxf(fmaxf(fabsf(P.x), fabsf(P.y)), fmaxf(fabsf(P.z), fabsf(P.w)));
+    if (own && (pmax > 16.f * mag_hi
+		|| (mag_hi != 0.f && !(fminf(mag_mark, mag_space) >= eps_u + 2e-6f * mag_hi)))) {
+	/* too close to the :279 threshold for fp32 sums (see needs_resum), cancelled or not finite: the window
+	 * again, in fp64, phase counted from its first sample (the per-sample table, from global memory: rare) */
 	double drm = 0., dim = 0., drs = 0., dis = 0.;
 	unsigned qq = base + i;
 	if (qq >= R)
