@@ -77,73 +77,6 @@ def test_random_mode_records_match_the_oracle(seed):
     assert decoded >= nwords, (mode, kw, decoded, nwords)
 
 
-STRESS_MODES = [("1200", {}), ("300", {}), ("rtty", dict(sample_rate=8000)), ("same", {}),
-                ("2400", dict(sample_rate=44100)), ("110", dict(sample_rate=11025, stopbits=2.0))]
-
-
-@pytest.mark.parametrize("mi", range(len(STRESS_MODES)))
-@pytest.mark.parametrize("seed", range(4))
-def test_dropouts_bursts_and_resume(mi, seed):
-    """Streams that keep losing and finding the carrier: bursts of frames separated by silence,
-    noise and truncated frames of random lengths (ring restarts, the 20-strike carrier drop,
-    session reports), decoded once in one go and once in record buffers of a few frames with
-    the saved state carried over -- both must equal the oracle's rx loop."""
-    mode, kw = STRESS_MODES[mi]
-    rx = orc.Mode(mode, **kw)
-    rng = np.random.default_rng(7000 + 10 * mi + seed)
-    spb = int(rx.derived().nsamples_per_bit)
-    streams = []
-    for s in range(4):
-        parts = []
-        for _ in range(int(rng.integers(2, 5))):
-            kind = int(rng.integers(0, 4))
-            gap = int(rng.integers(1, 60)) * spb + int(rng.integers(0, spb))
-            if kind == 0:
-                parts.append(np.zeros(gap, np.float32))
-            elif kind == 1:
-                parts.append((0.2 * rng.standard_normal(gap)).astype(np.float32))
-            words = rng.integers(0, 1 << rx.n_data_bits, int(rng.integers(2, 12)), dtype=np.uint64).astype(np.uint32)
-            a = orc.tx_words(rx, words, float(rng.uniform(0.2, 1.0)), 4096, True)
-            if kind == 3:
-                a = a[:int(rng.integers(a.size // 3, a.size))]      # cut inside a frame
-            parts.append(a)
-        x = np.concatenate(parts).astype(np.float32)
-        x = (x + np.float32(0.003) * rng.standard_normal(x.size).astype(np.float32)).astype(np.float32)
-        streams.append(x)
-    eng, _ = T.engine_for((mode, kw))
-    recs, st = T.rx_on_gpu(eng, streams)
-    wants = [orc.rx_run(rx, x, literal=False) for x in streams]
-    for s in range(len(streams)):
-        T.compare_frames(T.as_oracle_frames(recs[s]), wants[s]["frames"], "%s stream %d" % (mode, s))
-        T.compare_reports(T.reports_of(recs[s], st[s]), wants[s]["reports"], "%s stream %d" % (mode, s))
-
-    # the same in record buffers of 3 frames, resumed until every stream is done
-    torch = T.torch
-    n = max(len(a) for a in streams)
-    buf = np.zeros((len(streams), T.pad4(n)), np.float32)
-    for i, a in enumerate(streams):
-        buf[i, :len(a)] = a
-    d = torch.from_numpy(buf).to(T.dev())
-    lens = torch.from_numpy(np.array([len(a) for a in streams], np.int32)).to(T.dev())
-    states = None
-    got = [[] for _ in streams]
-    for _ in range(400):
-        frames, states = eng.rx_batch(d, nsamples=n, nsamples_each=lens, max_frames=3, states=states)
-        fr, s1 = mm.frames_to_numpy(frames), mm.states_to_numpy(states)
-        for i in range(len(streams)):
-            got[i].extend(fr[i, :s1["nframes"][i]].copy())
-        if (s1["done"] == 1).all():
-            break
-        # the binding hands the state back; the record count starts over for the next buffer
-        s2 = s1.copy()
-        s2["nframes"] = 0
-        states = torch.from_numpy(s2.view(np.int32).reshape(len(streams), -1)).to(T.dev())
-    else:
-        raise AssertionError("streams did not finish")
-    for i in range(len(streams)):
-        T.compare_frames(T.as_oracle_frames(got[i]), wants[i]["frames"], "%s stream %d resumed" % (mode, i))
-
-
 import refcases  # noqa: E402
 
 

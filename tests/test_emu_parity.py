@@ -38,14 +38,12 @@ def test_reference_vectors_on_the_emulated_kernels_eager_copies():
     assert " passed" in tail and "failed" not in tail
 
 
-def test_random_modes_and_dropouts_on_the_emulated_kernels():
-    """tests/emu_fuzz.py: 64 random framings / rates / bit orders, 24 streams that keep losing and
-    finding the carrier (also decoded in 3-frame record buffers with resume): oracle TX -> emulated
-    kernels -> records equal to the oracle's rx loop; and the second batch of reference-CLI option
-    vectors (tests/refcases.py MORE)."""
-    tail = run_emulated("random_mode or dropouts or second_batch or batched_kernels_print", "late", 1200,
-                        module="emu_fuzz.py")
-    assert "failed" not in tail and ("137 passed" in tail or "138 passed" in tail)     # one seed is ring-limited
+def test_random_modes_and_option_vectors_on_the_emulated_kernels():
+    """tests/emu_fuzz.py: 64 random framings / rates / bit orders: oracle TX -> emulated kernels -> records
+    equal to the oracle's rx loop; and the second batch of reference-CLI option vectors (tests/refcases.py
+    MORE).  Streams that keep losing and finding the carrier are in tests/test_gpu_carrier_sessions.py."""
+    tail = run_emulated("random_mode or second_batch or batched_kernels_print", "late", 1200, module="emu_fuzz.py")
+    assert "failed" not in tail and ("113 passed" in tail or "114 passed" in tail)     # one seed is ring-limited
 
 
 def test_every_instantiation_on_the_emulated_kernels_with_perturbed_units():

@@ -614,19 +614,34 @@ def _same_result(a, b):
     return a["frames"] == b["frames"] and a["reports"] == b["reports"]
 
 
+def _replays(rx, a, what):
+    """the screen's search and its replay of the loop's bookkeeping give the oracle's records and reports"""
+    want = orc.rx_run(rx, a, literal=False)
+    got, s = tie_screen.run(rx, a, delta=0.0)
+    assert _same_result(got, want), what
+    frames, reports, _ = tie_screen.replay(rx, s.calls)
+    assert frames == [f[:5] for f in want["frames"]] and reports == want["reports"], what
+    assert _same_result(tie_screen.flipped(rx, a, (-1, "conf", 0.0)), want), what      # nothing flipped
+
+
 def test_tie_screen_replays_the_oracle_exactly():
-    """delta = 0: the screen's search is the oracle's, records and reports bit for bit, on every golden
-    vector and on 64 random framings."""
+    """delta = 0: the screen's search is the oracle's, records and reports bit for bit, and so is its replay
+    of the rx loop's bookkeeping, on every golden vector, on 64 random framings and on the carrier-session
+    streams of every preset (tests/test_gpu_carrier_sessions.py)."""
     import golden_util as gu
     import refcases
+    import test_gpu_carrier_sessions as CS
     for case in refcases.EVERY:
         g = gu.load(case["name"])
         _, rx = gu.modes(case)
         a = gu.audio(case, g)
         if case["rxnoise"]:
             a = (a + np.float32(-0.5) * np.float32(np.float32(case["rxnoise"]) * 2)).astype(np.float32)
-        got, _ = tie_screen.run(rx, a, delta=0.0)
-        assert _same_result(got, orc.rx_run(rx, a, literal=False)), case["name"]
+        _replays(rx, a, case["name"])
+    for which in CS.L.PRESETS:
+        c = CS.case("per-candidate", which)
+        for j, x in enumerate(c.rows):
+            _replays(c.modes[j], x, (which, j))
     for seed in range(64):
         rng = np.random.default_rng(1000 + seed)
         mode, kw = emu_fuzz.random_mode(rng)
@@ -635,8 +650,7 @@ def test_tie_screen_replays_the_oracle_exactly():
         x = np.concatenate([np.zeros(int(rng.integers(0, 3 * int(m.derived().nsamples_per_bit) + 1)), np.float32),
                             orc.tx_words(m, words, float(rng.uniform(0.3, 1.0)), 4096, True)])
         x = (x + np.float32(0.01) * rng.standard_normal(x.size).astype(np.float32)).astype(np.float32)
-        got, _ = tie_screen.run(m, x, delta=0.0)
-        assert _same_result(got, orc.rx_run(m, x, literal=False)), (mode, kw)
+        _replays(m, x, (mode, kw))
 
 
 def test_tie_screen_flags_a_constructed_tie():
@@ -677,6 +691,93 @@ def test_the_screen_rejects_few_of_the_random_cases():
             total += len(screened)
         print("%s: %d of %d random streams screened out" % (fam, bad, total))
         assert bad <= 0.1 * total, (fam, bad, total)
+
+
+TIE_OFFSETS = [-1e-5, -1e-6, -1e-7, 1e-7, 1e-6, 1e-5]
+
+
+@pytest.mark.parametrize("eps", TIE_OFFSETS)
+def test_tie_screen_flags_a_threshold_tie_at_every_offset(eps):
+    """confidence_threshold within eps (relative) of the weakest frame's confidence, on both sides: the
+    re-runs alone flag the stream (a confidence moves by much more than delta)."""
+    import golden_util as gu
+    import refcases
+    case = refcases.BY_NAME["small-1200"]
+    g = gu.load(case["name"])
+    _, rx = gu.modes(case)
+    a = gu.audio(case, g)
+    a = (a + np.float32(0.02) * np.random.default_rng(1).standard_normal(a.size).astype(np.float32)).astype(np.float32)
+    want = orc.rx_run(rx, a, literal=False)
+    c = min(f[1] for f in want["frames"] if np.isfinite(f[1]))
+    tied = orc.Mode(case["rx_mode"], **dict(case["rx_mkw"], confidence=float(np.float32(c * (1 + eps)))))
+    _, robust = tie_screen.screen(tied, a)
+    assert not robust, eps
+
+
+def _fade(r):
+    """1200 baud: a burst at 0.8, then with no gap one at 0.8 r: near r = 0.25 the squelch decides the fade"""
+    m = orc.Mode("1200")
+    rng = np.random.default_rng(5)
+    a = orc.tx_words(m, rng.integers(0, 256, 6).astype(np.uint32), 0.8, 4096, True)
+    b = orc.tx_words(m, rng.integers(0, 256, 6).astype(np.uint32), 1.0, 4096, True)
+    bg = (0.003 * rng.standard_normal(a.size + b.size)).astype(np.float32)
+    return m, (np.concatenate([a, np.float32(0.8 * r) * b]) + bg).astype(np.float32)
+
+
+def _squelch_ratio(r):
+    """amplitude / (0.25 track_amplitude) - 1 at the first search that reaches into the fade"""
+    m, x = _fade(r)
+    res = orc.rx_run(m, x, literal=False, want_calls=True)
+    j = next(i for i, cl in enumerate(res["calls"]) if cl[8] > 0 and cl[10] + cl[9] >= x.size // 2)
+    track = np.float32(0)
+    for f in res["frames"]:
+        if f[5] + f[3] >= res["calls"][j][10]:
+            break
+        track = np.float32((track + f[2]) / np.float32(2))
+    return float(res["calls"][j][8]) / float(np.float32(0.25) * track) - 1
+
+
+@pytest.mark.parametrize("eps", TIE_OFFSETS)
+def test_tie_screen_flags_a_squelch_tie_at_every_offset(eps):
+    """A fade tuned (secant on its amplitude ratio) so that the squelch `amplitude < track_amplitude * 0.25`
+    (src/minimodem.c:1286) sits within eps of a tie: flagged at every offset.  The re-runs alone miss the
+    +-1e-5 ties (an amplitude moves by about delta / sqrt(n)); the replay's margin catches them."""
+    r0, r1 = 0.25, 0.26
+    g0, g1 = _squelch_ratio(r0) - eps, _squelch_ratio(r1) - eps
+    for _ in range(30):
+        if abs(g1) < abs(eps) / 2 + 6e-8 or g1 == g0:          # (6e-8: half a float32 ulp at 1)
+            break
+        r0, r1, g0 = r1, r1 - g1 * (r1 - r0) / (g1 - g0), g1
+        g1 = _squelch_ratio(r1) - eps
+    assert abs(g1) < abs(eps) / 2 + 6e-8, (eps, r1, g1)
+    m, x = _fade(r1)
+    _, robust = tie_screen.screen(m, x)
+    assert not robust, (eps, r1)
+    _, robust = tie_screen.screen(m, _fade(0.3)[1])
+    assert robust
+
+
+def _calls(*c):
+    """(confidence, amplitude, snr, bits, start, step) per search, as Search.calls records them"""
+    return [(np.float32(v[0]), np.float32(v[1]), 4.0, v[2], v[3], v[4]) for v in c]
+
+
+@pytest.mark.parametrize("eps", TIE_OFFSETS)
+def test_tie_screen_flags_refine_trigger_and_refine_keep_ties(eps):
+    """Set call sequences: the refine trigger `confidence < peak_confidence * 0.75` (:1278) and refine-keep
+    `confidence2 > confidence` between two different winners (:1357-1389) within eps of a tie are flagged;
+    clear of the tie, or between equal winners, they are not.  The re-runs cannot see these: the two sides
+    of each comparison are moved together."""
+    mode = orc.Mode("1200")
+    acquire = [(3.0, 0.5, 0x55, 10, 13), (3.0, 0.5, 0x55, 10, 5)]
+    for e, flagged in ((eps, True), (0.05 if eps > 0 else -0.05, False)):
+        refined = [(2.0, 0.5, 0x55, 32, 3)] if np.float32(2.25 * (1 + e)) < np.float32(2.25) else []
+        trig = _calls(*acquire, (2.25 * (1 + e), 0.5, 0x55, 30, 10), *refined)
+        assert bool(tie_screen.replay(mode, trig, tie_screen.DELTA)[2]) == flagged, ("trigger", e)
+        keep = _calls((3.0, 0.5, 0x55, 10, 13), (3.0 * (1 + e), 0.5, 0x57, 14, 5))
+        assert bool(tie_screen.replay(mode, keep, tie_screen.DELTA)[2]) == flagged, ("keep", e)
+    same = _calls((3.0, 0.5, 0x55, 10, 13), (3.0 * (1 + eps), 0.5, 0x55, 10, 5))
+    assert not tie_screen.replay(mode, same, tie_screen.DELTA)[2], "equal winners"
 
 
 PIN = [("1200", {}, 1000, 0.3, False), ("300", dict(stopbits=1.5), 8193, 1.7, True),

@@ -13,7 +13,17 @@ The perturbed search is a `find_frame` callback for orc.rx_run: it visits the ca
 orc_find_frame's order (oracle/fsk_oracle.c, orc_find_frame), takes each candidate's per-window mark and
 space magnitudes from the oracle itself (Plan.frame_analyze with an all-'d' expect string), and applies
 orc_frame_analyze's frame statistic to them in float32, in the oracle's serial order.  With delta = 0 it
-is the oracle's search, bit for bit (test_tie_screen_replays_the_oracle_exactly)."""
+is the oracle's search, bit for bit (test_tie_screen_replays_the_oracle_exactly).
+
+The rx loop's own comparisons (oracle/fsk_oracle.c, orc_rx_run) are checked by `replay`: the loop's
+bookkeeping restated in float32 on what each search returned.  A confidence moves a lot under the
+perturbation, so the re-runs alone flag a tie of the threshold; an amplitude is a mean over the frame's
+windows and moves by about delta / sqrt(n), and the refine trigger and refine-keep compare values the
+re-runs may move together -- so the squelch, the refine trigger and refine-keep get explicit margins.
+A comparison inside its margin is then decided the other way in one more run of the oracle's loop
+(`flipped`): the stream is robust only if that run gives the same records too.  (A slowly drifting
+frame, as SAME's 92.16 samples per bit, meets `confidence < 0.75 peak_confidence` close to the tie at
+every realignment, and most such refines find the frame they started from: only the later peak changes.)"""
 
 import numpy as np
 
@@ -90,6 +100,12 @@ def frame_stat(mark, space, expect):
     return conf, bits, ampl.astype(f32), snr
 
 
+def bound(delta, c, snr):
+    """How far a perturbation of delta can move a finite confidence, to first order and with a factor 2:
+    snr moves by delta (1 + snr) of itself, the divergence by 4 delta."""
+    return 2.0 * delta * (abs(float(c)) * (1.0 + abs(float(snr))) + 4.0 * abs(float(snr)))
+
+
 class Search:
     """find_frame callback for orc.rx_run: the oracle's frame search on perturbed magnitudes.
     `margin_ok` turns False when a decisive comparison of the search is closer than the perturbation
@@ -101,11 +117,10 @@ class Search:
         self.seed = int(seed)
         self.call = 0
         self.margin_ok = True
+        self.calls = []                                 # per call: (confidence, amplitude, snr, bits, start, step)
 
     def bound(self, c, snr):
-        """How far the perturbation can move a finite confidence, to first order and with a factor 2:
-        snr moves by delta (1 + snr) of itself, the divergence by 4 delta."""
-        return 2.0 * self.delta * (abs(float(c)) * (1.0 + abs(float(snr))) + 4.0 * abs(float(snr)))
+        return bound(self.delta, c, snr)
 
     def find_frame(self, ctx, samples, frame_nsamples, first, tmax, step, limit, expect, bits_out, ampl_out,
                     start_out):
@@ -152,6 +167,8 @@ class Search:
                         break
             if self.delta and bests:
                 self._check_margins(conf, snr, bests[-1], bests, last, lim)
+        self.calls.append((best_c, best_a, float(snr[bests[-1]]) if order and bests else 0.0, best_bits, best_t,
+                           int(step)))
         bits_out[0] = best_bits
         ampl_out[0] = float(best_a)
         start_out[0] = best_t
@@ -174,6 +191,103 @@ class Search:
                     self.margin_ok = False
 
 
+def replay(mode, calls, delta=0.0, events=None):
+    """orc_rx_run's bookkeeping (oracle/fsk_oracle.c:488-562) in float32 on the searches' results, in the
+    oracle's order: (frames, reports, ties).  `ties` lists every squelch, refine trigger or refine-keep
+    (between two different winners) closer than a perturbation of `delta` can move it -- a confidence by
+    Search.bound, an amplitude by delta of itself, both with a factor 2 -- as (call index, "conf" or
+    "ampl", the value that decides it the other way).  inf and 0 are classes the device decides exactly.
+    With delta = 0 the frames and reports are the oracle's.
+    `events`, a list, receives (kind, coarse call index) of every loop event, the state at the end last."""
+    ev = events.append if events is not None else (lambda e: None)
+    d = mode.derived()
+    thr, q, h = f32(mode.confidence_threshold), f32(0.75), f32(0.25)
+    fin = lambda c: np.isfinite(c) and c != 0
+    frames, reports, ties = [], [], []
+    carrier, noconf, nfd, cns = False, 0, 0, 0
+    peak, peak_b, track, ctot, atot = f32(0), 0.0, f32(0), f32(0), f32(0)
+    i = 0
+    while i < len(calls):
+        conf, ampl, snr, bits, start, step = calls[i]
+        i += 1
+        b = bound(delta, conf, snr) if fin(conf) else 0.0
+        if delta and fin(conf) and fin(peak) and abs(float(conf) - float(q * peak)) <= b + 0.75 * peak_b:
+            ties.append((i - 1, "conf", _across(conf, f32(peak * q))))             # the refine trigger
+        refine = bool(conf < peak * q)
+        if refine:
+            peak, peak_b = f32(0), 0.0
+        if delta and track > 0 and abs(float(ampl) - float(h * track)) <= 2 * delta * (float(ampl) + 0.25 * float(track)):
+            ties.append((i - 1, "ampl", _across(ampl, f32(track * h))))            # the squelch
+        squelched = bool(ampl < track * h) and conf > thr
+        if ampl < track * h:
+            conf = f32(0)
+        if conf <= thr:
+            ev(("strike-squelch" if squelched else "strike-threshold", i - 1))
+            noconf += 1
+            if noconf > 20 and carrier:
+                ev(("drop", i - 1))
+                reports.append((nfd, cns, ctot, atot, len(frames)))
+                carrier, cns, ctot, atot, nfd, track = False, 0, f32(0), f32(0), 0, f32(0)
+            continue
+        if carrier and noconf >= 15:
+            ev(("held-15-strikes", i - 1))
+        cns += int(d.frame_nsamples)
+        acquired = 0
+        if carrier:
+            cns += int(start) - int(d.nsamples_overscan)
+        else:
+            carrier, acquired, refine = True, 1, True
+            ev(("acquire", i - 1))
+        if refine and not acquired:
+            ev(("refine-in-session", i - 1))
+        if refine and conf < np.inf and step > 1:
+            c2, a2, snr2, bits2, start2, _ = calls[i]
+            i += 1
+            if delta and fin(c2) and (bits2, start2) != (bits, start) \
+                    and abs(float(c2) - float(conf)) <= bound(delta, c2, snr2) + b:
+                ties.append((i - 1, "conf", conf if c2 > conf else np.nextafter(conf, f32(np.inf))))  # refine-keep
+            if c2 > conf:
+                bits, ampl, start = bits2, a2, start2
+        track = f32((track + ampl) / f32(2))
+        if peak < conf:
+            peak, peak_b = conf, b
+        ctot, atot = f32(ctot + conf), f32(atot + ampl)
+        nfd += 1
+        noconf = 0
+        frames.append((bits, conf, ampl, start, acquired))
+    if carrier:
+        ev(("open-at-end", i - 1))
+        reports.append((nfd, cns, ctot, atot, len(frames)))
+    if noconf:
+        ev(("ends-mid-count", i - 1))
+    return frames, reports, ties
+
+
+def _across(v, edge):
+    """the value nearest `edge` on the other side of `v < edge`"""
+    return edge if v < edge else np.nextafter(edge, f32(0))
+
+
+def flipped(mode, x, tie):
+    """the oracle's rx loop on x with one search result replaced: tie = (call index, "conf" or "ampl",
+    value), as replay lists them"""
+    plan = orc.Plan(mode.sample_rate, mode.mark_f, mode.space_f, mode.band_width)
+    j, what, value = tie
+    n = [0]
+
+    def find_frame(ctx, samples, frame_nsamples, first, tmax, step, limit, expect, bits_out, ampl_out, start_out):
+        c = orc.lib().orc_find_frame(orc.C.byref(plan.p), samples, frame_nsamples, first, tmax, step, limit,
+                                     expect, bits_out, ampl_out, start_out)
+        n[0] += 1
+        if n[0] - 1 == j:
+            if what == "conf":
+                c = float(value)
+            else:
+                ampl_out[0] = float(value)
+        return c
+    return orc.rx_run(mode, x, literal=False, find_frame=find_frame)
+
+
 def record_key(res):
     """What must agree: the frames' count, bits, frame starts and acquire flags."""
     return [(f[0], f[3], f[4]) for f in res["frames"]]
@@ -192,5 +306,9 @@ def screen(mode, x, seeds=SEEDS):
     for k in range(seeds):
         res, s = run(mode, x, DELTA, 1 + k)
         if not s.margin_ok or record_key(res) != key:
+            return want, False
+    _, s = run(mode, x, 0.0)
+    for tie in replay(mode, s.calls, DELTA)[2]:
+        if record_key(flipped(mode, x, tie)) != key:
             return want, False
     return want, True
