@@ -14,15 +14,15 @@ flaky case, and all other streams are compared exactly."""
 import numpy as np
 import pytest
 
+import golden_util as gu
 import minimodem_b200 as mm
 import orc
-import test_gpu_parity as T
+import rxcases
+from gpudev import upload
+from rxcases import BAUDS, RATES, engine_for, rx_on_gpu
+from rxfam import as_oracle_frames, compare_frames, compare_reports, reports_of
 
 pytestmark = pytest.mark.gpu
-
-BAUDS = [75, 110, 150, 300, 600, 1200, 2400, 4800]
-RATES = [8000, 11025, 16000, 22050, 44100, 48000]
-
 
 def random_mode(rng):
     while True:
@@ -65,14 +65,14 @@ def test_random_mode_records_match_the_oracle(seed):
         x = np.concatenate([np.zeros(lead, np.float32), a])
         x = (x + np.float32(0.01) * rng.standard_normal(x.size).astype(np.float32)).astype(np.float32)
         streams.append(x)
-    eng, _ = T.engine_for((mode, kw))
-    recs, st = T.rx_on_gpu(eng, streams)
+    eng, _ = engine_for((mode, kw))
+    recs, st = rx_on_gpu(eng, streams)
     decoded = 0
     for s, x in enumerate(streams):
         want = orc.rx_run(rx, x, literal=False)
-        got = T.as_oracle_frames(recs[s])
-        T.compare_frames(got, want["frames"], "%s %r stream %d" % (mode, kw, s))
-        T.compare_reports(T.reports_of(recs[s], st[s]), want["reports"], "%s %r stream %d" % (mode, kw, s))
+        got = as_oracle_frames(recs[s])
+        compare_frames(got, want["frames"], "%s %r stream %d" % (mode, kw, s))
+        compare_reports(reports_of(recs[s], st[s]), want["reports"], "%s %r stream %d" % (mode, kw, s))
         decoded += len(got)
     assert decoded >= nwords, (mode, kw, decoded, nwords)
 
@@ -86,17 +86,17 @@ def test_second_batch_of_option_vectors(case):
     here the emulated kernels have to reproduce their records, decoded bytes and stat lines."""
     if case["ring_limited"]:
         # the kernels follow the flat semantic: all of the text, of which the reference printed the start
-        g = T.gu.load(case["name"])
-        _, rx = T.gu.modes(case)
-        a = T.gu.audio(case, g)
-        eng, _ = T.engine_for(case)
-        (recs,), st = T.rx_on_gpu(eng, [a])
-        got = T.as_oracle_frames(recs)
-        T.compare_frames(got, orc.rx_run(rx, a, literal=False)["frames"], case["name"])
+        g = gu.load(case["name"])
+        _, rx = gu.modes(case)
+        a = gu.audio(case, g)
+        eng, _ = engine_for(case)
+        (recs,), st = rx_on_gpu(eng, [a])
+        got = as_oracle_frames(recs)
+        compare_frames(got, orc.rx_run(rx, a, literal=False)["frames"], case["name"])
         out = orc.decode_records(rx, refcases.decoder_of(case, rx), orc.frame_records(got))
         assert out == bytes(g["text"]) and out.startswith(bytes(g["stdout"]))
         return
-    T.test_rx_batch_on_reference_vectors(case)
+    rxcases.check_reference_vector(case)
 
 
 @pytest.mark.parametrize("seed", range(40))
@@ -111,7 +111,7 @@ def test_batched_kernels_print_what_the_reference_cli_prints(seed, tmp_path):
     import sys
     sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden"))
     from make_golden import read_wav
-    from test_oracle_fuzz_vs_cli import random_invocation
+    from clicases import random_invocation
     if not orc.have_ref() or not os.path.exists(orc.REF_CLI):
         pytest.skip("needs the reference CLI (oracle/_ref)")
     rng = np.random.default_rng(12000 + seed)
@@ -127,11 +127,11 @@ def test_batched_kernels_print_what_the_reference_cli_prints(seed, tmp_path):
     flat = orc.rx_run(m, audio, literal=False)["frames"]
     if [f[:1] + f[3:5] for f in lit] != [f[:1] + f[3:5] for f in flat]:
         pytest.skip("the reference's ring changes this one")
-    eng, _ = T.engine_for((mode, kw))
+    eng, _ = engine_for((mode, kw))
     n = audio.size
-    buf = np.zeros((2, T.pad4(n)), np.float32)
+    buf = np.zeros((2, rxcases.pad4(n)), np.float32)
     buf[:, :n] = audio
-    frames, states = eng.rx_batch(T.torch.from_numpy(buf).to(T.dev()), nsamples=n)
+    frames, states = eng.rx_batch(upload(buf), nsamples=n)
     out, cnt = eng.decode_batch(mm.decoder_for_mode(mode, m.n_data_bits), frames, states)
     o, c = out.cpu().numpy(), cnt.cpu().numpy()
     for s in range(2):

@@ -176,9 +176,9 @@ def test_auto_oracle_reproduces_the_cli_auto_carrier_vectors(name):
 def test_gpu_auto_carrier_file_on_the_emulated_kernels():
     """tests/test_gpu_auto_carrier.py on the host SIMT emulation of the kernels (tests/emu), with the
     emulated sqrt moved by up to 64 ulp."""
-    import test_emu_parity
-    tail = test_emu_parity.run_emulated("not live_stream", "late", 1800, module="test_gpu_auto_carrier.py",
-                                        extra_env={"FSK_EMU_ULP": "64"})
+    from gpudev import run_emulated
+    tail = run_emulated("not live_stream", "late", 1800, module="test_gpu_auto_carrier.py",
+                        extra_env={"FSK_EMU_ULP": "64"})
     assert " passed" in tail and "failed" not in tail
 
 

@@ -16,24 +16,13 @@ import pytest
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, os.path.join(ROOT, "tests", "emu"))
 sys.path.insert(0, os.path.join(ROOT, "tests", "golden"))
-import emu_mode               # noqa: E402
 import golden_util as gu      # noqa: E402
 import orc                    # noqa: E402
 import refcases               # noqa: E402
 from make_golden import read_wav  # noqa: E402
+from clicases import emulation_as_product, random_invocation  # noqa: E402
 
 DROPIN = os.path.join(ROOT, "oracle", "_ref", "minimodem_dropin")
-
-
-def emulation_as_product():
-    """A directory in which the emulation build answers to the product library's name."""
-    emu_mode.build()
-    d = os.path.join(ROOT, "tests", "emu", "as_product")
-    os.makedirs(d, exist_ok=True)
-    link = os.path.join(d, "libfsk_b200.so")
-    if not os.path.islink(link):
-        os.symlink(os.path.join("..", "libfsk_b200_emu.so"), link)
-    return d
 
 
 def _nocarrier_ampl(stderr):
@@ -99,7 +88,6 @@ def test_dropin_cli_equals_reference_cli_on_a_random_invocation(seed, tmp_path):
     own src/fsk.c, for a random baud rate / sample rate / framing / bit order / tone pair: the same
     stdout, the same CARRIER / NOCARRIER lines (confidence to the parity tolerance)."""
     import numpy as np
-    from test_oracle_fuzz_vs_cli import random_invocation
     if not os.path.exists(DROPIN):
         pytest.skip("oracle/_ref/minimodem_dropin not built")
     rng = np.random.default_rng(9000 + seed)

@@ -7,22 +7,12 @@ GPU minutes are spent; timing, the approximate sqrt/div units and the hardware i
 checked only by the `gpu` run.  The emulation library is never loaded by the product."""
 import os
 import subprocess
-import sys
 
 import pytest
 
+from gpudev import run_emulated
+
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-
-
-def run_emulated(select, async_mode, timeout, module="test_gpu_parity.py", extra_env=None):
-    env = dict(os.environ, FSK_B200_EMU="1", FSK_EMU_ASYNC=async_mode, **(extra_env or {}))
-    env.pop("FSK_B200_LIB", None)
-    r = subprocess.run([sys.executable, "-m", "pytest", os.path.join(ROOT, "tests", module),
-                        "-m", "gpu", "-q", "-x", "-p", "no:cacheprovider", "-k", select],
-                       cwd=ROOT, env=env, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, timeout=timeout)
-    tail = r.stdout.decode(errors="replace")[-3000:]
-    assert r.returncode == 0, tail
-    return tail
 
 
 def test_parity_suite_on_the_emulated_kernels_late_copies():

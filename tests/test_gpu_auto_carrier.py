@@ -9,8 +9,6 @@ within 1e-5 (relative) of a tie -- its two largest band magnitudes, or its large
 frame search that tests/tie_screen.py's perturbed runs can tip marks the stream as not robust.  Robust
 streams must give the oracle's records and bands exactly (confidences within the usual bar); the device's
 band magnitudes are the fsk_b200_detect_carrier_batch ones, within about 1e-6 of the oracle's."""
-import os
-import re
 import zlib
 
 import numpy as np
@@ -20,88 +18,16 @@ import autoorc
 import golden_util as gu
 import orc
 import refcases
+from gpudev import dev, mm, pcm, rows, sync, torch, upload
+from rxcases import COVER, KEYS, auto_combos, tone_stream
+from rxfam import as_oracle_frames, compare_frames, compare_reports, reports_of
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-KERNELS = os.path.join(ROOT, "minimodem_b200", "csrc", "fsk_b200_kernels.cu")
 
-# (G, W, L) of AUTO_COMBOS -> a preset (mode, sample rate) whose default launch shape it is
-COVER = {
-    (8, 3, 2): ("1200", 48000),
-    (16, 2, 4): ("rtty", 8000),
-    (16, 3, 4): ("300", 48000),
-    (16, 3, 1): ("uic-train", 8000),
-    (32, 1, 4): ("rtty", 48000),
-    (32, 2, 4): ("110", 48000),
-    (32, 3, 2): ("uic-ground", 48000),
-}
 PRESETS = ["rtty", "tdd", "callerid", "uic-train", "uic-ground", "V.21", "2400", "1200", "600", "300", "110"]
-
-
-def auto_combos():
-    src = open(KERNELS).read()
-    m = re.search(r"#define AUTO_COMBOS\(X\)((?:[^\n]*\\\n)*[^\n]*)", src)
-    return {tuple(int(v) for v in t) for t in re.findall(r"X\((\d+), (\d+), (\d+)\)", m.group(1))}
 
 
 def test_the_cover_table_is_the_auto_combo_list():
     assert set(COVER) == auto_combos()
-
-
-def emulated():
-    import conftest
-    return conftest.EMU_DEVICE is not None
-
-
-def torch():
-    return pytest.importorskip("torch")
-
-
-def dev():
-    import conftest
-    if conftest.EMU_DEVICE is not None:
-        return conftest.EMU_DEVICE
-    assert torch().cuda.is_available(), "GPU tests need a CUDA device"
-    return torch().device("cuda:0")
-
-
-def sync():
-    if not emulated():
-        torch().cuda.synchronize()
-
-
-def mm():
-    import minimodem_b200
-    return minimodem_b200
-
-
-def fsk_audio(bits, spb, mark, space, rate, amplitude):
-    """Phase-continuous FSK: sample i carries bit floor(i / spb), at the exact (fractional) bit period."""
-    n = int(len(bits) * spb)
-    b = np.asarray(bits, np.int64)[np.minimum((np.arange(n) / spb).astype(np.int64), len(bits) - 1)]
-    f = np.where(b == 1, mark, space)
-    return (amplitude * np.sin(2 * np.pi * np.cumsum(f) / rate)).astype(np.float32)
-
-
-def tone_stream(rng, m, b_shift, nbands, nwords):
-    """One transmission of random data words on a random tone pair of this mode's band grid, the mark
-    tone off its band centre by up to 0.3 band.  UIC frames (the expect string 11110010 and 39 data bits,
-    no start or stop bits) come from fsk_audio after a mark leader; everything else from the oracle's
-    transmitter."""
-    bw = float(m.band_width)
-    lo, hi = max(2, 2 - b_shift), min(nbands - 3, nbands - 3 - b_shift)
-    bm = int(rng.integers(lo, max(lo + 1, hi)))
-    mark = float(bm * bw + rng.uniform(-0.3, 0.3) * bw)
-    amplitude = float(rng.uniform(0.3, 1.0))
-    if m.expect_data_string is not None:
-        bits = [1] * 10
-        for _ in range(nwords):
-            bits += [1, 1, 1, 1, 0, 0, 1, 0] + [int(v) for v in rng.integers(0, 2, 39)]
-        bits += [1] * 2
-        return fsk_audio(bits, float(m.sample_rate) / float(m.data_rate), mark, mark + b_shift * bw,
-                         m.sample_rate, amplitude)
-    tx = orc.Mode(m.mode, sample_rate=m.sample_rate, mark=mark, space=mark + b_shift * bw)
-    words = rng.integers(0, 1 << m.n_data_bits, nwords, dtype=np.uint64).astype(np.uint32)
-    return orc.tx_words(tx, words, amplitude, 4096, True)
 
 
 _CASES = {}
@@ -141,30 +67,19 @@ def engine(mode, rate):
     return e
 
 
-def rows(streams, dtype, align):
-    n = max(len(a) for a in streams)
-    stride = (n + align - 1) & ~(align - 1)
-    buf = np.zeros((len(streams), stride), dtype)
-    for i, a in enumerate(streams):
-        buf[i, :len(a)] = a
-    return buf, n
-
-
-def pcm(a):
-    return np.clip(np.round(a * 32768.0), -32768, 32767).astype(np.int16)
-
-
 def run_auto(eng, buf, n, lens, states=None, auto_states=None):
     t = torch()
-    frames, st, ast, bands = eng.rx_batch_auto(t.from_numpy(buf).to(dev()), nsamples=n,
-                                               nsamples_each=t.from_numpy(lens).to(dev()), states=states,
+    frames, st, ast, bands = eng.rx_batch_auto(upload(buf), nsamples=n,
+                                               nsamples_each=upload(lens), states=states,
                                                auto_states=auto_states, rec_band=True)
     sync()
     return frames, st, ast, bands
 
 
 def check_against_oracle(screened, fr, st, bands, what):
-    import test_gpu_parity as T
+    """rxfam.check_against_oracle's record and report checks on the robust streams, plus each record's band;
+    kept apart on purpose: the auto call's screen (autoorc.screen) has no frame-count bar for the streams it
+    screens out, and it may screen out one stream of a case, not half"""
     nok = 0
     for s, (w, robust) in enumerate(screened):
         if not robust:
@@ -172,16 +87,13 @@ def check_against_oracle(screened, fr, st, bands, what):
         nok += 1
         k = int(st["nframes"][s])
         recs = fr[s, :k]
-        T.compare_frames(T.as_oracle_frames(recs), w["frames"], "%s stream %d" % (what, s))
-        T.compare_reports(T.reports_of(recs, st[s]), w["reports"], "%s stream %d" % (what, s))
+        compare_frames(as_oracle_frames(recs), w["frames"], "%s stream %d" % (what, s))
+        compare_reports(reports_of(recs, st[s]), w["reports"], "%s stream %d" % (what, s))
         got_f = [int(b) for r, b in zip(recs, bands[s, :k]) if int(r["frame_start"]) != mm().FRAME_REPORT]
         got_r = [int(b) for r, b in zip(recs, bands[s, :k]) if int(r["frame_start"]) == mm().FRAME_REPORT]
         assert got_f == w["frame_band"], (what, s, got_f, w["frame_band"])
         assert got_r == w["report_band"][:len(got_r)], (what, s, got_r, w["report_band"])
     assert nok >= len(screened) - 1, (what, "screened out", len(screened) - nok)
-
-
-KEYS = sorted(COVER)
 
 
 @pytest.mark.gpu
@@ -234,7 +146,7 @@ def test_auto_instance_int16_rows_equal_the_float_rows(key):
         for b in (b32, b16):
             st0 = np.zeros(len(streams), mm().STATE_DTYPE)
             st0["pos"][:] = resume
-            states = t.from_numpy(st0.view(np.int32).reshape(len(streams), -1).copy()).to(dev())
+            states = upload(st0.view(np.int32).reshape(len(streams), -1).copy())
             outs.append(run_auto(eng, b, n, lens, states=states))
             G, W, L = key
             assert "k_rx_auto<G=%d,W=%d,L=%d," % (G, W, L) in eng.last_kernel()
@@ -273,8 +185,8 @@ def test_auto_state_carries_a_stream_across_calls(key, src):
         buf, n = rows(streams, np.float32, 4)
     lens = np.array([len(a) for a in streams], np.int32)
     whole = records_of(*(lambda r: (r[0], r[1], r[3]))(run_auto(eng, buf, n, lens)))
-    x = t.from_numpy(buf).to(dev())
-    each = t.from_numpy(lens).to(dev())
+    x = upload(buf)
+    each = upload(lens)
     states = t.zeros((len(streams), mm().STATE_WORDS), dtype=t.int32).to(dev())
     auto = t.zeros((len(streams), mm().AUTO_STATE_BYTES), dtype=t.uint8).to(dev())
     got = [[] for _ in streams]
@@ -289,7 +201,7 @@ def test_auto_state_carries_a_stream_across_calls(key, src):
             break
         assert "src=%s" % src in eng.last_kernel()
         st["nframes"][:] = 0
-        states = t.from_numpy(st.view(np.int32).reshape(len(streams), -1).copy()).to(dev())
+        states = upload(st.view(np.int32).reshape(len(streams), -1).copy())
     assert call >= 2 and got == whole, (key, src)
 
 
@@ -311,7 +223,7 @@ def test_a_stream_on_the_configured_tones_gives_the_fixed_tone_records():
     fa, sa, ast, bands = run_auto(eng, buf, n, lens)
     auto_kernel = eng.last_kernel()
     t = torch()
-    fb, sb = eng.rx_batch(t.from_numpy(buf).to(dev()), nsamples=n)
+    fb, sb = eng.rx_batch(upload(buf), nsamples=n)
     sync()
     assert eng.last_kernel().split("<")[1].split(",mode")[0] in auto_kernel, (eng.last_kernel(), auto_kernel)
     sa, sb = mm().states_to_numpy(sa), mm().states_to_numpy(sb)
@@ -338,9 +250,8 @@ def test_cli_auto_carrier_vectors_decode_on_the_device(name):
     fr, st = mm().frames_to_numpy(frames), mm().states_to_numpy(states)
     k = int(st["nframes"][0])
     recs = [r for r in fr[0, :k] if int(r["frame_start"]) != mm().FRAME_REPORT]
-    import test_gpu_parity as T
-    assert orc.ref_decode(rx, T.as_oracle_frames(recs)) == bytes(g["stdout"])
-    res = {"frames": T.as_oracle_frames(recs), "frame_band": [int(b) for r, b in zip(fr[0, :k], bands.cpu().numpy()[0, :k])
+    assert orc.ref_decode(rx, as_oracle_frames(recs)) == bytes(g["stdout"])
+    res = {"frames": as_oracle_frames(recs), "frame_band": [int(b) for r, b in zip(fr[0, :k], bands.cpu().numpy()[0, :k])
                                                               if int(r["frame_start"]) != mm().FRAME_REPORT]}
     want = [ln.strip() for ln in bytes(g["stderr"]).decode().splitlines() if ln.startswith("### CARRIER")]
     got = [autoorc.carrier_line(rx, b) for f, b in zip(res["frames"], res["frame_band"]) if f[4]]
@@ -375,8 +286,8 @@ def live_records(mode, rate, streams, cut):
             got[s] += r
     for o in range(0, n, cut):
         w = min(cut, n - o)
-        step(t.from_numpy(np.ascontiguousarray(buf[:, o:o + w])).to(dev()),
-             t.from_numpy(np.clip(lens - o, 0, w).astype(np.int32)).to(dev()))
+        step(upload(np.ascontiguousarray(buf[:, o:o + w])),
+             upload(np.clip(lens - o, 0, w).astype(np.int32)))
     eng.set_holdback(0)
     step(z((S, 4), t.float32), 0)
     assert int(dropped.cpu().numpy().sum()) == 0
@@ -411,8 +322,8 @@ def test_live_stream_records_do_not_depend_on_the_cut():
             return [texts[s] + text[s, :counts[s]].tobytes() for s in range(len(streams))]
         for o in range(0, n, cut):
             w = min(cut, n - o)
-            chunk = t.from_numpy(np.ascontiguousarray(buf[:, o:o + w])).to(dev())
-            valid = t.from_numpy(np.clip(lens - o, 0, w).astype(np.int32)).to(dev())
+            chunk = upload(np.ascontiguousarray(buf[:, o:o + w]))
+            valid = upload(np.clip(lens - o, 0, w).astype(np.int32))
             texts = take(lr.feed(chunk, valid))
         texts = take(lr.finish())
         outs.append(texts)

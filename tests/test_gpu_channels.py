@@ -13,22 +13,20 @@ import zlib
 import numpy as np
 import pytest
 
-import orc
-import tie_screen
-import test_gpu_stream_tones as TT
-from test_gpu_stream_tones import COVER, KEYS, ORIGINATE, ANSWER
+from gpudev import bands_tensor, dev, mm, pcm, records, rows, state_rows, sync, torch, upload
+from rxcases import (ANSWER, COVER, KEYS, ORIGINATE, channel_rows, check_channels_against_oracle, duplex_case,
+                     on_pair, push_model, random_states, run_channels, transmission)
 
 EINVAL = 22
 f32 = np.float32
-mm, torch, dev, sync, rows, pcm, on_pair = TT.mm, TT.torch, TT.dev, TT.sync, TT.rows, TT.pcm, TT.on_pair
 
 
 def test_gpu_channels_file_on_the_emulated_kernels():
     """The `gpu` tests below on the host SIMT emulation of the kernels: copies landing late, the
     approximate units moved by up to 64 ulp."""
-    import test_emu_parity
-    tail = test_emu_parity.run_emulated("gpu", "late", 2400, module="test_gpu_channels.py",
-                                        extra_env={"FSK_EMU_ULP": "64"})
+    from gpudev import run_emulated
+    tail = run_emulated("gpu", "late", 2400, module="test_gpu_channels.py",
+                        extra_env={"FSK_EMU_ULP": "64"})
     assert " passed" in tail and "failed" not in tail
 
 
@@ -41,65 +39,10 @@ def test_live_receiver_channels_need_tones():
 # --------------------------------------------------------------------------
 # helpers
 # --------------------------------------------------------------------------
-def t_(a):
-    """a device copy (the emulated device shares host memory, so from_numpy alone would alias `a`)"""
-    return torch().from_numpy(np.array(a, copy=True, order="C")).to(dev())
 
 
 def nbands_of(mode, rate):
     return int(mm().RxEngine.for_mode(mode, rate).params.nbands)
-
-
-def disabled_pair(rng, nb):
-    return [[nb, 5], [5, nb], [0xFFFFFFFF, 0xFFFFFFFF]][int(rng.integers(3))]
-
-
-def bands_tensor(b):
-    return t_(np.asarray(b, np.int64).astype(np.uint32).view(np.int32).reshape(-1, 2))
-
-
-def channel_rows(mode, rate, nrows, k, seed):
-    """nrows rows, each the sum of min(k, 2) transmissions on random valid pairs with lead-ins and AWGN;
-    k pairs per row: the row's signals first, then random valid pairs or disabled ones (k >= 3 has at least
-    one disabled channel per row).  Returns (streams, lengths, bands [nrows*k][2] uint32)."""
-    rng = np.random.default_rng(seed)
-    eng = mm().RxEngine.for_mode(mode, rate)
-    bw, nb = float(eng.params.band_width), int(eng.params.nbands)
-    streams, lens, bands = [], [], []
-    for r in range(nrows):
-        pairs = [TT.random_pair(rng, bw, nb) for _ in range(min(k, 2))]
-        x = np.zeros(0, np.float32)
-        for fm, fs in pairs:
-            m = on_pair(mode, rate, fm, fs)
-            a, _ = TT.lay_out(rng, m, TT.transmission(rng, m, int(rng.integers(3, 6)), float(rng.uniform(0.3, 0.8))),
-                              0.0)
-            if a.size > x.size:
-                a, x = x, a
-            x = x.copy()
-            x[:a.size] += a
-        x = (x + f32(rng.uniform(1e-4, 2e-3)) * rng.standard_normal(x.size).astype(np.float32)).astype(np.float32)
-        streams.append(x)
-        lens.append(x.size if r else int(x.size * 0.7))          # row 0 cut short of its stride
-        row = [list(mm().tone_bands(eng.params, *p)) for p in pairs]
-        for j in range(len(pairs), k):
-            if j == len(pairs) or rng.random() < 0.4:
-                row.append(disabled_pair(rng, nb))
-            else:
-                row.append(list(mm().tone_bands(eng.params, *TT.random_pair(rng, bw, nb))))
-        bands += row
-    return streams, np.array(lens, np.int32), np.array(bands, np.uint32)
-
-
-def run_channels(eng, buf, n, lens, bands, k, states=None, max_frames=None, per_row=True):
-    fr, st = eng.rx_batch_tones(t_(buf), bands, nsamples=n, nsamples_each=t_(lens) if per_row else None,
-                                states=states, max_frames=max_frames, channels_per_row=k)
-    sync()
-    return fr, st
-
-
-def records(fr, st):
-    fr, st = mm().frames_to_numpy(fr), mm().states_to_numpy(st)
-    return [fr[c, :int(st["nframes"][c])].tobytes() for c in range(len(st))], st
 
 
 # --------------------------------------------------------------------------
@@ -125,7 +68,7 @@ def test_channels_equal_the_tone_call_on_copied_rows(key):
             rep, lrep = np.repeat(buf, k, axis=0), np.repeat(lens, k)
             fa, sa = run_channels(eng, buf, nall, lens, bands, k, per_row=per_row)
             ka = eng.last_kernel()
-            fb, sb = eng.rx_batch_tones(t_(rep), bands, nsamples=nall, nsamples_each=t_(lrep) if per_row else None)
+            fb, sb = eng.rx_batch_tones(upload(rep), bands, nsamples=nall, nsamples_each=upload(lrep) if per_row else None)
             sync()
             kb = eng.last_kernel()
             what = (key, k, dtype.__name__, per_row)
@@ -143,29 +86,6 @@ def test_channels_equal_the_tone_call_on_copied_rows(key):
 # --------------------------------------------------------------------------
 # 2. and 3. the oracle: a full-duplex line and a passband
 # --------------------------------------------------------------------------
-def check_channels_against_oracle(eng, mode, rate, lines, pairs_per_row, k, what):
-    """pairs_per_row: per row, k (mark Hz, space Hz) pairs.  Every channel against the screened oracle on
-    its row and pair; the device decoder's text against the oracle's for every robust channel."""
-    flat = [p for ps in pairs_per_row for p in ps]
-    bands = eng.tone_bands([p[0] for p in flat], [p[1] for p in flat], device=dev())
-    buf, n = rows(lines, np.float32, 4)
-    lens = np.array([a.size for a in lines], np.int32)
-    frames, states = run_channels(eng, buf, n, lens, bands, k)
-    assert eng.last_kernel().endswith(" channels=%d" % k), eng.last_kernel()
-    screened = [tie_screen.screen(on_pair(mode, rate, *p), lines[c // k]) for c, p in enumerate(flat)]
-    fr, st = mm().frames_to_numpy(frames), mm().states_to_numpy(states)
-    assert (st["done"] == 1).all()
-    TT.check_against_oracle(screened, fr, st, what)
-    out, cnt = eng.decode_batch(mm().decoder_for_mode(mode, int(eng.params.n_data_bits)), frames, states)
-    sync()
-    out, cnt = out.cpu().numpy(), cnt.cpu().numpy()
-    rx = orc.Mode(mode, sample_rate=rate)
-    texts = []
-    for c, (w, robust) in enumerate(screened):
-        texts.append(out[c, :cnt[c]].tobytes())
-        if robust:
-            assert texts[-1] == orc.decode_records(rx, rx.decoder, orc.frame_records(w["frames"])), (what, c)
-    return texts
 
 
 @pytest.mark.gpu
@@ -176,8 +96,8 @@ def test_full_duplex_bell103_lines_against_the_oracle():
     mo, ma = on_pair("300", 48000, *ORIGINATE), on_pair("300", 48000, *ANSWER)
     lines = []
     for _ in range(3):
-        a = TT.transmission(rng, mo, int(rng.integers(4, 7)), float(rng.uniform(0.2, 0.8)))
-        b = TT.transmission(rng, ma, int(rng.integers(4, 7)), float(rng.uniform(0.2, 0.8)))
+        a = transmission(rng, mo, int(rng.integers(4, 7)), float(rng.uniform(0.2, 0.8)))
+        b = transmission(rng, ma, int(rng.integers(4, 7)), float(rng.uniform(0.2, 0.8)))
         oa, ob = (int(v) for v in rng.integers(0, 3000, 2))
         x = np.zeros(max(oa + a.size, ob + b.size) + int(rng.integers(0, 1500)), np.float32)
         x[oa:oa + a.size] += a
@@ -202,7 +122,7 @@ def test_rtty_passband_against_the_oracle():
             mark = 700.0 + 400.0 * i + float(rng.uniform(-20, 20))
             ps.append((mark + 170.0, mark))
             m = on_pair("rtty", 8000, *ps[-1])
-            a = TT.transmission(rng, m, int(rng.integers(4, 7)), float(rng.uniform(0.2, 0.6)))
+            a = transmission(rng, m, int(rng.integers(4, 7)), float(rng.uniform(0.2, 0.6)))
             a = np.concatenate([np.zeros(int(rng.integers(0, 1500)), np.float32), a])
             y = np.zeros(max(x.size, a.size), np.float32)
             y[:x.size] += x
@@ -221,8 +141,8 @@ def test_rtty_passband_against_the_oracle():
 # 4. disabled channels, 5. output overflow
 # --------------------------------------------------------------------------
 def duplex_rows():
-    """Three Bell103 lines of test_gpu_stream_tones: both directions summed, originate only, answer only"""
-    streams, _, _ = TT.duplex_case()
+    """Three Bell103 lines of rxcases.duplex_case: both directions summed, originate only, answer only"""
+    streams, _, _ = duplex_case()
     return [streams[6], streams[0], streams[1]]
 
 
@@ -248,8 +168,8 @@ def test_a_disabled_channel_is_skipped_and_leaves_its_row_alone():
             st0 = np.zeros(9, mm().STATE_DTYPE)
             st0["pos"][c], st0["carrier"][c], st0["track_amplitude"][c], st0["nframes"][c] = 1234, 1, 0.5, 2
             frames = t.full((9, eng.max_frames(n), 5), 0x5A5A5A5A, dtype=t.int32).to(dev())
-            fb, sb = eng.rx_batch_tones(t_(buf), bands, nsamples=n, nsamples_each=t_(lens), frames=frames,
-                                        states=TT.state_rows(st0), channels_per_row=k)
+            fb, sb = eng.rx_batch_tones(upload(buf), bands, nsamples=n, nsamples_each=upload(lens), frames=frames,
+                                        states=state_rows(st0), channels_per_row=k)
             sync()
             assert (frames.cpu().numpy()[c] == 0x5A5A5A5A).all(), (c, bad)
             rb, sb = records(fb, sb)
@@ -282,7 +202,7 @@ def test_channel_output_overflow_resumes_to_the_records_of_one_pass(src):
         if (st["done"] == 1).all():
             break
         st["nframes"][:] = 0
-        states = TT.state_rows(st)
+        states = state_rows(st)
     assert call >= 2 and got == whole
     st["nframes"] = sw["nframes"]
     assert st.tobytes() == sw.tobytes()
@@ -291,40 +211,6 @@ def test_channel_output_overflow_resumes_to_the_records_of_one_pass(src):
 # --------------------------------------------------------------------------
 # 6. the push against a numpy model
 # --------------------------------------------------------------------------
-def push_model(rows_, fill, states, k, bands, nbands, chunk, clen):
-    rows_, fill, states = rows_.copy(), fill.copy(), states.copy()
-    dropped = np.zeros(len(fill), np.int64)
-    stride = rows_.shape[1]
-    for r in range(len(fill)):
-        have = int(fill[r])
-        ch = range(r * k, r * k + k)
-        act = [c for c in ch if bands is None or (bands[c][0] < nbands and bands[c][1] < nbands)]
-        m = min((min(int(states["pos"][c]), have) for c in act), default=have)
-        tail = have - m
-        old = rows_[r].copy()
-        rows_[r, :tail] = old[m:have]
-        ln = int(clen[r])
-        drop = max(0, ln - (stride - tail))
-        ln -= drop
-        rows_[r, tail:tail + ln] = chunk[r, :ln]
-        fill[r], dropped[r] = tail + ln, drop
-        for c in ch:
-            p = min(int(states["pos"][c]), have)
-            states["pos"][c] = p - min(p, m)
-            states["nframes"][c] = 0
-            states["done"][c] = 0
-    return rows_, fill, states, dropped
-
-
-def random_states(rng, n, fill, k):
-    st = np.frombuffer(rng.integers(0, 2**32, n * mm().STATE_WORDS, dtype=np.uint64).astype(np.uint32).tobytes(),
-                       mm().STATE_DTYPE).copy()
-    for c in range(n):
-        have = int(fill[c // k])
-        u = rng.random()
-        st["pos"][c] = (int(rng.integers(0, have + 1)) if u < 0.7 else
-                        have + int(rng.integers(1, 1000)) if u < 0.9 else int(rng.integers(2**32, 2**40)))
-    return st
 
 
 @pytest.mark.gpu
@@ -353,9 +239,9 @@ def test_push_follows_the_channel_rule():
             clen = rng.integers(0, 301, nrows).astype(np.int32)
             clen[0] = 300
             want = push_model(rows0, fill.astype(np.int64), st0, k, bands, nb, chunk, clen)
-            R, F, S, D = t_(rows0), t_(fill), TT.state_rows(st0), t_(np.full(nrows, -1, np.int32))
-            bt = t_(bands.view(np.int32)) if bands is not None else None
-            mm().stream_push(R, F, S, t_(chunk), t_(clen), dropped=D, channels_per_row=k, tone_bands=bt, nbands=nb)
+            R, F, S, D = upload(rows0), upload(fill), state_rows(st0), upload(np.full(nrows, -1, np.int32))
+            bt = upload(bands.view(np.int32)) if bands is not None else None
+            mm().stream_push(R, F, S, upload(chunk), upload(clen), dropped=D, channels_per_row=k, tone_bands=bt, nbands=nb)
             sync()
             what = (k, with_bands)
             assert (R.cpu().numpy() == want[0]).all(), what
@@ -366,8 +252,8 @@ def test_push_follows_the_channel_rule():
             if with_bands:
                 assert want[1][2] == min(int(clen[2]), stride)  # row 2 kept nothing
             if k == 1 and not with_bands:
-                R2, F2, S2, D2 = t_(rows0), t_(fill), TT.state_rows(st0), t_(np.full(nrows, -1, np.int32))
-                ch2, cl2 = t_(chunk), t_(clen)
+                R2, F2, S2, D2 = upload(rows0), upload(fill), state_rows(st0), upload(np.full(nrows, -1, np.int32))
+                ch2, cl2 = upload(chunk), upload(clen)
                 p = lambda x: C.c_void_p(x.data_ptr())
                 assert mm().lib().fsk_b200_stream_push(p(R2), nrows, stride, p(F2), p(S2), p(ch2), 300, p(cl2), 0,
                                                        p(D2), None) == 0
@@ -419,7 +305,7 @@ def test_live_receiver_with_channels_does_not_depend_on_the_cut():
             chunk = np.zeros((nrows, max_chunk), np.float32)
             for r in range(nrows):
                 chunk[r, :m[r]] = buf[r, fed[r]:fed[r] + m[r]]
-            texts = take(lr.feed(t.from_numpy(chunk).to(dev()), t.from_numpy(m.astype(np.int32)).to(dev())))
+            texts = take(lr.feed(upload(chunk), upload(m.astype(np.int32))))
             fed += m
         texts = take(lr.finish())
         assert texts == whole, max_chunk

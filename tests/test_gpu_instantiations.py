@@ -25,32 +25,13 @@ import minimodem_b200 as mm
 import orc
 import tie_screen
 import txorc
+from gpudev import dev, emulated, rows, sync, torch, upload
+from rxcases import engine, framing, oracle_mode, session_case
+from rxfam import FAMILIES, PER_CAND, PRESETS, compare_rx, set_env
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 KERNELS = os.path.join(ROOT, "minimodem_b200", "csrc", "fsk_b200_kernels.cu")
 EPS = np.float32(1.1920928955078125e-07)
-
-
-def emulated():
-    import conftest
-    return conftest.EMU_DEVICE is not None
-
-
-def torch():
-    return pytest.importorskip("torch")
-
-
-def dev():
-    import conftest
-    if conftest.EMU_DEVICE is not None:
-        return conftest.EMU_DEVICE
-    assert torch().cuda.is_available(), "GPU tests need a CUDA device"
-    return torch().device("cuda:0")
-
-
-def sync():
-    if not emulated():
-        torch().cuda.synchronize()
 
 
 # ---------------------------------------------------------------------------------------------------
@@ -60,7 +41,6 @@ def sync():
 # bit periods of 40..160 samples, so that the windows tile (shared-segment and prefix-table kernels),
 # "long" = bit periods over 1536 samples (the twiddle table leaves shared memory: the generic kernels).
 # n = the window count (expect string length) that makes the launcher pick the shape.
-PER_CAND = {"FSK_B200_MULTI": "0", "FSK_B200_PREFIX": "0"}
 
 
 def _fast(G, W, L, n):
@@ -180,53 +160,6 @@ def test_the_tables_cover_every_instantiation():
 # ---------------------------------------------------------------------------------------------------
 # random framings
 # ---------------------------------------------------------------------------------------------------
-PAIRS = {"short": [(b, r) for b in emu_fuzz.BAUDS for r in emu_fuzz.RATES if 10 <= r / b <= 60],
-         "tile": [(600, 48000), (300, 48000), (1200, 48000)],
-         "long": [(25, 48000), (20, 44100)]}
-
-
-def framing(cls, n, seed):
-    """(mode, kw, expect override or None): a random framing of class `cls` whose expect string has n
-    windows -- its own if it has n, else its own cut to n or continued with don't-care windows"""
-    rng = np.random.default_rng(seed)
-    pairs = PAIRS[cls]
-    while True:
-        baud, rate = pairs[int(rng.integers(0, len(pairs)))]
-        kw = dict(sample_rate=rate)
-        kw["n_data_bits"] = int(rng.choice([5, 6, 7, 8, 9, 12, 16] if n < 24 else [n - 8, n - 6, n - 4]))
-        kw["startbits"] = int(rng.choice([1, 1, 2]))
-        kw["stopbits"] = float(rng.choice([1.0, 1.0, 1.5, 2.0]))
-        kw["msb_first"] = bool(rng.integers(0, 2))
-        kw["invert_start_stop"] = bool(rng.integers(0, 2))
-        kw["inverted"] = bool(rng.integers(0, 2))
-        if cls == "tile" and kw["stopbits"] == 1.5:
-            continue
-        try:
-            m = orc.Mode(str(baud), **kw)
-            d = m.derived()
-            orc.Plan(m.sample_rate, m.mark_f, m.space_f, m.band_width)
-        except Exception:
-            continue
-        if max(m.mark_f, m.space_f) >= rate / 2 - m.band_width:
-            continue
-        own = bytes(d.expect_data)
-        exp = None if len(own) == n else (own[:n] if len(own) > n else own + b"d" * (n - len(own)))
-        return str(baud), kw, exp
-
-
-def oracle_mode(mode, kw, exp):
-    m = orc.Mode(mode, **kw)
-    m.expect_data_string = exp
-    return m
-
-
-def engine(mode, kw, exp):
-    names = dict(startbits="nstartbits", stopbits="nstopbits")
-    ov = {names.get(k, k): v for k, v in kw.items() if k != "sample_rate"}
-    cfg = mm.rx_config_for_mode(mode, kw.get("sample_rate", 48000), **ov)
-    if exp is not None:
-        cfg.expect_data_string = exp
-    return mm.RxEngine(mm.rx_params(cfg))
 
 
 _CASES = {}
@@ -265,34 +198,6 @@ SCREEN_COUNT = {}
 REACHED = set()
 
 
-def compare_rx(case, recs, st, what):
-    import test_gpu_parity as T
-    mode, kw, exp, m, streams, screened = case
-    assert (st["done"] == 1).all(), what
-    for s, (want, robust) in enumerate(screened):
-        got = T.as_oracle_frames(recs[s])
-        if robust:
-            T.compare_frames(got, want["frames"], "%s stream %d" % (what, s))
-            T.compare_reports(T.reports_of(recs[s], st[s]), want["reports"], "%s stream %d" % (what, s))
-        else:
-            assert abs(len(got) - len(want["frames"])) <= 1, (what, s, len(got), len(want["frames"]))
-
-
-def _setenv(monkeypatch, env):
-    for k in ("FSK_B200_LANES", "FSK_B200_SPLIT", "FSK_B200_MULTI", "FSK_B200_PREFIX", "FSK_B200_PFX_FILL"):
-        monkeypatch.delenv(k, raising=False)
-    for k, v in env.items():
-        monkeypatch.setenv(k, v)                # read when the engine is created
-
-
-def _rows(streams, n, dtype, align=4):
-    stride = (n + align - 1) & ~(align - 1)
-    buf = np.zeros((len(streams), stride), dtype)
-    for i, a in enumerate(streams):
-        buf[i, :len(a)] = a
-    return buf
-
-
 def _skip_tma(key):
     if emulated() and len(key) == 6 and key[3] == 3 and key[4] == 1:
         pytest.skip("the host emulation does not model cp.async.bulk / mbarrier")
@@ -310,19 +215,19 @@ def test_rx_instantiation_on_random_framings(key, monkeypatch):
     row = RX_TABLE[key]
     case = rx_case(row["cls"], row["n"])
     mode, kw, exp, m, streams, screened = case
-    _setenv(monkeypatch, row["env"])
+    set_env(monkeypatch, row["env"])
     eng = engine(mode, kw, exp)
     assert eng.params.expect_n_bits == row["n"]
     n = max(len(a) for a in streams)
     lens = np.array([len(a) for a in streams], np.int32)
     t = torch()
-    frames, states = eng.rx_batch(t.from_numpy(_rows(streams, n, np.float32)).to(dev()), nsamples=n,
-                                  nsamples_each=t.from_numpy(lens).to(dev()))
+    frames, states = eng.rx_batch(upload(rows(streams, np.float32, n=n)[0]), nsamples=n,
+                                  nsamples_each=upload(lens))
     sync()
     assert kernel_key(eng.last_kernel()) == key, eng.last_kernel()
     REACHED.add(key)
     fr, st = mm.frames_to_numpy(frames), mm.states_to_numpy(states)
-    compare_rx(case, [fr[i, :st["nframes"][i]] for i in range(len(streams))], st, "%s %s %r" % (key, mode, kw))
+    compare_rx(screened, [fr[i, :st["nframes"][i]] for i in range(len(streams))], st, "%s %s %r" % (key, mode, kw))
     fam = "mode%d" % key[3] if key[0] != "generic" else "generic"
     c = SCREEN_COUNT.setdefault(fam, [0, 0])
     c[0] += sum(1 for _, r in screened if not r)
@@ -337,13 +242,13 @@ def test_rx_instantiation_int16_rows_equal_the_float_rows(key, monkeypatch):
     in one pass and resumed from a position that is not a multiple of 8."""
     row = RX_TABLE[key]
     mode, kw, exp, m, streams, _ = rx_case(row["cls"], row["n"])
-    _setenv(monkeypatch, row["env"])
+    set_env(monkeypatch, row["env"])
     eng = engine(mode, kw, exp)
     n = max(len(a) for a in streams)
     t = torch()
-    pcm = _rows([np.clip(np.round(a * 32768.0), -32768, 32767) for a in streams], n, np.int16, 8)
-    lens = t.from_numpy(np.array([len(a) for a in streams], np.int32)).to(dev())
-    d16 = t.from_numpy(pcm).to(dev())
+    pcm, _ = rows([np.clip(np.round(a * 32768.0), -32768, 32767) for a in streams], np.int16, 8, n=n)
+    lens = upload(np.array([len(a) for a in streams], np.int32))
+    d16 = upload(pcm)
     f32 = mm.s16_to_f32(d16)
     fr_a, st_a = eng.rx_batch(f32, nsamples=n, nsamples_each=lens)
     fr_b, st_b = eng.rx_batch(d16, nsamples=n, nsamples_each=lens)
@@ -360,7 +265,7 @@ def test_rx_instantiation_int16_rows_equal_the_float_rows(key, monkeypatch):
     resume = mm.states_to_numpy(st_b).copy()
     resume[:] = np.zeros(1, resume.dtype)
     resume["pos"][:] = 13
-    st_c = t.from_numpy(resume.view(np.int32).reshape(len(streams), -1).copy()).to(dev())
+    st_c = upload(resume.view(np.int32).reshape(len(streams), -1).copy())
     st_d = st_c.clone()
     fr_c, st_c = eng.rx_batch(f32, nsamples=n, nsamples_each=lens, states=st_c)
     fr_d, st_d = eng.rx_batch(d16, nsamples=n, nsamples_each=lens, states=st_d)
@@ -403,7 +308,7 @@ def test_find_frame_instantiation_per_bit_magnitudes_vs_fp64(key, monkeypatch):
     row = FF_TABLE[key]
     mode, kw, exp = framing(row["cls"], row["n"], 9000 + row["n"] + (500 if row["cls"] == "long" else 0))
     m = oracle_mode(mode, kw, exp)
-    _setenv(monkeypatch, row["env"])
+    set_env(monkeypatch, row["env"])
     eng = engine(mode, kw, exp)
     p = eng.params
     assert p.expect_n_bits == row["n"]
@@ -423,7 +328,7 @@ def test_find_frame_instantiation_per_bit_magnitudes_vs_fp64(key, monkeypatch):
         w[:seg.size] = seg
         buf[s] = (w + sigmas[s % 3] * rng.standard_normal(wlen)).astype(np.float32)
     t = torch()
-    T = lambda a, dt: t.from_numpy(np.ascontiguousarray(np.asarray(a).astype(dt))).to(dev())
+    T = lambda a, dt: upload(np.ascontiguousarray(np.asarray(a).astype(dt)))
     full = lambda v, dt: T(np.full(nstreams, v), dt)
     step = max(tmc // 8, 1)
     frames, mags = eng.find_frame_batch(T(buf, np.float32), full(wlen, np.int32), full(p.nsamples_overscan, np.int32),
@@ -544,14 +449,14 @@ def test_tx_instantiation_on_random_configurations(fmt, align, lut):
         assert (out.data_ptr() % 16 == 0 and (stride * out.element_size()) % 16 == 0) == (align == "aligned")
         states = te.new_states(n, dev())
         lens = t.tensor([len(x) for x in texts], dtype=t.int32).to(dev())
-        _, cnt = te.text_batch(t.from_numpy(tb).to(dev()), lens, states, 0, out=out)
+        _, cnt = te.text_batch(upload(tb), lens, states, 0, out=out)
         sync()
         c1 = cnt.cpu().numpy().copy()
         a1 = flat.cpu().numpy().copy()
         # an empty tick: the idle tone where a byte went out, then the trailer
         zero = t.zeros((n,), dtype=t.int32, device=dev())
         flat.fill_(sentinel)
-        _, cnt2 = te.text_batch(t.from_numpy(tb).to(dev()), zero, states, mm.TX_IDLE_IF_EMPTY | mm.TX_FINAL, out=out)
+        _, cnt2 = te.text_batch(upload(tb), zero, states, mm.TX_IDLE_IF_EMPTY | mm.TX_FINAL, out=out)
         sync()
         c2 = cnt2.cpu().numpy().copy()
         a2 = flat.cpu().numpy().copy()
@@ -594,9 +499,9 @@ def test_tx_batch_odd_stride(lut):
     ref0 = orc.tx_words(m, words[0], 1.0, lut, True)
     nout = ref0.size + 5
     stride = nout | 1
-    table = t.from_numpy(mm.sin_table(lut)).to(dev())
+    table = upload(mm.sin_table(lut))
     out = t.full((n, stride), -3.0, dtype=t.float32, device=dev())
-    mm.tx_batch(cfg, t.from_numpy(words.astype(np.int32)).to(dev()), nout, table=table, out=out, stride=stride)
+    mm.tx_batch(cfg, upload(words.astype(np.int32)), nout, table=table, out=out, stride=stride)
     sync()
     o = out.cpu().numpy()
     for s in range(n):
@@ -630,7 +535,6 @@ def test_tie_screen_replays_the_oracle_exactly():
     streams of every preset (tests/test_gpu_carrier_sessions.py)."""
     import golden_util as gu
     import refcases
-    import test_gpu_carrier_sessions as CS
     for case in refcases.EVERY:
         g = gu.load(case["name"])
         _, rx = gu.modes(case)
@@ -638,8 +542,8 @@ def test_tie_screen_replays_the_oracle_exactly():
         if case["rxnoise"]:
             a = (a + np.float32(-0.5) * np.float32(np.float32(case["rxnoise"]) * 2)).astype(np.float32)
         _replays(rx, a, case["name"])
-    for which in CS.L.PRESETS:
-        c = CS.case("per-candidate", which)
+    for which in PRESETS:
+        c = session_case(FAMILIES["per-candidate"], which)
         for j, x in enumerate(c.rows):
             _replays(c.modes[j], x, (which, j))
     for seed in range(64):
@@ -680,8 +584,7 @@ def test_the_screen_rejects_few_of_the_random_cases():
     for key, row in RX_TABLE.items():
         fam = "generic" if key[0] == "generic" else "mode%d" % key[3]
         fams.setdefault(fam, set()).add((row["cls"], row["n"]))
-    import conftest
-    if conftest.EMU_DEVICE is not None:
+    if emulated():
         pytest.skip("counted at the device's sizes, without the emulation")
     for fam, cases in sorted(fams.items()):
         bad = total = 0

@@ -23,71 +23,17 @@ default shape.
 
 Under FSK_B200_EMU=1 (tests/emu) the file runs on the host emulation of the kernels (test_emu_parity.py
 runs it with copies landing early and late); the TMA bulk fill is not modelled there and its rows skip."""
-import re
 import zlib
 
 import numpy as np
 import pytest
 
-import autoorc
 import minimodem_b200 as mm
-import orc
-import test_gpu_instantiations as I
 import tie_screen
-
-SMEM_MAX = 232448          # cudaDevAttrMaxSharedMemoryPerBlockOptin of an H100 (and of the emulation)
-KNOBS = ("FSK_B200_LANES", "FSK_B200_SPLIT", "FSK_B200_MULTI", "FSK_B200_PREFIX", "FSK_B200_PFX_FILL",
-         "FSK_B200_RING", "FSK_B200_WPB", "FSK_B200_NO_SLIDE")
-PER_CAND = {"FSK_B200_MULTI": "0", "FSK_B200_PREFIX": "0"}
-SHARED = {"FSK_B200_MULTI": "2", "FSK_B200_PREFIX": "0"}
-
-# family -> the call, the rows, the environment, and the kernel it must launch: (last_kernel name, mode,
-# fill); `cls` / `n`: the random framing of test_gpu_instantiations.framing that the family also runs
-FAMILIES = {
-    "per-candidate": dict(call="rx", src="f32", env=PER_CAND, kern=("k_rx", 0, 0), cls="short", n=10),
-    "per-candidate-noslide": dict(call="rx", src="f32", env=dict(PER_CAND, FSK_B200_NO_SLIDE="1"),
-                                  kern=("k_rx", 0, 0), cls="short", n=12),
-    "per-candidate-s16": dict(call="rx", src="s16", env=PER_CAND, kern=("k_rx", 0, 0), cls="short", n=11),
-    "shared-segment": dict(call="rx", src="f32", env=SHARED, kern=("k_rx", 2, 0), cls="tile", n=10),
-    "shared-segment-s16": dict(call="rx", src="s16", env=SHARED, kern=("k_rx", 2, 0), cls="tile", n=11),
-    "prefix-table-tma": dict(call="rx", src="f32", env={"FSK_B200_PREFIX": "1", "FSK_B200_PFX_FILL": "1"},
-                             kern=("k_rx", 3, 1), cls="tile", n=8),
-    "prefix-table-cp": dict(call="rx", src="f32", env={"FSK_B200_PREFIX": "1", "FSK_B200_PFX_FILL": "0"},
-                            kern=("k_rx", 3, 0), cls="tile", n=7),
-    "prefix-table-s16": dict(call="rx", src="s16", env={"FSK_B200_PREFIX": "1", "FSK_B200_PFX_FILL": "0"},
-                             kern=("k_rx", 3, 0), cls="tile", n=11),
-    "tones": dict(call="tones", src="f32", env={}, kern=("k_rx_tones", 0, 0)),
-    "tones-s16": dict(call="tones", src="s16", env={}, kern=("k_rx_tones", 0, 0)),
-    "auto": dict(call="auto", src="f32", env={}, kern=("k_rx_auto", 0, 0)),
-    "auto-s16": dict(call="auto", src="s16", env={}, kern=("k_rx_auto", 0, 0)),
-}
-PRESETS = [("1200", 48000), ("300", 48000), ("rtty", 8000), ("same", 48000)]
-# the presets a family cannot launch, with the reason
-NOT_LAUNCHED = {
-    ("shared-segment", "same"): "SAME's 10 windows have no shared-segment plan: the per-candidate kernel runs",
-    ("shared-segment-s16", "same"): "as the float rows",
-    ("tones", "same"): "SAME's shape (G=8, W=4, L=4) has no per-stream tone build (AUTO_COMBOS)",
-    ("tones-s16", "same"): "as the float rows",
-    ("auto", "same"): "as the tone call",
-    ("auto-s16", "same"): "as the tone call",
-}
-
-LK = re.compile(r"(k_rx|k_rx_auto|k_rx_tones)<G=(\d+),W=(\d+),L=(\d+),mode=(\d)\([a-z-]+\),fill=(\d),src=([a-z0-9,]+)> "
-                r"threads=(\d+) ring=(\d+) smem=(\d+) blocks=(\d+) lookahead=(\d+)$")
-
-
-def launch(eng):
-    """last_kernel() as a dict"""
-    s = eng.last_kernel()
-    m = LK.match(s)
-    assert m, s
-    k = dict(zip(("name", "G", "W", "L", "mode", "fill", "src", "threads", "ring", "smem", "blocks", "lookahead"),
-                 m.groups()))
-    for f in k:
-        if f not in ("name", "src"):
-            k[f] = int(k[f])
-    k["text"] = s
-    return k
+from gpudev import dev, pcm, state_rows, torch, upload
+from rxcases import shape_case as case
+from rxfam import (FAMILIES, NOT_LAUNCHED, PER_CAND, PRESETS, SHAPE_FAMILIES, SHARED, SMEM_MAX, call, check_family,
+                   compare_rx, launch, new_engine, set_env, skip_tma)
 
 
 def shape(k):
@@ -99,76 +45,6 @@ def max_advance(p):
     return max(p.try_max_nocarrier, p.try_max_carrier) - 1 + p.frame_nsamples
 
 
-def set_env(monkeypatch, env):
-    for k in KNOBS:
-        monkeypatch.delenv(k, raising=False)
-    for k, v in env.items():
-        monkeypatch.setenv(k, v)            # read when the engine is created
-
-
-# ---------------------------------------------------------------------------------------------------
-# cases: streams from the oracle's transmitter
-# ---------------------------------------------------------------------------------------------------
-_CASES = {}
-
-
-def _pcm(a):
-    return np.clip(np.round(a * 32768.0), -32768, 32767).astype(np.int16)
-
-
-def case(fam, which):
-    """(engine factory, streams, lengths, per-stream tone bands or None, oracle Mode) for a family and a
-    preset (mode, rate) or "random".  6 streams: ragged lead-ins, sigma = 0.01 noise (1e-4 for the auto
-    call, whose streams start with silence longer than the deepest ring), every third stream drops the
-    carrier and finds it again, the last one is cut mid-frame.  Computed once per (call, which)."""
-    f = FAMILIES[fam]
-    key = (f["call"], f.get("cls"), f.get("n"), which)
-    if key in _CASES:
-        return _CASES[key]
-    rng = np.random.default_rng(zlib.crc32(repr(key).encode()))
-    if which == "random":
-        mode, kw, exp = I.framing(f["cls"], f["n"], 7000 + f["n"])
-        m = I.oracle_mode(mode, kw, exp)
-        make = lambda: I.engine(mode, kw, exp)
-    else:
-        mode, rate = which
-        m = orc.Mode(mode, sample_rate=rate)
-        make = lambda: mm.RxEngine.for_mode(mode, rate)
-    spb = float(m.derived().nsamples_per_bit)
-    streams, bands = [], []
-    probe = make()
-    p = probe.params
-    nb = int(p.nbands)
-    for s in range(6):
-        if f["call"] == "auto":
-            import test_gpu_auto_carrier as AC
-            bs = autoorc.b_shift(m)
-            parts = [np.zeros(int(rng.integers(20000, 26000)), np.float32), AC.tone_stream(rng, m, bs, nb, 5)]
-            if s % 3 == 1:
-                parts += [np.zeros(int(rng.uniform(30, 50) * spb), np.float32), AC.tone_stream(rng, m, bs, nb, 4)]
-            sigma = 1e-4
-        else:
-            tm = m
-            if f["call"] == "tones":
-                import test_gpu_stream_tones as ST
-                fm, fs = ST.random_pair(rng, float(m.band_width), nb)
-                bands.append([int(v) for v in mm.tone_bands(p, fm, fs)])
-                tm = ST.on_pair(m.mode, m.sample_rate, fm, fs)
-                tm.__dict__.update({k: v for k, v in m.__dict__.items() if k not in ("mark_f", "space_f")})
-            words = lambda k: rng.integers(0, 1 << m.n_data_bits, k, dtype=np.uint64).astype(np.uint32)
-            parts = [np.zeros(int(rng.integers(0, 3 * spb + 1)), np.float32),
-                     orc.tx_words(tm, words(int(rng.integers(6, 10))), float(rng.uniform(0.3, 1.0)), 4096, True)]
-            if s % 3 == 1:
-                parts += [np.zeros(int(rng.uniform(20, 40) * spb), np.float32),
-                          orc.tx_words(tm, words(4), float(rng.uniform(0.3, 1.0)), 4096, True)]
-            sigma = 0.01
-        x = np.concatenate(parts)
-        if s == 5:
-            x = x[:int(x.size * rng.uniform(0.6, 0.9))]
-        x = (x + np.float32(sigma) * rng.standard_normal(x.size).astype(np.float32)).astype(np.float32)
-        streams.append(x)
-    _CASES[key] = (make, streams, np.array([x.size for x in streams], np.int32), bands or None, m)
-    return _CASES[key]
 
 
 class Run:
@@ -189,57 +65,15 @@ class Run:
 
 def run(eng, fam, c, max_frames=None, states=None, auto_states=None):
     make, streams, lens, bands, m = c
-    f = FAMILIES[fam]
-    t = I.torch()
-    n = int(lens.max())
-    buf = I._rows(streams, n, np.float32, 8)
-    if f["src"] == "s16":
-        buf = _pcm(buf)
-    x = t.from_numpy(buf).to(I.dev())
-    le = t.from_numpy(lens).to(I.dev())
+    if FAMILIES[fam]["src"] == "s16":
+        streams = [pcm(x) for x in streams]
+    r = call(eng, fam, streams, lens, bands=bands, max_frames=max_frames, states=states, auto_states=auto_states,
+             rec_band=True)
     extra = None
-    if f["call"] == "rx":
-        fr, st = eng.rx_batch(x, nsamples=n, nsamples_each=le, max_frames=max_frames, states=states)
-    elif f["call"] == "tones":
-        tb = t.from_numpy(np.array(bands, np.int32)).to(I.dev())
-        fr, st = eng.rx_batch_tones(x, tb, nsamples=n, nsamples_each=le, max_frames=max_frames, states=states)
-    else:
-        fr, st, ast, rb = eng.rx_batch_auto(x, nsamples=n, nsamples_each=le, max_frames=max_frames, states=states,
-                                            auto_states=auto_states, rec_band=True)
-    I.sync()
-    fr, sn = mm.frames_to_numpy(fr), mm.states_to_numpy(st)
-    recs = [fr[s, :int(sn["nframes"][s])].tobytes() for s in range(len(streams))]
-    if f["call"] == "auto":
-        rb = rb.cpu().numpy()
-        extra = (ast.cpu().numpy().tobytes(), [rb[s, :int(sn["nframes"][s])].tobytes() for s in range(len(streams))])
-        return Run(recs, sn.copy(), extra, launch(eng)), st, ast
-    return Run(recs, sn.copy(), extra, launch(eng)), st, None
-
-
-def new_engine(monkeypatch, fam, c, extra_env=None, tune=None):
-    f = FAMILIES[fam]
-    set_env(monkeypatch, dict(f["env"], **(extra_env or {})))
-    eng = c[0]()
-    if f["call"] == "auto":
-        eng.set_auto_carrier(autoorc.DEFAULT_THRESHOLD)
-    if tune:
-        eng.tune(**tune)
-    return eng
-
-
-def check_family(fam, k):
-    name, mode, fill = FAMILIES[fam]["kern"]
-    assert (k["name"], k["mode"], k["fill"]) == (name, mode, fill), (fam, k["text"])
-    assert k["src"].split(",")[0] == FAMILIES[fam]["src"], (fam, k["text"])
-    if fam == "per-candidate":
-        assert k["src"] == "f32,slide", k["text"]
-    if fam == "per-candidate-noslide":
-        assert k["src"] == "f32", k["text"]
-
-
-def skip_tma(fam):
-    if I.emulated() and FAMILIES[fam]["kern"][2] == 1:
-        pytest.skip("the host emulation does not model cp.async.bulk / mbarrier")
+    if r.auto is not None:
+        extra = (r.auto.cpu().numpy().tobytes(), [r.rec_band[s, :int(r.st["nframes"][s])].tobytes()
+                                                  for s in range(len(streams))])
+    return Run(r.recs, r.st, extra, r.k), r.states, r.auto
 
 
 def ring_for_full_lookahead(base, p):
@@ -273,7 +107,7 @@ def report(fam, k, nrecs):
 # ---------------------------------------------------------------------------------------------------
 # 1. ring depth at a pinned shape
 # ---------------------------------------------------------------------------------------------------
-FAM_KEYS = list(FAMILIES)
+FAM_KEYS = SHAPE_FAMILIES
 RING_ROWS = [(fam, w) for fam in FAM_KEYS for w in PRESETS + ["random"]
              if not (FAMILIES[fam]["call"] != "rx" and w == "random") and (fam, w[0]) not in NOT_LAUNCHED]
 
@@ -291,7 +125,7 @@ def test_ring_depth_does_not_change_the_records(fam, which, monkeypatch):
     byte for byte, and the launch shows the ring and the look-ahead asked for."""
     skip_tma(fam)
     c = case(fam, which)
-    eng = new_engine(monkeypatch, fam, c)
+    eng = new_engine(monkeypatch, fam, c[0])
     base, _, _ = run(eng, fam, c)
     k0 = base.k
     check_family(fam, k0)
@@ -302,7 +136,7 @@ def test_ring_depth_does_not_change_the_records(fam, which, monkeypatch):
     pin = dict(lanes_per_stream=k0["G"], warps_per_block=min(4, k0["threads"] // 32))
     env = {"FSK_B200_SPLIT": str(k0["L"])}
     if pin["warps_per_block"] != k0["threads"] // 32:
-        e1 = new_engine(monkeypatch, fam, c, env, pin)
+        e1 = new_engine(monkeypatch, fam, c[0], env, pin)
         got, _, _ = run(e1, fam, c)
         assert shape(got.k) == shape(k0) and got.k["threads"] == 128, got.k["text"]
         got.same_as(base, (fam, which, "4 warps"))
@@ -312,7 +146,7 @@ def test_ring_depth_does_not_change_the_records(fam, which, monkeypatch):
     rings = [k0["ring"] + 128, k0["ring"] + 256, r_full, deepest_ring(k0, 4 * r_full)]
     assert rings[-1] >= r_full + 128, (fam, which, rings, k0["text"])
     for ring in rings:
-        e2 = new_engine(monkeypatch, fam, c, env, dict(pin, ring_floats=ring))
+        e2 = new_engine(monkeypatch, fam, c[0], env, dict(pin, ring_floats=ring))
         got, _, _ = run(e2, fam, c)
         k = got.k
         assert shape(k) == shape(k0) and k["threads"] == k0["threads"], (fam, which, ring, k0["text"], k["text"])
@@ -334,13 +168,13 @@ def test_an_overflowing_call_resumed_on_another_ring_gives_one_pass(fam, monkeyp
     a different ring (and look-ahead), in calls of 3 records, and the records joined equal one pass."""
     skip_tma(fam)
     c = case(fam, ("300", 48000) if fam != "tones" else ("1200", 48000))
-    eng = new_engine(monkeypatch, fam, c)
+    eng = new_engine(monkeypatch, fam, c[0])
     one, _, _ = run(eng, fam, c)
     k0 = one.k
     p = eng.params
     env = {"FSK_B200_SPLIT": str(k0["L"])}
     pin = dict(lanes_per_stream=k0["G"], warps_per_block=min(4, k0["threads"] // 32))
-    engines = [eng, new_engine(monkeypatch, fam, c, env, dict(pin, ring_floats=ring_for_full_lookahead(k0, p)))]
+    engines = [eng, new_engine(monkeypatch, fam, c[0], env, dict(pin, ring_floats=ring_for_full_lookahead(k0, p)))]
     joined = [b""] * len(c[1])
     states = auto_states = None
     launches = set()
@@ -355,7 +189,7 @@ def test_an_overflowing_call_resumed_on_another_ring_gives_one_pass(fam, monkeyp
             break
         st = got.st.copy()
         st["nframes"][:] = 0            # the records of the next call start at its row's first slot
-        states = I.torch().from_numpy(st.view(np.int32).reshape(len(st), -1).copy()).to(I.dev())
+        states = state_rows(st)
     assert len(launches) == 2 and i >= 3, (launches, i)
     assert joined == one.recs, fam
     st = got.st.copy()
@@ -373,20 +207,19 @@ def test_an_overflowing_call_resumed_on_another_ring_gives_one_pass(fam, monkeyp
 def test_a_deep_ring_with_free_lanes_moves_g_and_keeps_the_oracle_records(which, env, monkeypatch):
     """lanes_per_stream left at 0: the launcher derives G from the streams that fit per SM, so a ring 2048
     floats deeper raises G -- the L-way combine then sums in another order, so the records are held to the
-    screened oracle (as test_gpu_instantiations.compare_rx does), not to the default run."""
+    screened oracle (as rxfam.compare_rx does), not to the default run."""
     fam = "per-candidate" if env is PER_CAND else "shared-segment"
     c = case(fam, which)
-    eng = new_engine(monkeypatch, fam, c)
+    eng = new_engine(monkeypatch, fam, c[0])
     base, _, _ = run(eng, fam, c)
-    e2 = new_engine(monkeypatch, fam, c, tune=dict(ring_floats=base.k["ring"] + 2048))
+    e2 = new_engine(monkeypatch, fam, c[0], tune=dict(ring_floats=base.k["ring"] + 2048))
     got, _, _ = run(e2, fam, c)
     k = got.k
     assert k["ring"] == base.k["ring"] + 2048 and k["mode"] == base.k["mode"], k["text"]
     assert k["G"] > base.k["G"], (base.k["text"], k["text"])
     make, streams, lens, _, m = c
     screened = [tie_screen.screen(m, x) for x in streams]
-    ocase = (m.mode, {}, None, m, streams, screened)
-    I.compare_rx(ocase, [np.frombuffer(r, mm.FRAME_DTYPE) for r in got.recs], got.st, k["text"])
+    compare_rx(screened, [np.frombuffer(r, mm.FRAME_DTYPE) for r in got.recs], got.st, k["text"])
     print("%s: %s -> %s; %d of %d streams held to the oracle's records" % (
         fam, base.k["text"], k["text"], sum(1 for _, r in screened if r), len(screened)))
 
@@ -406,7 +239,7 @@ def test_warps_per_block_do_not_change_the_records(fam, which, monkeypatch):
     FSK_B200_PREFIX=1, which its families set."""
     skip_tma(fam)
     c = case(fam, which)
-    eng = new_engine(monkeypatch, fam, c)
+    eng = new_engine(monkeypatch, fam, c[0])
     base, _, _ = run(eng, fam, c)
     k0 = base.k
     check_family(fam, k0)
@@ -415,7 +248,7 @@ def test_warps_per_block_do_not_change_the_records(fam, which, monkeypatch):
     rows = [dict(warps_per_block=w) for w in (1, 2, 3, 4)] + [dict(warps_per_block=3, ring_floats=r_full)]
     smem = {}
     for tv in rows:
-        e2 = new_engine(monkeypatch, fam, c, env, dict(tv, lanes_per_stream=k0["G"]))
+        e2 = new_engine(monkeypatch, fam, c[0], env, dict(tv, lanes_per_stream=k0["G"]))
         got, _, _ = run(e2, fam, c)
         k = got.k
         assert shape(k) == shape(k0), (fam, tv, k0["text"], k["text"])
@@ -469,16 +302,16 @@ def test_a_ring_too_large_for_one_stream_falls_back_to_the_generic_kernel(src, m
     screened oracle's records."""
     fam = "per-candidate" if src == "f32" else "per-candidate-s16"
     c = case(fam, ("1200", 48000))
-    eng = new_engine(monkeypatch, fam, c, tune=dict(ring_floats=SMEM_MAX // 4 + 128))
+    eng = new_engine(monkeypatch, fam, c[0], tune=dict(ring_floats=SMEM_MAX // 4 + 128))
     got, _, _ = run(eng, fam, c)
     k = got.k
     assert (k["mode"], k["G"], k["ring"], k["lookahead"]) == (1, 32, 0, 0), k["text"]
     assert "mode=1(generic)" in k["text"] and k["src"] == src, k["text"]
     make, streams, lens, _, m = c
     if src == "s16":
-        streams = [_pcm(x).astype(np.float32) / np.float32(32768.0) for x in streams]
+        streams = [pcm(x).astype(np.float32) / np.float32(32768.0) for x in streams]
     screened = [tie_screen.screen(m, x) for x in streams]
-    I.compare_rx((m.mode, {}, None, m, streams, screened), [np.frombuffer(r, mm.FRAME_DTYPE) for r in got.recs],
+    compare_rx(screened, [np.frombuffer(r, mm.FRAME_DTYPE) for r in got.recs],
                  got.st, k["text"])
 
 
@@ -489,9 +322,9 @@ def test_a_ring_that_leaves_no_room_for_the_sliding_table_drops_slide(monkeypatc
     differently, DESIGN.md 3, so the sliding run is not the reference)."""
     c = case("per-candidate", ("1200", 48000))
     pin = dict(lanes_per_stream=32, warps_per_block=1)
-    slide = new_engine(monkeypatch, "per-candidate", c, tune=pin)
+    slide = new_engine(monkeypatch, "per-candidate", c[0], tune=pin)
     a, _, _ = run(slide, "per-candidate", c)
-    flat = new_engine(monkeypatch, "per-candidate-noslide", c, tune=pin)
+    flat = new_engine(monkeypatch, "per-candidate-noslide", c[0], tune=pin)
     b, _, _ = run(flat, "per-candidate-noslide", c)
     assert a.k["src"] == "f32,slide" and b.k["src"] == "f32", (a.k["text"], b.k["text"])
     extra = a.k["smem"] - b.k["smem"]
@@ -501,9 +334,9 @@ def test_a_ring_that_leaves_no_room_for_the_sliding_table_drops_slide(monkeypatc
     blocks = (SMEM_MAX - extra - b.k["smem"]) // step + 1
     ring = b.k["ring"] + 128 * blocks
     assert b.k["smem"] + step * blocks <= SMEM_MAX < b.k["smem"] + step * blocks + extra
-    e1 = new_engine(monkeypatch, "per-candidate", c, tune=dict(pin, ring_floats=ring))
+    e1 = new_engine(monkeypatch, "per-candidate", c[0], tune=dict(pin, ring_floats=ring))
     got, _, _ = run(e1, "per-candidate", c)
-    e2 = new_engine(monkeypatch, "per-candidate-noslide", c, tune=dict(pin, ring_floats=ring))
+    e2 = new_engine(monkeypatch, "per-candidate-noslide", c[0], tune=dict(pin, ring_floats=ring))
     want, _, _ = run(e2, "per-candidate-noslide", c)
     assert got.k["src"] == "f32" and shape(got.k) == shape(b.k) and got.k["ring"] == ring, got.k["text"]
     assert want.k["text"] == got.k["text"]
@@ -547,7 +380,7 @@ def _nb_case(fam):
 
 def _batch(eng, fam, rows, max_frames):
     """rows: (samples, length or None for the whole stride, state) -> (records, states, sentinel left)"""
-    t = I.torch()
+    t = torch()
     n = max(max(r[0].size for r in rows), max(r[1] or 0 for r in rows))
     stride = (n + 7) & ~7
     buf = np.zeros((len(rows), stride), np.float32)
@@ -557,27 +390,11 @@ def _batch(eng, fam, rows, max_frames):
         buf[i, :x.size] = x
         lens[i] = stride if ln is None else ln
         st[i] = s0
-    x = t.from_numpy(buf).to(I.dev())
-    le = t.from_numpy(lens).to(I.dev())
-    states = t.from_numpy(st.view(np.int32).reshape(len(rows), -1).copy()).to(I.dev())
-    frames = t.full((len(rows), max_frames, 5), 0x5A5A5A5A, dtype=t.int32).to(I.dev())
-    call = FAMILIES[fam]["call"]
-    if call == "rx":
-        fr, so = eng.rx_batch(x, nsamples=stride, nsamples_each=le, max_frames=max_frames, frames=frames, states=states)
-    elif call == "tones":
-        tb = t.from_numpy(np.array([r[3] for r in rows], np.int64).astype(np.uint32).view(np.int32)).to(I.dev())
-        fr, so = eng.rx_batch_tones(x, tb, nsamples=stride, nsamples_each=le, max_frames=max_frames, frames=frames,
-                                    states=states)
-    else:
-        fr, so, _ = eng.rx_batch_auto(x, nsamples=stride, nsamples_each=le, max_frames=max_frames, frames=frames,
-                                      states=states)
-    I.sync()
-    raw = fr.cpu().numpy()
-    fr, so = mm.frames_to_numpy(fr), mm.states_to_numpy(so)
-    out = []
-    for i in range(len(rows)):
-        out.append((fr[i, :int(so["nframes"][i])].tobytes(), so[i].tobytes(), bool((raw[i] == 0x5A5A5A5A).all())))
-    return out, launch(eng)
+    frames = t.full((len(rows), max_frames, 5), 0x5A5A5A5A, dtype=t.int32).to(dev())
+    bands = [r[3] for r in rows] if FAMILIES[fam]["call"] == "tones" else None
+    r = call(eng, fam, upload(buf), lens, n=stride, bands=bands, states=st, max_frames=max_frames, frames=frames)
+    raw = r.fr.view(np.int32).reshape(len(rows), -1)
+    return [(r.recs[i], r.st[i].tobytes(), bool((raw[i] == 0x5A5A5A5A).all())) for i in range(len(rows))], r.k
 
 
 @pytest.mark.gpu
@@ -590,18 +407,7 @@ def test_a_streams_records_do_not_depend_on_its_place_or_its_neighbours(fam, G, 
     an invalid tone pair (tone call), silence as long as the batch (auto call).  Every row's records and
     state equal its lone run byte for byte; the done and invalid-pair rows come back untouched."""
     make, m, targets, nbrs = _nb_case(fam)
-    env = dict(FAMILIES[fam]["env"])
-
-    def engine():
-        set_env(monkeypatch, env)
-        e = make()
-        if FAMILIES[fam]["call"] == "auto":
-            e.set_auto_carrier(autoorc.DEFAULT_THRESHOLD)
-        if G:
-            e.tune(lanes_per_stream=G)
-        return e
-
-    eng = engine()
+    eng = new_engine(monkeypatch, fam, make, tune=dict(lanes_per_stream=G) if G else None)
     # the lone runs; max_frames: every target fits, the long neighbour does not
     mf = 1
     for x, ln, s0, bp in targets:
@@ -672,7 +478,7 @@ def test_tune_refuses_bad_values_and_keeps_the_previous_tuning(monkeypatch):
     a tune() between two calls on one engine takes effect at the next call."""
     fam = "per-candidate"
     c = case(fam, ("1200", 48000))
-    eng = new_engine(monkeypatch, fam, c)
+    eng = new_engine(monkeypatch, fam, c[0])
     base, _, _ = run(eng, fam, c)
     eng.tune(lanes_per_stream=16, warps_per_block=3, ring_floats=base.k["ring"] + 384)
     tuned, _, _ = run(eng, fam, c)

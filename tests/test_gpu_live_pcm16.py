@@ -24,17 +24,11 @@ import autoorc
 import golden_util as gu
 import orc
 import refcases
-import test_gpu_channels as TC
-import test_gpu_stream_lifetimes as SL
-import test_gpu_stream_tones as TT
+from gpudev import bands_tensor, dev, emulated, mm, pcm, state_rows, sync, torch, upload, widen
+from rxcases import ANSWER, ORIGINATE, TONE_PRESETS, call_audio, cuts, duplex_audio, random_states
 
 EINVAL, ENOTSUP = 22, 95
 OPEN, END, ENDED = 1, 2, 2
-mm, torch, dev, sync, t_ = TT.mm, TT.torch, TT.dev, TT.sync, TC.t_
-
-
-def widen(x):
-    return np.asarray(x, np.int16).astype(np.float32) * np.float32(1.0 / 32768.0)
 
 
 # --------------------------------------------------------------------------
@@ -43,8 +37,8 @@ def widen(x):
 @pytest.mark.parametrize("async_mode", ["eager", "late"])
 def test_live_pcm16_on_the_emulated_kernels(async_mode):
     """The `gpu` tests below on the host SIMT emulation of the kernels."""
-    import test_emu_parity
-    tail = test_emu_parity.run_emulated("gpu", async_mode, 3000, module="test_gpu_live_pcm16.py")
+    from gpudev import run_emulated
+    tail = run_emulated("gpu", async_mode, 3000, module="test_gpu_live_pcm16.py")
     assert " passed" in tail and "failed" not in tail
 
 
@@ -92,24 +86,24 @@ def test_int16_push_equals_the_float_push(k):
             for per_row in (True, False):
                 fill = rng.integers(0, stride + 1, nrows).astype(np.int32)
                 rows16 = rng.integers(-32768, 32768, (nrows, stride)).astype(np.int16)
-                st0 = TC.random_states(rng, nrows * k, fill, k)
+                st0 = random_states(rng, nrows * k, fill, k)
                 flag_some(rng, st0, nrows, k)
                 bands = None
                 if with_bands:
                     bands = rng.integers(0, nb, (nrows * k, 2)).astype(np.uint32)
                     off = rng.random(nrows * k) < 0.4
                     bands[off, int(rng.integers(2))] = nb
-                bt = TC.bands_tensor(bands) if bands is not None else None
+                bt = bands_tensor(bands) if bands is not None else None
                 chunk16 = rng.integers(-32768, 32768, (nrows, width)).astype(np.int16)
-                clen = t_(rng.integers(0, width + 1, nrows).astype(np.int32)) if per_row else int(rng.integers(0, width + 1))
+                clen = upload(rng.integers(0, width + 1, nrows).astype(np.int32)) if per_row else int(rng.integers(0, width + 1))
                 ev = None
                 if with_events:
-                    ev = t_(np.array([(r % 4) | (int(rng.integers(0, 64)) << 2) for r in range(nrows)], np.uint8))
+                    ev = upload(np.array([(r % 4) | (int(rng.integers(0, 64)) << 2) for r in range(nrows)], np.uint8))
                 out = {}
                 for name, rows, chunk in (("f32", widen(rows16), widen(chunk16)), ("s16", rows16, chunk16)):
-                    R, F, S = t_(rows), t_(fill), TT.state_rows(st0)
-                    D = t_(np.full(nrows, -1, np.int32))
-                    mm().stream_push(R, F, S, t_(chunk), clen, dropped=D, channels_per_row=k, tone_bands=bt,
+                    R, F, S = upload(rows), upload(fill), state_rows(st0)
+                    D = upload(np.full(nrows, -1, np.int32))
+                    mm().stream_push(R, F, S, upload(chunk), clen, dropped=D, channels_per_row=k, tone_bands=bt,
                                      nbands=nb, row_events=ev)
                     sync()
                     out[name] = R.cpu().numpy(), F.cpu().numpy(), S.cpu().numpy(), D.cpu().numpy()
@@ -186,7 +180,7 @@ def vector_pcm(name):
     if "audio_s16" in g.files:
         return case, g, g["audio_s16"]
     a = gu.audio(case, g)
-    x = TT.pcm(a)
+    x = pcm(a)
     assert widen(x).tobytes() == a.tobytes(), name
     return case, g, x
 
@@ -201,14 +195,14 @@ def overrides(case):
 def test_reference_vectors_in_random_cuts(name):
     """Each stream gets the vector's int16 audio in its own random cut, stream 1 a trickle; every stream's
     text adds up to the reference CLI's stdout byte for byte.  The --auto-carrier runs with auto_carrier=."""
-    if TT.emulated() and name in LONG:
+    if emulated() and name in LONG:
         pytest.skip("too long for the emulator")
     case, g, a = vector_pcm(name)
     rate = int(case["rx_mkw"].get("sample_rate", 48000))
     kw = overrides(case)
     if name.startswith("cli-auto-carrier"):
         kw["auto_carrier"] = autoorc.DEFAULT_THRESHOLD
-    nstreams, max_chunk = (3 if TT.emulated() else 4), 2048
+    nstreams, max_chunk = (3 if emulated() else 4), 2048
     lr = mm().LiveReceiver(case["rx_mode"], sample_rate=rate, nstreams=nstreams, max_chunk=max_chunk, device=dev(),
                            pcm16=True, **kw)
     assert lr.rows.dtype == torch().int16
@@ -229,7 +223,7 @@ def test_reference_vectors_in_random_cuts(name):
                 n = min(n, 333)
             chunk[i, :n] = a[fed[i]:fed[i] + n]
             clen[i], fed[i] = n, fed[i] + n
-        take(*lr.feed(t_(chunk), t_(clen)))
+        take(*lr.feed(upload(chunk), upload(clen)))
     take(*lr.finish())
     sync()
     assert int(lr.dropped.sum()) == 0
@@ -259,11 +253,11 @@ def twin_receivers(c, nrows, max_chunk):
         # per channel "o" originate, "a" answer, "x" disabled; one channel per row: the two rows alternate
         e0 = mm().RxEngine.for_mode(c["mode"], c["rate"])
         nb = int(e0.params.nbands)
-        pair = {"o": list(mm().tone_bands(e0.params, *TT.ORIGINATE)), "a": list(mm().tone_bands(e0.params, *TT.ANSWER)),
+        pair = {"o": list(mm().tone_bands(e0.params, *ORIGINATE)), "a": list(mm().tone_bands(e0.params, *ANSWER)),
                 "x": [nb, nb]}
         chans = c["chans"][:c["k"]] if c["k"] > 1 else "".join(c["chans"][r % 2] for r in range(nrows))
         bands = np.array([pair[ch] for ch in (chans * nrows if c["k"] > 1 else chans)], np.int32)
-        kw = dict(tones=t_(bands), channels_per_row=c["k"])
+        kw = dict(tones=upload(bands), channels_per_row=c["k"])
     if c.get("auto"):
         kw = dict(auto_carrier=autoorc.DEFAULT_THRESHOLD)
     return [mm().LiveReceiver(c["mode"], c["rate"], nrows, max_chunk=max_chunk, device=dev(), pcm16=p, **kw)
@@ -287,7 +281,7 @@ def test_pcm16_receiver_equals_the_float_receiver_feed_by_feed(name):
     noise after an end that is dropped)."""
     c = TWINS[name]
     rng = np.random.default_rng(zlib.crc32(name.encode()))
-    nrows = 4 if TT.emulated() else 48
+    nrows = 4 if emulated() else 48
     m = orc.Mode(c["mode"], sample_rate=c["rate"])
     max_chunk = 1500 if c["rate"] == 48000 else 500
     rf, rs = twin_receivers(c, nrows, max_chunk)
@@ -297,9 +291,9 @@ def test_pcm16_receiver_equals_the_float_receiver_feed_by_feed(name):
     for r in range(nrows):
         calls, tick = [], int(rng.integers(0, 3))
         for _ in range(2 if c.get("events") else 1):
-            x = SL.duplex_audio(rng, int(rng.integers(2, 4))) if "chans" in c else SL.call_audio(rng, m, int(rng.integers(2, 5)))
-            x = TT.pcm(x)
-            pieces = SL.cuts(rng, x.size, max_chunk)
+            x = duplex_audio(rng, int(rng.integers(2, 4))) if "chans" in c else call_audio(rng, m, int(rng.integers(2, 5)))
+            x = pcm(x)
+            pieces = cuts(rng, x.size, max_chunk)
             calls.append((tick, x, pieces))
             tick += len(pieces) + int(rng.integers(1, 4))
         sched.append(calls)
@@ -321,9 +315,9 @@ def test_pcm16_receiver_equals_the_float_receiver_feed_by_feed(name):
             if c.get("events") and not live and rng.random() < 0.3:
                 clen[r] = int(rng.integers(1, max_chunk + 1))
                 chunk[r, :clen[r]] = rng.integers(-3000, 3000, clen[r])
-        ev = dict(opened=t_(opened), ended=t_(ended)) if c.get("events") else {}
-        a = snapshot(rf, rf.feed(t_(widen(chunk)), t_(clen), **ev))
-        b = snapshot(rs, rs.feed(t_(chunk), t_(clen), **ev))
+        ev = dict(opened=upload(opened), ended=upload(ended)) if c.get("events") else {}
+        a = snapshot(rf, rf.feed(upload(widen(chunk)), upload(clen), **ev))
+        b = snapshot(rs, rs.feed(upload(chunk), upload(clen), **ev))
         assert a == b, (name, tick)
         ntext += sum(len(x) for x in b[0])
     assert "src=s16" in rs.engine.last_kernel() and "src=f32" in rf.engine.last_kernel()
@@ -357,7 +351,7 @@ def test_the_query_picks_the_row_type():
     t = torch()
     lr = mm().LiveReceiver("1200", 48000, 3, max_chunk=1000, device=dev(), pcm16=True)
     assert lr.engine.rx_batch_s16_runs(3) and lr.rows.dtype == t.int16 and lr.stride % 8 == 0
-    lr.feed(t_(np.zeros((3, 1000), np.int16)))
+    lr.feed(upload(np.zeros((3, 1000), np.int16)))
     sync()
     assert "src=s16" in lr.engine.last_kernel()
     c = NO_S16
@@ -366,7 +360,7 @@ def test_the_query_picks_the_row_type():
     assert not eng.rx_batch_s16_runs(3)
     rng = np.random.default_rng(24)
     m = orc.Mode(c["mode"], sample_rate=c["rate"], **over)
-    streams = [TT.pcm(SL.call_audio(rng, m, 4)) for _ in range(3)]
+    streams = [pcm(call_audio(rng, m, 4)) for _ in range(3)]
     max_chunk = 999
     rs, rf = [mm().LiveReceiver(c["mode"], c["rate"], 3, max_chunk=max_chunk, device=dev(), pcm16=p, **over)
               for p in (True, False)]
@@ -380,7 +374,7 @@ def test_the_query_picks_the_row_type():
         for i, a in enumerate(streams):
             n = min(w, a.size - fed[i])
             chunk[i, :n], clen[i], fed[i] = a[fed[i]:fed[i] + n], n, fed[i] + n
-        sa, sb = snapshot(rs, rs.feed(t_(chunk), t_(clen))), snapshot(rf, rf.feed(t_(widen(chunk)), t_(clen)))
+        sa, sb = snapshot(rs, rs.feed(upload(chunk), upload(clen))), snapshot(rf, rf.feed(upload(widen(chunk)), upload(clen)))
         assert sa == sb
         got = [g + x for g, x in zip(got, sa[0])]
         want = [g + x for g, x in zip(want, sb[0])]
@@ -399,7 +393,7 @@ def test_the_query_agrees_with_the_call_on_every_preset(rate):
     x = t.zeros((3, 2048), dtype=t.int16).to(dev())
     assert L.fsk_b200_rx_batch_s16_runs(None, 3) == -EINVAL
     seen = set()
-    for name in TT.PRESETS:
+    for name in TONE_PRESETS:
         try:
             eng = mm().RxEngine.for_mode(name, rate)
         except RuntimeError:                             # tones above this rate's Nyquist band ("12000" at 8 kHz)
@@ -432,13 +426,13 @@ def test_loopback_from_the_live_transmitter(mode, rate):
     LiveReceiver(pcm16=True), gives the transmitted text back."""
     import txorc
     t = torch()
-    n = 2 if TT.emulated() else 32
+    n = 2 if emulated() else 32
     rng = np.random.default_rng(zlib.crc32(mode.encode()))
     if mode == "callerid":
         g = gu.load("70-callerid-mdmf")
         texts, wants = [bytes(g["text"])] * n, [bytes(g["stdout"])] * n
     else:
-        texts = [bytes(int(v) for v in rng.integers(32, 127, 8 if TT.emulated() else int(rng.integers(10, 40))))
+        texts = [bytes(int(v) for v in rng.integers(32, 127, 8 if emulated() else int(rng.integers(10, 40))))
                  for _ in range(n)]
         wants = list(texts)
     tx = mm().LiveTransmitter(mode, rate, nstreams=n, max_text=max(len(x) for x in texts), idle=False, device=dev())
@@ -450,7 +444,7 @@ def test_loopback_from_the_live_transmitter(mode, rate):
     buf = np.zeros((n, max(len(x) for x in texts)), np.uint8)
     for i, x in enumerate(texts):
         buf[i, :len(x)] = np.frombuffer(x, np.uint8)
-    a1, c1 = tx.feed(t_(buf), t_(np.array([len(x) for x in texts], np.int32)))
+    a1, c1 = tx.feed(upload(buf), upload(np.array([len(x) for x in texts], np.int32)))
     a2, c2 = tx.finish()
     sync()
     assert a1.dtype == t.int16
@@ -466,7 +460,7 @@ def test_loopback_from_the_live_transmitter(mode, rate):
         for s, a in enumerate(audio):
             piece = a[o:o + max_chunk]
             chunk[s, :piece.size], clen[s] = piece, piece.size
-        text, cnt = snapshot(rx, rx.feed(t_(chunk), t_(clen)))[:2]
+        text, cnt = snapshot(rx, rx.feed(upload(chunk), upload(clen)))[:2]
         got = [g + x for g, x in zip(got, text)]
     got = [g + x for g, x in zip(got, snapshot(rx, rx.finish())[0])]
     for s in range(n):

@@ -27,10 +27,10 @@ import pytest
 import autoorc
 import minimodem_b200 as mm
 import orc
-import test_gpu_instantiations as I
-import test_gpu_launch_shapes as LS
-import test_gpu_parity as T
+import rxfam
 import tie_screen
+from gpudev import dev, emulated, pcm, sync, torch, upload
+from rxfam import as_oracle_frames, compare_frames, compare_reports, reports_of
 
 pytestmark = pytest.mark.gpu
 
@@ -106,9 +106,9 @@ class AliasedRows:
         self.hot = sorted(hot)
         self.body = next(i for i in range(nchunks) if i not in hot)
         self.physical = (1 + len(self.hot)) * CHUNK
-        self.emu = I.emulated()
+        self.emu = emulated()
         self._map(nchunks)
-        t = I.torch()
+        t = torch()
         nel = self.nbytes // self.es            # the rows and the guard behind them
         if self.emu:
             arr = np.ctypeslib.as_array(C.cast(self.base, C.POINTER(np.ctypeslib.as_ctypes_type(self.dtype))),
@@ -120,7 +120,7 @@ class AliasedRows:
             o = _Cai()
             o.__cuda_array_interface__ = dict(shape=(nel,), typestr=self.dtype.str, data=(self.base, False),
                                               strides=None, version=2)
-            self.flat = t.as_tensor(o, device=I.dev())
+            self.flat = t.as_tensor(o, device=dev())
         self.t = self.flat[:rows * STRIDE].view(rows, STRIDE)
         rng = np.random.default_rng(99 + self.es)
         for ci in [self.body] + self.hot:
@@ -147,8 +147,8 @@ class AliasedRows:
                 a = libc.mmap(base + ci * CHUNK, CHUNK, 0x1 | 0x2, 0x01 | 0x10, fd, 0)    # RW, SHARED|FIXED
                 assert a == base + ci * CHUNK, C.get_errno()
             return
-        t = I.torch()
-        t.zeros(1, device=I.dev())                      # the primary context, current on this thread
+        t = torch()
+        t.zeros(1, device=dev())                      # the primary context, current on this thread
         d = self.drv = _Driver()
         cu = d.cu
         prop = d.prop(d.device())
@@ -175,9 +175,9 @@ class AliasedRows:
              "cuMemSetAccess")
 
     def write(self, e0, a):
-        t = I.torch()
-        self.flat[e0:e0 + a.size] = t.from_numpy(np.ascontiguousarray(a)).to(I.dev())
-        I.sync()
+        t = torch()
+        self.flat[e0:e0 + a.size] = upload(np.ascontiguousarray(a))
+        sync()
 
     def read(self, e0, e1):
         return self.flat[e0:e1].cpu().numpy().copy()
@@ -192,7 +192,7 @@ class AliasedRows:
             for fd in self.fds.values():
                 os.close(fd)
             return
-        I.sync()
+        sync()
         cu = self.drv.cu
         for ci in self.mapped:
             self.drv.ok(cu.cuMemUnmap(C.c_uint64(self.base + ci * CHUNK), C.c_size_t(CHUNK)), "cuMemUnmap")
@@ -205,7 +205,7 @@ def loud(rng, n, dtype, rate=48000):
     """noise of sigma 0.4 plus a 0.4 tone at 1700 Hz (inside the Bell202 and Bell103 bands)"""
     x = 0.4 * rng.standard_normal(n) + 0.4 * np.sin(2 * np.pi * 1700.0 / rate * np.arange(n))
     x = x.astype(np.float32)
-    return LS._pcm(x) if np.dtype(dtype) == np.int16 else x
+    return pcm(x) if np.dtype(dtype) == np.int16 else x
 
 
 _ROWS = {}
@@ -215,9 +215,9 @@ _ROWS = {}
 def rows():
     """the aliased layouts, one per sample type, made on first use and unmapped at the end of the module"""
     info = {}
-    if not I.emulated():
-        I.torch().zeros(1, device=I.dev())             # the primary context, current on this thread
-        I.torch().cuda.empty_cache()
+    if not emulated():
+        torch().zeros(1, device=dev())             # the primary context, current on this thread
+        torch().cuda.empty_cache()
         info["before"] = _Driver().mem_info()[0]
 
     def get(dtype):
@@ -231,8 +231,8 @@ def rows():
         r.close()
     _ROWS.clear()
     assert phys <= 128 << 20, phys
-    if not I.emulated():
-        I.torch().cuda.empty_cache()
+    if not emulated():
+        torch().cuda.empty_cache()
         after = _Driver().mem_info()[0]
         print("long rows: %d MB physical; cuMemGetInfo free %d MB before, %d MB after"
               % (phys >> 20, info["before"] >> 20, after >> 20))
@@ -241,20 +241,14 @@ def rows():
 # ---------------------------------------------------------------------------------------------------
 # families and streams
 # ---------------------------------------------------------------------------------------------------
-CHANNELS = {"channels-2": 2, "channels-3": 3}
-GENERIC = {"generic": "f32", "generic-s16": "s16"}
-FAMS = list(LS.FAMILIES) + list(CHANNELS) + list(GENERIC)
-PRESET = {"prefix-table-tma": ("300", 48000), "prefix-table-cp": ("300", 48000), "prefix-table-s16": ("300", 48000)}
+FAMS = list(rxfam.FAMILIES)
 
 
-def fam_info(fam):
-    """(call, src, env, preset, number of words)"""
-    if fam in CHANNELS:
-        return "tones", "f32", {}, ("1200", 48000), 12
-    if fam in GENERIC:
-        return "rx", GENERIC[fam], {}, ("25", 48000), 3
-    f = LS.FAMILIES[fam]
-    return f["call"], f["src"], f["env"], PRESET.get(fam, ("1200", 48000)), 12
+def preset_of(fam):
+    """(preset, number of words) of a family's stream: the generic kernel's bit periods need 25 baud"""
+    if fam.startswith("generic"):
+        return ("25", 48000), 3
+    return (("300", 48000) if fam.startswith("prefix-table") else ("1200", 48000)), 12
 
 
 _STREAMS = {}
@@ -273,65 +267,27 @@ def stream(preset, nwords):
     return _STREAMS[key]
 
 
-def engine(monkeypatch, fam):
-    call, src, env, preset, _ = fam_info(fam)
-    LS.set_env(monkeypatch, env)
-    eng = mm.RxEngine.for_mode(*preset)
-    if call == "auto":
-        eng.set_auto_carrier(autoorc.DEFAULT_THRESHOLD)
-    return eng
-
-
-def check_launch(eng, fam):
-    s = eng.last_kernel()
-    if fam in GENERIC:
-        assert s.startswith("k_rx<") and "mode=1(" in s and ("src=s16" in s) == (GENERIC[fam] == "s16"), s
-        return
-    if fam in CHANNELS:
-        assert s.endswith(" channels=%d" % CHANNELS[fam]), s
-        s = s[:s.rindex(" channels=")]
-        assert s.startswith("k_rx_tones<"), s
-        return
-    m = LS.LK.match(s)
-    assert m, s
-
-    class _E:
-        def last_kernel(self):
-            return s
-    LS.check_family(fam, LS.launch(_E()))
-
-
 def decode(eng, fam, x, n, pos, nrows=1, row=0):
     """one call over the [nrows, stride] tensor x (row `row` starts at pos; the others are done) ->
-    (records of that row's stream(s) as bytes, states as numpy)"""
-    t = I.torch()
-    call = fam_info(fam)[0]
-    k = CHANNELS.get(fam, 1)
+    (records of that row's stream(s) as bytes, then the auto states of the row, and states as numpy)"""
+    f = rxfam.FAMILIES[fam]
+    k = f.get("k", 1)
     st = np.zeros(nrows * k, mm.STATE_DTYPE)
     st["done"] = 1
     st["pos"][row * k:(row + 1) * k] = pos
     st["done"][row * k:(row + 1) * k] = 0
-    states = t.from_numpy(st.view(np.int32).reshape(nrows * k, -1).copy()).to(I.dev())
-    mf = 96
-    if call == "rx":
-        fr, so = eng.rx_batch(x, nsamples=n, max_frames=mf, states=states)
-    elif call == "tones":
+    bands = None
+    if f["call"] == "tones":
         p = eng.params
-        pairs = [mm.tone_bands(p, 1200.0, 2200.0) if fam_info(fam)[3][0] == "1200" else mm.tone_bands(p, 1270.0, 1070.0)]
+        pairs = [mm.tone_bands(p, 1200.0, 2200.0) if preset_of(fam)[0][0] == "1200" else mm.tone_bands(p, 1270.0, 1070.0)]
         pairs += [mm.tone_bands(p, 1070.0, 1270.0), [p.nbands, p.nbands]][:k - 1]
-        tb = t.from_numpy(np.array(pairs * nrows, np.int32).reshape(nrows * k, 2)).to(I.dev())
-        fr, so = eng.rx_batch_tones(x, tb, nsamples=n, max_frames=mf, states=states, channels_per_row=k)
-    else:
-        fr, so, ast, rb = eng.rx_batch_auto(x, nsamples=n, max_frames=mf, states=states, rec_band=True)
-    I.sync()
-    check_launch(eng, fam)
-    fr, sn = mm.frames_to_numpy(fr), mm.states_to_numpy(so)
-    recs = [fr[c, :int(sn["nframes"][c])].tobytes() for c in range(row * k, (row + 1) * k)]
-    out = sn[row * k:(row + 1) * k].copy()
-    if call == "auto":
-        out_a = ast.cpu().numpy()[row].tobytes()
-        recs.append(out_a)
-    return recs, out
+        bands = np.array(pairs * nrows, np.int32).reshape(nrows * k, 2)
+    r = rxfam.call(eng, fam, x, n=n, bands=bands, states=st, max_frames=96, rec_band=True)
+    rxfam.check_family(fam, r.k)
+    recs = r.recs[row * k:(row + 1) * k]
+    if r.auto is not None:
+        recs.append(r.auto.cpu().numpy()[row].tobytes())
+    return recs, r.st[row * k:(row + 1) * k].copy()
 
 
 def placement(case, n, spb, xlen):
@@ -348,7 +304,7 @@ def small_twin(big, n, P, start, x, src):
     """the same samples in a small row at base p0 = start mod 128, loud noise after its own n; -> (tensor, n, p0)"""
     p0 = start % 128
     lead = big.read(start - p0, P)
-    body = x if src == "f32" else LS._pcm(x)
+    body = x if src == "f32" else pcm(x)
     seg = np.concatenate([lead, body]).astype(big.dtype)
     ns = p0 + (n - start)
     tail = loud(np.random.default_rng(5), 8192, big.dtype)
@@ -357,7 +313,7 @@ def small_twin(big, n, P, start, x, src):
     buf = np.zeros((1, stride), big.dtype)
     buf[0, :row.size] = row
     buf[0, row.size:] = tail[:stride - row.size]
-    return I.torch().from_numpy(buf).to(I.dev()), ns, p0
+    return upload(buf), ns, p0
 
 
 def check_equal(big_run, small_run, shift, what):
@@ -381,15 +337,16 @@ def first_diff(a, b):
 
 
 def run_case(rows, monkeypatch, fam, n, case, row=0):
-    call, src, env, preset, nwords = fam_info(fam)
+    src = rxfam.FAMILIES[fam]["src"]
+    preset, nwords = preset_of(fam)
     m, x = stream(preset, nwords)
     spb = float(m.derived().nsamples_per_bit)
     big = rows(np.float32 if src == "f32" else np.int16)
     P, start = placement(case, n, spb, x.size)
     e0 = row * STRIDE
     assert big.is_hot(e0 + start - 128, e0 + P + x.size + 1), (n, case)
-    big.write(e0 + P, x if src == "f32" else LS._pcm(x))
-    eng = engine(monkeypatch, fam)
+    big.write(e0 + P, x if src == "f32" else pcm(x))
+    eng = rxfam.new_engine(monkeypatch, fam, lambda: mm.RxEngine.for_mode(*preset))
     nrows = 2 if row else 1
     got = decode(eng, fam, big.t[:nrows], n, start, nrows=nrows, row=row)
     xs, ns, p0 = small_twin(big, e0 + n, e0 + P, e0 + start, x, src)
@@ -398,7 +355,7 @@ def run_case(rows, monkeypatch, fam, n, case, row=0):
     check_equal(got, want, start - p0, what)
     st = want[1]
     assert (st["done"][:2] == 1).all(), what          # (channels-3: the third channel is disabled)
-    if case == "at-start" and fam not in GENERIC:
+    if case == "at-start" and not fam.startswith("generic"):
         assert st["nframes"][0] >= nwords - 1, (what, st["nframes"])
     return want, xs, ns, p0, m
 
@@ -411,16 +368,14 @@ def run_case(rows, monkeypatch, fam, n, case, row=0):
 @pytest.mark.parametrize("fam", FAMS)
 def test_stream_at_the_end_of_a_long_row(rows, monkeypatch, fam, nid, n, case):
     """A stream at the end of a row of n samples decodes as at the start of a small row."""
-    if fam in LS.FAMILIES:
-        LS.skip_tma(fam)
+    rxfam.skip_tma(fam)
     run_case(rows, monkeypatch, fam, n, case)
 
 
 @pytest.mark.parametrize("fam", FAMS)
 def test_second_row_beyond_2_32_elements(rows, monkeypatch, fam):
     """Row 1 of two rows of 2^32 samples starts at element 2^32: the row offsets are size_t."""
-    if fam in LS.FAMILIES:
-        LS.skip_tma(fam)
+    rxfam.skip_tma(fam)
     run_case(rows, monkeypatch, fam, MAX_ROW, "at-start", row=1)
 
 
@@ -432,8 +387,8 @@ def test_small_row_is_the_oracles(rows, monkeypatch):
     want, robust = tie_screen.screen(m, seg)
     assert robust
     got = np.frombuffer(recs[0], mm.FRAME_DTYPE)
-    T.compare_frames(T.as_oracle_frames(got), want["frames"], "small twin")
-    T.compare_reports(T.reports_of(got, st[0]), want["reports"], "small twin")
+    compare_frames(as_oracle_frames(got), want["frames"], "small twin")
+    compare_reports(reports_of(got, st[0]), want["reports"], "small twin")
 
 
 @pytest.mark.parametrize("nid,n", [ROW_LENGTHS[0], ROW_LENGTHS[-3]], ids=[ROW_LENGTHS[0][0], ROW_LENGTHS[-3][0]])
@@ -441,7 +396,7 @@ def test_find_frame_and_detect_carrier_near_2_32(rows, nid, n):
     """fsk_b200_find_frame_batch with offset[s] and nvalid[s] near 2^32 (the search window running past
     nvalid), and fsk_b200_detect_carrier_batch with offset[s] near 2^32, against the same samples in a
     small row."""
-    t = I.torch()
+    t = torch()
     m, x = stream(("1200", 48000), 12)
     big = rows(np.float32)
     P = n - x.size
@@ -454,14 +409,14 @@ def test_find_frame_and_detect_carrier_near_2_32(rows, nid, n):
 
     def ff(buf, base, nvalid):
         k = offs.size
-        u = lambda a: t.from_numpy(np.asarray(a, np.uint32).view(np.int32)).to(I.dev())
+        u = lambda a: upload(np.asarray(a, np.uint32).view(np.int32))
         o = u(offs - base)
         fr = []
         for i in range(k):
             f = eng.find_frame_batch(buf, u([nvalid]), u([0]), u([p.try_max_nocarrier]), u([max(1, p.try_max_nocarrier // 3)]),
-                                     t.from_numpy(np.array([np.inf], np.float32)).to(I.dev()),
-                                     offset=o[i:i + 1], expect_sel=t.from_numpy(np.array([1], np.uint8)).to(I.dev()))
-            I.sync()
+                                     upload(np.array([np.inf], np.float32)),
+                                     offset=o[i:i + 1], expect_sel=upload(np.array([1], np.uint8)))
+            sync()
             assert eng.last_kernel().startswith("k_find_frame"), eng.last_kernel()
             fr.append(f.cpu().numpy().tobytes())
         return fr
@@ -471,8 +426,8 @@ def test_find_frame_and_detect_carrier_near_2_32(rows, nid, n):
     assert any(np.frombuffer(r, mm.FRAME_DTYPE)["confidence"][0] > 0 for r in a)
     fft = int(p.fftsize)
     for off in (P + 100, n - fft):
-        o1 = t.from_numpy(np.array([off], np.uint32).view(np.int32)).to(I.dev())
-        o2 = t.from_numpy(np.array([off - (P - p0)], np.uint32).view(np.int32)).to(I.dev())
+        o1 = upload(np.array([off], np.uint32).view(np.int32))
+        o2 = upload(np.array([off - (P - p0)], np.uint32).view(np.int32))
         g = mm.detect_carrier_batch(fft, big.t[:1], fft, 0.001, offset=o1).cpu().numpy()
         w = mm.detect_carrier_batch(fft, xs, fft, 0.001, offset=o2).cpu().numpy()
         assert (g == w).all() and int(w[0]) > 0, (off, g, w)
@@ -480,16 +435,16 @@ def test_find_frame_and_detect_carrier_near_2_32(rows, nid, n):
 
 def test_rx_calls_refuse_rows_above_the_limit():
     """nsamples_all > 2^32 - 4 returns -EINVAL in every rx call and launches nothing; 2^32 - 4 is taken."""
-    t = I.torch()
+    t = torch()
     eng = mm.RxEngine.for_mode("1200", 48000)
     lib = mm.api.lib()
-    x = t.zeros((1, 64), dtype=t.float32, device=I.dev())
-    x16 = t.zeros((1, 64), dtype=t.int16, device=I.dev())
-    fr = t.zeros((1, 4, 5), dtype=t.int32, device=I.dev())
-    st = t.zeros((1, mm.STATE_WORDS), dtype=t.int32, device=I.dev())
-    ast = t.zeros((1, mm.api.AUTO_STATE_BYTES), dtype=t.uint8, device=I.dev())
-    each = t.from_numpy(np.array([64], np.int32)).to(I.dev())
-    tb = eng.tone_bands(1200.0, 2200.0, device=I.dev())
+    x = t.zeros((1, 64), dtype=t.float32, device=dev())
+    x16 = t.zeros((1, 64), dtype=t.int16, device=dev())
+    fr = t.zeros((1, 4, 5), dtype=t.int32, device=dev())
+    st = t.zeros((1, mm.STATE_WORDS), dtype=t.int32, device=dev())
+    ast = t.zeros((1, mm.api.AUTO_STATE_BYTES), dtype=t.uint8, device=dev())
+    each = upload(np.array([64], np.int32))
+    tb = eng.tone_bands(1200.0, 2200.0, device=dev())
     eng.set_auto_carrier(autoorc.DEFAULT_THRESHOLD)
     P = mm.api._ptr
     h = mm.api._stream_handle()
@@ -517,7 +472,7 @@ def test_rx_calls_refuse_rows_above_the_limit():
             assert "2^32 - 4" in mm.api.lib().fsk_b200_last_error().decode(), name
         before = mm.launch_count()
         assert call(MAX_ROW) == 0, name         # per-row lengths (64) bound the rows
-        I.sync()
+        sync()
         assert mm.launch_count() > before, name
     hf = np.zeros((1, 4), mm.FRAME_DTYPE)
     hs = np.zeros(1, mm.STATE_DTYPE)
@@ -533,16 +488,16 @@ def test_rx_calls_refuse_rows_above_the_limit():
 def test_stream_push_caps_a_row_at_the_limit(rows, start):
     """The live push with pos = 0 (no tail move) and a row `start` samples short of 2^32 - 4: what fits
     below the limit is appended, the rest counted in `dropped`, and nothing at or past 2^32 - 4 changes."""
-    t = I.torch()
+    t = torch()
     big = rows(np.float32)
     have = MAX_ROW - start
     before = big.read(have - 64, MAX_ROW + 64)
     chunk = np.arange(1, 33, dtype=np.float32)[None, :] * np.float32(0.25)
-    fill = t.from_numpy(np.array([have], np.uint32).view(np.int32)).to(I.dev())
-    dropped = t.zeros(1, dtype=t.int32, device=I.dev())
-    st = t.zeros((1, mm.STATE_WORDS), dtype=t.int32, device=I.dev())
-    mm.stream_push(big.t[:1], fill, st, t.from_numpy(chunk).to(I.dev()), dropped=dropped)
-    I.sync()
+    fill = upload(np.array([have], np.uint32).view(np.int32))
+    dropped = t.zeros(1, dtype=t.int32, device=dev())
+    st = t.zeros((1, mm.STATE_WORDS), dtype=t.int32, device=dev())
+    mm.stream_push(big.t[:1], fill, st, upload(chunk), dropped=dropped)
+    sync()
     f = int(fill.cpu().numpy().view(np.uint32)[0])
     d = int(dropped.cpu().numpy()[0])
     assert (f, d) == (MAX_ROW, 32 - start), (f, d)
@@ -557,7 +512,7 @@ def test_stream_push_caps_a_row_at_the_limit(rows, start):
 
 def test_no_mapping_is_left_behind():
     """A layout made and unmapped returns its memory: the reserved range is gone and free memory is back."""
-    if I.emulated():
+    if emulated():
         r = AliasedRows(np.int16, rows=1)
         base, nb = r.base, r.nbytes
         r.close()
@@ -566,10 +521,10 @@ def test_no_mapping_is_left_behind():
                 lo, hi = (int(v, 16) for v in line.split()[0].split("-"))
                 assert hi <= base or lo >= base + nb, line
         return
-    t = I.torch()
+    t = torch()
     t.cuda.empty_cache()
     drv = _Driver()
-    t.zeros(1, device=I.dev())
+    t.zeros(1, device=dev())
     free0 = drv.mem_info()[0]
     r = AliasedRows(np.int16, rows=1)
     t.cuda.empty_cache()
@@ -592,20 +547,20 @@ def test_no_mapping_is_left_behind():
 def test_tx_channel_lead_in_near_2_32():
     """A channel whose lead-in alone passes a small nsamples_out adds nothing to its row; out_len is the
     lead-in plus the signal, saturated at 2^32 - 1."""
-    t = I.torch()
+    t = torch()
     eng = mm.TxEngine.for_mode("1200", 48000, float_samples=True)
-    text = t.from_numpy(np.frombuffer(b"HELLO 2^32", np.uint8).reshape(1, -1).repeat(3, 0).copy()).to(I.dev())
-    lens = t.from_numpy(np.array([10, 10, 10], np.int32)).to(I.dev())
-    tones = eng.tone_pairs([1200.0, 1070.0, 2025.0], [2200.0, 1270.0, 2225.0], device=I.dev())
+    text = upload(np.frombuffer(b"HELLO 2^32", np.uint8).reshape(1, -1).repeat(3, 0).copy())
+    lens = upload(np.array([10, 10, 10], np.int32))
+    tones = eng.tone_pairs([1200.0, 1070.0, 2025.0], [2200.0, 1270.0, 2225.0], device=dev())
     leads = np.array([0, TOP - 1, TOP - 4000], np.uint32)
-    lead = t.from_numpy(leads.view(np.int32)).to(I.dev())
-    out = t.full((1, 4096), 7.0, dtype=t.float32, device=I.dev())
+    lead = upload(leads.view(np.int32))
+    out = t.full((1, 4096), 7.0, dtype=t.float32, device=dev())
     r = eng.text_channels(text, lens, tones, 3, 4000, lead_in=lead, out=out)
     o, out_len = r[0], r[1]
-    I.sync()
-    ref = t.full((1, 4096), 7.0, dtype=t.float32, device=I.dev())
+    sync()
+    ref = t.full((1, 4096), 7.0, dtype=t.float32, device=dev())
     r1 = eng.text_channels(text[:1], lens[:1], tones[:1], 1, 4000, lead_in=lead[:1], out=ref)
-    I.sync()
+    sync()
     assert o.cpu().numpy().tobytes() == r1[0].cpu().numpy().tobytes()
     ol = out_len.cpu().numpy().view(np.uint32)
     sig = int(r1[1].cpu().numpy().view(np.uint32)[0])
@@ -615,7 +570,7 @@ def test_tx_channel_lead_in_near_2_32():
 
 def test_tx_channels_length_bound_at_2_32():
     """The longest channel a text_stride allows plus nsamples_out may reach 2^32 - 1 samples, not 2^32."""
-    t = I.torch()
+    t = torch()
     eng = mm.TxEngine.for_mode("1200", 48000, float_samples=True)
     need = lambda S: mm.tx_max_samples(eng, S, mm.api.TX_FINAL)
     lo, hi = 1, 1 << 24                     # the largest text_stride whose channel fits below 2^32 - 1 - 64
@@ -625,12 +580,12 @@ def test_tx_channels_length_bound_at_2_32():
     S = lo
     nout = TOP - 1 - need(S)
     assert 64 <= nout < 4096, (S, need(S))
-    text = t.zeros((1, S), dtype=t.uint8, device=I.dev())
+    text = t.zeros((1, S), dtype=t.uint8, device=dev())
     text[0, 0] = ord("A")
-    lens = t.from_numpy(np.array([1], np.int32)).to(I.dev())
-    tones = eng.tone_pairs([1200.0], [2200.0], device=I.dev())
-    out = t.zeros((1, 4096), dtype=t.float32, device=I.dev())
-    out_len = t.zeros(1, dtype=t.int32, device=I.dev())
+    lens = upload(np.array([1], np.int32))
+    tones = eng.tone_pairs([1200.0], [2200.0], device=dev())
+    out = t.zeros((1, 4096), dtype=t.float32, device=dev())
+    out_len = t.zeros(1, dtype=t.int32, device=dev())
     lib, P = mm.api.lib(), mm.api._ptr
     call = lambda n: lib.fsk_b200_tx_text_channels(eng._te, P(text), 1, 1, S, P(lens), P(tones), None, P(out), 4096,
                                                    n, P(out_len), mm.api._stream_handle())
@@ -638,6 +593,6 @@ def test_tx_channels_length_bound_at_2_32():
     assert call(nout + 1) == -22
     assert mm.launch_count() == before
     assert call(nout) == 0
-    I.sync()
+    sync()
     assert mm.launch_count() > before
     assert int(out_len.cpu().numpy()[0]) > 0 and bool((out.cpu().numpy()[0, :64] != 0).any())

@@ -16,105 +16,15 @@ import golden_util as gu
 import minimodem_b200 as mm
 import orc
 import refcases
+import rxcases
+from clicases import emulation_as_product, write_wav
+from gpudev import dev, upload
+from rxcases import engine_for, pad4, rx_on_gpu
+from rxfam import as_oracle_frames, compare_frames, compare_reports, reports_of
 
 pytestmark = pytest.mark.gpu
 
 torch = pytest.importorskip("torch")
-
-
-def dev():
-    import conftest
-    if conftest.EMU_DEVICE is not None:		# FSK_B200_EMU=1: the kernels' source on the host emulator
-        return conftest.EMU_DEVICE
-    assert torch.cuda.is_available(), "GPU tests need a CUDA device"
-    return torch.device("cuda:0")
-
-
-def engine_for(case_or_mode, rx=True):
-    if isinstance(case_or_mode, dict):
-        mode, kw = case_or_mode["rx_mode"], case_or_mode["rx_mkw"]
-    else:
-        mode, kw = case_or_mode
-    names = dict(mark="f_mark", space="f_space", bandwidth="band_width", startbits="nstartbits",
-                 stopbits="nstopbits", confidence="confidence_threshold", limit="confidence_search_limit")
-    ov = {names.get(k, k): v for k, v in kw.items() if k not in ("sample_rate", "baudot")}
-    if kw.get("baudot"):            # the -5 option
-        ov["n_data_bits"] = 5
-    cfg = mm.rx_config_for_mode(mode, kw.get("sample_rate", 48000), **ov)
-    return mm.RxEngine(mm.rx_params(cfg)), cfg
-
-
-def pad4(n):
-    return (n + 3) & ~3
-
-
-def rx_on_gpu(eng, streams, lanes=0):
-    """streams: list of 1-D float32 arrays -> list of frame-record arrays."""
-    n = max(len(a) for a in streams)
-    stride = pad4(n)
-    buf = np.zeros((len(streams), stride), np.float32)
-    lens = np.zeros(len(streams), np.int32)
-    for i, a in enumerate(streams):
-        buf[i, :len(a)] = a
-        lens[i] = len(a)
-    if lanes:
-        eng.tune(lanes_per_stream=lanes)
-    d = torch.from_numpy(buf).to(dev())
-    frames, states = eng.rx_batch(d, nsamples=n, nsamples_each=torch.from_numpy(lens).to(dev()))
-    torch.cuda.synchronize()
-    fr = mm.frames_to_numpy(frames)
-    st = mm.states_to_numpy(states)
-    assert (st["done"] == 1).all()
-    return [fr[i, :st["nframes"][i]] for i in range(len(streams))], st
-
-
-def as_oracle_frames(recs):
-    out = []
-    for r in recs:
-        fs = int(r["frame_start"])
-        if fs == mm.FRAME_REPORT:
-            continue
-        bits = int(r["bits_lo"]) | (int(r["bits_hi"]) << 32)
-        out.append((bits, np.float32(r["confidence"]), np.float32(r["amplitude"]), fs & 0x7FFFFFFF,
-                    1 if fs & mm.FRAME_ACQUIRED else 0, 0))
-    return out
-
-
-def reports_of(recs, st_row):
-    """Carrier-session statistics exactly as the device accumulated them: the REPORT
-    records (carrier drops, src/minimodem.c:1298-1307) plus the session still open at
-    the end of the stream (:1469-1474), which lives in the stream state."""
-    reps, count, nfr = [], 0, 0
-    for r in recs:
-        fs = int(r["frame_start"])
-        if fs == mm.FRAME_REPORT:
-            reps.append((count, int(r["bits_lo"]) | (int(r["bits_hi"]) << 32), np.float32(r["confidence"]),
-                         np.float32(r["amplitude"]), nfr))
-            count = 0
-        else:
-            count = 1 if fs & mm.FRAME_ACQUIRED else count + 1
-            nfr += 1
-    if st_row["carrier"]:
-        assert int(st_row["nframes_decoded"]) == count
-        reps.append((count, int(st_row["carrier_nsamples"]), np.float32(st_row["confidence_total"]),
-                     np.float32(st_row["amplitude_total"]), nfr))
-    return reps
-
-
-def compare_reports(got, want, what=""):
-    assert len(got) == len(want), (what, got, want)
-    for a, b in zip(got, want):
-        assert a[0] == b[0] and a[1] == b[1] and a[4] == b[4], (what, a, b)
-        assert gu.close(a[2], b[2], cond=gu.CONF_COND) and gu.close(a[3], b[3]), (what, a, b)
-
-
-def compare_frames(got, want, what=""):
-    assert len(got) == len(want), (what, len(got), len(want))
-    for i, (a, b) in enumerate(zip(got, want)):
-        assert a[0] == b[0], (what, i, hex(a[0]), hex(b[0]))
-        assert a[3] == b[3] and a[4] == b[4], (what, i, a, b)
-        assert gu.close(a[1], b[1], cond=gu.CONF_COND), (what, i, a[1], b[1])
-        assert gu.close(a[2], b[2]), (what, i, a[2], b[2])
 
 
 # --------------------------------------------------------------------------
@@ -125,37 +35,7 @@ RX_CASES = [c for c in refcases.EVERY]
 
 @pytest.mark.parametrize("case", RX_CASES, ids=[c["name"] for c in RX_CASES])
 def test_rx_batch_on_reference_vectors(case):
-    g = gu.load(case["name"])
-    _, rx = gu.modes(case)
-    a = gu.audio(case, g)
-    if case["rxnoise"]:
-        a = (a + np.float32(-0.5) * np.float32(np.float32(case["rxnoise"]) * 2)).astype(np.float32)
-    eng, cfg = engine_for(case)
-    want = orc.rx_run(rx, a, literal=False, rx_one=False)
-    (recs,), st = rx_on_gpu(eng, [a])
-    got = as_oracle_frames(recs)
-    compare_frames(got, want["frames"], case["name"])
-    if orc.have_ref():
-        # byte-identical decode, the reference's own pass criterion (tests/self-test: cmp)
-        frames = got
-        if case["rx_one"]:          # --rx-one: stop at the first carrier drop (:1310)
-            nacq = [i for i, f in enumerate(frames) if f[4]]
-            if len(nacq) > 1:
-                frames = frames[:nacq[1]]
-        assert orc.ref_decode(rx, frames, decoder=refcases.decoder_of(case, rx)) == bytes(g["stdout"])
-    # stat line (the -P tests grep it for "confidence=inf ... (rate perfect)")
-    reps = reports_of(recs, st[0])
-    compare_reports(reps, want["reports"], case["name"])
-    lines = [orc.report_line(rx, r) for r in reps]
-    wantl = gu.stat_lines(g)
-    if case["rx_one"]:
-        lines = lines[:1]
-    assert len(lines) >= len(wantl) >= 1
-    fa, fb = lines[0].split(), wantl[0].split()
-    assert fa[:3] == fb[:3] and fa[4:] == fb[4:], (lines[0], wantl[0])
-    assert gu.close(float(fa[3].split("=")[1]), float(fb[3].split("=")[1]), 2e-3, cond=gu.CONF_COND)
-    if case["perfect"]:
-        assert "confidence=inf" in lines[0] and "(rate perfect)" in lines[0]
+    rxcases.check_reference_vector(case)
 
 
 @pytest.mark.parametrize("lanes", [4, 8, 16, 32])
@@ -205,7 +85,7 @@ def test_find_frame_batch_noisy(mode, kw):
                    max(tmax // (8 if fine else 3), 1), 0)
         limit[s] = np.inf if fine else 2.3
         sel[s] = 0 if carrier else 1
-    t = lambda a, dt: torch.from_numpy(np.ascontiguousarray(a.astype(dt))).to(dev())
+    t = lambda a, dt: upload(np.ascontiguousarray(a.astype(dt)))
     frames = eng.find_frame_batch(t(buf, np.float32), t(args[:, 0], np.int32), t(args[:, 1], np.int32),
                                   t(args[:, 2], np.int32), t(args[:, 3], np.int32), t(limit, np.float32),
                                   expect_sel=t(sel, np.uint8))
@@ -305,8 +185,8 @@ def test_detect_carrier_batch(rate, bw, n):
         if s % 9 == 0:
             y = 0.0 * y                                   # silence: no band reaches the threshold
         x[s, off[s]:off[s] + n] = y.astype(np.float32)
-    d = torch.from_numpy(x).to(dev())
-    got = mm.detect_carrier_batch(fftsize, d, n, 0.05, offset=torch.from_numpy(off).to(dev()))
+    d = upload(x)
+    got = mm.detect_carrier_batch(fftsize, d, n, 0.05, offset=upload(off))
     torch.cuda.synchronize()
     got = got.cpu().numpy()
     want_fn = None
@@ -351,8 +231,8 @@ def test_tx_batch_bit_exact(mode, kw):
     tcfg = mm.tx_config_from(cfg)
     ref0 = orc.tx_words(m, words[0], 1.0, 4096, True)
     nout = ref0.size + 260
-    out = mm.tx_batch(tcfg, torch.from_numpy(words.astype(np.int32)).to(dev()), nout,
-                      lead_in=torch.from_numpy(lead.astype(np.int32)).to(dev()))
+    out = mm.tx_batch(tcfg, upload(words.astype(np.int32)), nout,
+                      lead_in=upload(lead.astype(np.int32)))
     torch.cuda.synchronize()
     o = out.cpu().numpy()
     for s in range(nstreams):
@@ -511,8 +391,8 @@ def test_rx_batch_output_overflow_and_resume():
     buf = np.zeros((len(xs), pad4(n)), np.float32)
     for i, a in enumerate(xs):
         buf[i, :len(a)] = a
-    d = torch.from_numpy(buf).to(dev())
-    lens = torch.from_numpy(np.array([len(a) for a in xs], np.int32)).to(dev())
+    d = upload(buf)
+    lens = upload(np.array([len(a) for a in xs], np.int32))
     full, st_full = eng.rx_batch(d, nsamples=n, nsamples_each=lens)
     small, st = eng.rx_batch(d, nsamples=n, nsamples_each=lens, max_frames=10)
     torch.cuda.synchronize()
@@ -578,7 +458,7 @@ def test_s16_ingest_and_device_ascii_decode(name):
     k = int(st_f["nframes"][0])
     assert k > 0 and np.array_equal(fr_f[:, :k], fr_s[:, :k])
     # device conversion kernel on its own
-    d = mm.s16_to_f32(torch.from_numpy(hs).to(dev()))
+    d = mm.s16_to_f32(upload(hs))
     torch.cuda.synchronize()
     assert np.array_equal(d.cpu().numpy(), hf)
     # device decode of the device-resident records
@@ -658,8 +538,8 @@ def test_decode_batch_every_decoder(kind):
     rec, nfr = _synthetic_records(kind, rx, rng, nstreams, max_frames)
     st = np.zeros(nstreams, mm.STATE_DTYPE)
     st["nframes"] = nfr
-    d_rec = torch.from_numpy(rec.view(np.int32)).to(dev())
-    d_st = torch.from_numpy(st.view(np.int32).reshape(nstreams, -1)).to(dev())
+    d_rec = upload(rec.view(np.int32))
+    d_st = upload(st.view(np.int32).reshape(nstreams, -1))
     out, cnt = eng.decode_batch(k, d_rec, d_st)
     torch.cuda.synchronize()
     o, c = out.cpu().numpy(), cnt.cpu().numpy()
@@ -690,9 +570,9 @@ def test_decode_batch_every_decoder(kind):
     st2["nframes"] = nfr - st1["nframes"]
     rec2 = np.zeros_like(rec)
     rec2[:, :max_frames - half] = rec[:, half:]
-    o1, c1 = eng.decode_batch(k, d_rec, torch.from_numpy(st1.view(np.int32).reshape(nstreams, -1)).to(dev()), dstates=dst)
-    o2, c2 = eng.decode_batch(k, torch.from_numpy(rec2.view(np.int32)).to(dev()),
-                              torch.from_numpy(st2.view(np.int32).reshape(nstreams, -1)).to(dev()), dstates=dst)
+    o1, c1 = eng.decode_batch(k, d_rec, upload(st1.view(np.int32).reshape(nstreams, -1)), dstates=dst)
+    o2, c2 = eng.decode_batch(k, upload(rec2.view(np.int32)),
+                              upload(st2.view(np.int32).reshape(nstreams, -1)), dstates=dst)
     torch.cuda.synchronize()
     o1, c1, o2, c2 = o1.cpu().numpy(), c1.cpu().numpy(), o2.cpu().numpy(), c2.cpu().numpy()
     for s in range(nstreams):
@@ -718,7 +598,7 @@ def test_rx_then_device_decode_prints_what_the_reference_printed(name):
     n = a.size
     buf = np.zeros((2, pad4(n)), np.float32)
     buf[:, :n] = a
-    frames, states = eng.rx_batch(torch.from_numpy(buf).to(dev()), nsamples=n)
+    frames, states = eng.rx_batch(upload(buf), nsamples=n)
     kind = mm.decoder_for_mode(case["rx_mode"], rx.n_data_bits)
     out, cnt = eng.decode_batch(kind, frames, states)
     torch.cuda.synchronize()
@@ -756,8 +636,8 @@ def test_uic_frames_end_to_end():
         for i, a in enumerate(streams):
             buf[i, :len(a)] = a
             lens[i] = len(a)
-        frames, states = eng.rx_batch(torch.from_numpy(buf).to(dev()), nsamples=n,
-                                      nsamples_each=torch.from_numpy(lens).to(dev()))
+        frames, states = eng.rx_batch(upload(buf), nsamples=n,
+                                      nsamples_each=upload(lens))
         out, cnt = eng.decode_batch(kind, frames, states)
         torch.cuda.synchronize()
         fr, st = mm.frames_to_numpy(frames), mm.states_to_numpy(states)
@@ -796,7 +676,7 @@ def test_host_buffer_path_in_many_slabs(fmt, monkeypatch):
     eng, _ = engine_for(case)
     monkeypatch.delenv("FSK_B200_SLAB_BYTES")
     ref_eng, _ = engine_for(case)
-    frames, states = ref_eng.rx_batch(torch.from_numpy(hf).to(dev()), nsamples=n)
+    frames, states = ref_eng.rx_batch(upload(hf), nsamples=n)
     torch.cuda.synchronize()
     want_fr, want_st = mm.frames_to_numpy(frames), mm.states_to_numpy(states)
     if fmt == "f32":
@@ -812,16 +692,6 @@ def test_host_buffer_path_in_many_slabs(fmt, monkeypatch):
 # --------------------------------------------------------------------------
 # the drop-in boundary end to end: the unmodified reference CLI on this library
 # --------------------------------------------------------------------------
-def _write_wav(path, samples, rate, as_float):
-    import struct
-    if as_float:
-        data, fmt, bits = samples.astype("<f4").tobytes(), 3, 32
-    else:
-        data, fmt, bits = np.round(samples * 32768.0).astype("<i2").tobytes(), 1, 16
-    hdr = b"RIFF" + struct.pack("<I", 36 + len(data)) + b"WAVE" + b"fmt " + struct.pack(
-        "<IHHIIHH", 16, fmt, 1, rate, rate * bits // 8, bits // 8, bits) + b"data" + struct.pack("<I", len(data))
-    with open(path, "wb") as f:
-        f.write(hdr + data)
 
 
 CLI_CASES = [c for c in refcases.EVERY + refcases.CLI_ONLY if c["audio"]]
@@ -843,11 +713,10 @@ def test_reference_cli_on_this_library(case, tmp_path):
     a = gu.audio(case, g)
     rate = int(g["audio_len"][1])
     wav = str(tmp_path / "x.wav")
-    _write_wav(wav, a, rate, bool(g["audio_len"][2]))
+    write_wav(wav, a, rate, bool(g["audio_len"][2]))
     env = dict(os.environ)
     if conftest.EMU_DEVICE is not None:         # FSK_B200_EMU=1: the emulation build answers to the library's name
-        import test_dropin_cli
-        env["LD_LIBRARY_PATH"] = test_dropin_cli.emulation_as_product()
+        env["LD_LIBRARY_PATH"] = emulation_as_product()
     r = subprocess.run([exe, "--rx", "--file", wav] + list(case["rx"]), env=env, stdout=subprocess.PIPE,
                        stderr=subprocess.PIPE, timeout=600)
     assert r.returncode == 0, r.stderr[-500:]
@@ -947,7 +816,7 @@ def test_streams_fed_in_chunks_give_the_records_of_one_pass(mode, kw):
             chunk[i, :k] = full[i][fed[i]:fed[i] + k]
             clen[i] = k
             fed[i] += k
-        mm.stream_push(rows, fill, states, torch.from_numpy(chunk).to(dev()), torch.from_numpy(clen).to(dev()),
+        mm.stream_push(rows, fill, states, upload(chunk), upload(clen),
                        dropped=dropped)
         frames, states = eng.rx_batch(rows, nsamples=stride, nsamples_each=fill, max_frames=max_frames, states=states)
         torch.cuda.synchronize()
@@ -1019,7 +888,7 @@ def test_live_receiver_prints_the_reference_output_however_the_stream_is_cut(nam
             chunk[i, :k] = a[fed[i]:fed[i] + k]
             clen[i] = k
             fed[i] += k
-        take(*lr.feed(torch.from_numpy(chunk).to(dev()), torch.from_numpy(clen).to(dev())))
+        take(*lr.feed(upload(chunk), upload(clen)))
     take(*lr.finish())
     torch.cuda.synchronize()
     assert int(lr.dropped.sum()) == 0
@@ -1057,7 +926,7 @@ def test_per_bit_magnitudes_vs_oracle(mode, kw):
         sigma = (0.0, 0.0, 0.05, 0.3)[s % 4]
         pos = int(rng.integers(0, clean.size - wlen))
         buf[s] = (clean[pos:pos + wlen] + sigma * rng.standard_normal(wlen)).astype(np.float32)
-    t = lambda a, dt: torch.from_numpy(np.ascontiguousarray(np.asarray(a).astype(dt))).to(dev())
+    t = lambda a, dt: upload(np.ascontiguousarray(np.asarray(a).astype(dt)))
     full = lambda v, dt: t(np.full(nstreams, v), dt)
     step = max(tmc // 8, 1)
     frames, mags = eng.find_frame_batch(t(buf, np.float32), full(wlen, np.int32), full(first, np.int32),
@@ -1220,8 +1089,8 @@ def test_baseline_configs_large_batch_sample_vs_oracle(mode, kw, nstreams, nword
     st = mm.states_to_numpy(states)
     assert (st["done"] == 1).all()
     rows = np.arange(0, nstreams, max(1, nstreams // max(8, nstreams // 100)))
-    fr = mm.frames_to_numpy(frames[torch.from_numpy(rows).to(dev())])
-    hx = x[torch.from_numpy(rows).to(dev())].cpu().numpy()
+    fr = mm.frames_to_numpy(frames[upload(rows)])
+    hx = x[upload(rows)].cpu().numpy()
     n_flip = 0
     for i, s in enumerate(rows):
         want = orc.rx_run(m, hx[i, :n].copy(), literal=False)
@@ -1264,8 +1133,8 @@ def test_rx_batch_s16_resident_is_bit_identical_to_the_float_path(mode, kw):
     pcm = np.zeros((nstreams, stride), np.int16)
     for s, r in enumerate(rows):
         pcm[s, :r.size] = r
-    lens_t = torch.from_numpy(np.asarray(lens, np.int32)).to(dev())
-    d16 = torch.from_numpy(pcm).to(dev())
+    lens_t = upload(np.asarray(lens, np.int32))
+    d16 = upload(pcm)
     f32 = mm.s16_to_f32(d16)
     fr_a, st_a = eng.rx_batch(f32, nsamples=n, nsamples_each=lens_t)
     fr_b, st_b = eng.rx_batch(d16, nsamples=n, nsamples_each=lens_t)
@@ -1284,7 +1153,7 @@ def test_rx_batch_s16_resident_is_bit_identical_to_the_float_path(mode, kw):
     st_c.zero_()
     sc = mm.states_to_numpy(st_c).copy()
     sc["pos"][:] = 13
-    st_c = torch.from_numpy(sc.view(np.int32).reshape(nstreams, -1)).to(dev())
+    st_c = upload(sc.view(np.int32).reshape(nstreams, -1))
     st_d = st_c.clone()
     fr_c, st_c = eng.rx_batch(f32, nsamples=n, nsamples_each=lens_t, states=st_c)
     fr_d, st_d = eng.rx_batch(d16, nsamples=n, nsamples_each=lens_t, states=st_d)
@@ -1313,7 +1182,7 @@ def test_live_receiver_frames_with_three_stop_bits_in_tiny_chunks():
     eng, _ = engine_for(case)
     buf = np.zeros((1, pad4(a.size)), np.float32)
     buf[0, :a.size] = a
-    frames, states = eng.rx_batch(torch.from_numpy(buf).to(dev()), nsamples=a.size)
+    frames, states = eng.rx_batch(upload(buf), nsamples=a.size)
     out, cnt = eng.decode_batch(mm.decoder_for_mode(case["rx_mode"], rx.n_data_bits), frames, states)
     torch.cuda.synchronize()
     want = bytes(out.cpu().numpy()[0, :int(cnt.cpu().numpy()[0])])
@@ -1338,7 +1207,7 @@ def test_live_receiver_frames_with_three_stop_bits_in_tiny_chunks():
             chunk[i, :k] = a[fed[i]:fed[i] + k]
             clen[i] = k
             fed[i] += k
-        take(*lr.feed(torch.from_numpy(chunk).to(dev()), torch.from_numpy(clen).to(dev())))
+        take(*lr.feed(upload(chunk), upload(clen)))
     take(*lr.finish())
     torch.cuda.synchronize()
     for i in range(nstreams):

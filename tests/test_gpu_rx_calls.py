@@ -17,7 +17,7 @@ import pytest
 
 import autoorc
 import minimodem_b200 as mm
-import test_gpu_instantiations as I
+from gpudev import dev, sync, torch, upload
 
 EINVAL = 22
 STRIDE = 64
@@ -44,8 +44,8 @@ KERNEL = {"fixed": "k_rx<", "host": "k_rx<", "auto": "k_rx_auto<", "tones": "k_r
 # --------------------------------------------------------------------------
 def test_rx_calls_on_the_emulated_kernels():
     """The `gpu` tests below on the host SIMT emulation of the kernels."""
-    import test_emu_parity
-    tail = test_emu_parity.run_emulated("gpu", "late", 900, module="test_gpu_rx_calls.py")
+    from gpudev import run_emulated
+    tail = run_emulated("gpu", "late", 900, module="test_gpu_rx_calls.py")
     assert " passed" in tail and "failed" not in tail
 
 
@@ -57,7 +57,7 @@ class Call:
     calls); call(**overrides) replaces any of them."""
 
     def __init__(self, name):
-        t = I.torch()
+        t = torch()
         self.name = name
         self.kind, self.elem, self.family = CALLS[name]
         self.host = self.kind == "host"
@@ -74,12 +74,12 @@ class Call:
                              max_frames=4, states=st)
             return
         n = self.k
-        x = t.zeros((1, STRIDE), dtype=t.float32 if self.elem == 4 else t.int16, device=I.dev())
-        fr = t.zeros((n, 4, 5), dtype=t.int32, device=I.dev())
-        st = t.zeros((n, mm.STATE_WORDS), dtype=t.int32, device=I.dev())
-        ast = t.zeros((n, mm.api.AUTO_STATE_BYTES), dtype=t.uint8, device=I.dev())
-        each = t.from_numpy(np.array([STRIDE], np.int32)).to(I.dev())
-        tb = self.eng.tone_bands([1200.0, 1070.0][:n], [2200.0, 1270.0][:n], device=I.dev())
+        x = t.zeros((1, STRIDE), dtype=t.float32 if self.elem == 4 else t.int16, device=dev())
+        fr = t.zeros((n, 4, 5), dtype=t.int32, device=dev())
+        st = t.zeros((n, mm.STATE_WORDS), dtype=t.int32, device=dev())
+        ast = t.zeros((n, mm.api.AUTO_STATE_BYTES), dtype=t.uint8, device=dev())
+        each = upload(np.array([STRIDE], np.int32))
+        tb = self.eng.tone_bands([1200.0, 1070.0][:n], [2200.0, 1270.0][:n], device=dev())
         self.keep = (x, fr, st, ast, each, tb)
         P = mm.api._ptr
         self.args = dict(e=self.eng._e, samples=P(x), nrows=1, stride=STRIDE, each=P(each), n_all=STRIDE,
@@ -172,7 +172,7 @@ def test_rx_call_launches_its_kernel_family(name):
     c = Call(name)
     before = mm.launch_count()
     assert c() == 0, (name, mm.api.lib().fsk_b200_last_error().decode())
-    I.sync()
+    sync()
     assert mm.launch_count() > before, name
     lk = c.eng.last_kernel()
     assert lk.startswith(KERNEL[c.kind]), (name, lk)

@@ -49,17 +49,15 @@ import pytest
 
 import autoorc
 import orc
+import rxfam
 import tie_screen
-import test_gpu_instantiations as I
-import test_gpu_launch_shapes as LS
+import gpudev
+from gpudev import dev, mm, pcm, records, sync, torch, upload, widen
+from rxcases import check_channels_against_oracle, live_text, on_pair, one_pass_text, random_pair, run_channels
+from rxfam import as_oracle_frames, compare_frames, compare_reports, reports_of
 
 f32 = np.float32
 NAN, INF = f32(np.nan), f32(np.inf)
-
-
-def mm():
-    import minimodem_b200
-    return minimodem_b200
 
 
 # --------------------------------------------------------------------------------------------------
@@ -67,8 +65,8 @@ def mm():
 # --------------------------------------------------------------------------------------------------
 def test_sample_domain_file_on_the_emulated_kernels():
     """The `gpu` tests below on the host SIMT emulation of the kernels (the TMA bulk fill excepted)."""
-    import test_emu_parity
-    tail = test_emu_parity.run_emulated("gpu", "late", 3000, module="test_gpu_sample_domain.py")
+    from gpudev import run_emulated
+    tail = run_emulated("gpu", "late", 3000, module="test_gpu_sample_domain.py")
     assert " passed" in tail and "failed" not in tail
 
 
@@ -221,10 +219,7 @@ def test_the_references_frames_at_each_scale_are_the_recorded_ones():
 # --------------------------------------------------------------------------------------------------
 # the device against the FLAT oracle, per launch family
 # --------------------------------------------------------------------------------------------------
-PER_CAND = LS.PER_CAND
-FAMILIES = dict(LS.FAMILIES)
-FAMILIES["generic"] = dict(call="rx", src="f32", env=PER_CAND, kern=("k_rx", 1, 0))
-FAMILIES["generic-s16"] = dict(call="rx", src="s16", env=PER_CAND, kern=("k_rx", 1, 0))
+FAMILIES = {f: v for f, v in rxfam.FAMILIES.items() if not f.startswith("channels")}
 PRESET = {"per-candidate": ("1200", 48000), "shared-segment": ("300", 48000), "prefix-table": ("rtty", 8000),
           "tones": ("1200", 48000), "auto": ("1200", 48000), "generic": ("25", 48000)}
 FLOAT_KINDS = ["nan", "nan-burst", "+inf", "-inf", "click-1e4", "click-1e30"]
@@ -235,14 +230,6 @@ REPORT = {}
 
 def preset(fam):
     return next(v for k, v in PRESET.items() if fam.startswith(k))
-
-
-def pcm(a):
-    return np.clip(np.round(a.astype(np.float64) * 32768.0), -32768, 32767).astype(np.int16)
-
-
-def widen(q):
-    return q.astype(np.float32) * f32(1.0 / 32768.0)
 
 
 def places(m, x, seed, lead=None):
@@ -313,9 +300,8 @@ class Case:
             if self.call in ("tones", "auto"):
                 nb = int(mm().RxEngine.for_mode(mode, rate).params.nbands)
             if self.call == "tones":
-                import test_gpu_stream_tones as TT
-                fm, fs = TT.random_pair(rng, float(base.band_width), nb)
-                m = TT.on_pair(mode, rate, fm, fs)
+                fm, fs = random_pair(rng, float(base.band_width), nb)
+                m = on_pair(mode, rate, fm, fs)
                 pairs.append((fm, fs))
             if self.call == "auto":
                 # a pair on the band grid that the scan finds: the places come from the oracle on that pair
@@ -375,59 +361,29 @@ def case_of(fam):
 
 
 def engine_for(fam, c, monkeypatch):
-    LS.set_env(monkeypatch, FAMILIES[fam]["env"])
-    eng = mm().RxEngine.for_mode(c.mode, c.rate)
-    if c.call == "auto":
-        eng.set_auto_carrier(autoorc.DEFAULT_THRESHOLD)
-    return eng
+    return rxfam.new_engine(monkeypatch, fam, lambda: mm().RxEngine.for_mode(c.mode, c.rate))
 
 
-def launch(eng, c, rows, bases):
-    """rows: float32 or int16 arrays, bases: the clean stream each row comes from (its tone pair) ->
+def launch(eng, c, rows_, bases):
+    """rows_: float32 or int16 arrays, bases: the clean stream each row comes from (its tone pair) ->
     (records per row, states, bands per row or None, last_kernel)"""
-    t = I.torch()
-    n = max(r.size for r in rows)
-    buf = I._rows(rows, n, rows[0].dtype, 8)
-    lens = t.from_numpy(np.array([r.size for r in rows], np.int32)).to(I.dev())
-    x = t.from_numpy(buf).to(I.dev())
     bands = None
-    if c.call == "rx":
-        fr, st = eng.rx_batch(x, nsamples=n, nsamples_each=lens)
-    elif c.call == "tones":
+    if c.call == "tones":
         pairs = [c.pairs[b] for b in bases]
-        tb = eng.tone_bands([p[0] for p in pairs], [p[1] for p in pairs], device=I.dev())
-        fr, st = eng.rx_batch_tones(x, tb, nsamples=n, nsamples_each=lens)
-    else:
-        fr, st, _, rb = eng.rx_batch_auto(x, nsamples=n, nsamples_each=lens, rec_band=True)
-        bands = rb.cpu().numpy()
-    I.sync()
-    fr, st = mm().frames_to_numpy(fr), mm().states_to_numpy(st)
-    assert (st["done"] == 1).all()
-    return [fr[s, :int(st["nframes"][s])] for s in range(len(rows))], st, bands, eng.last_kernel()
-
-
-def check_family(fam, text):
-    k = LS.LK.match(text)
-    assert k, text
-    name, mode, fill = FAMILIES[fam]["kern"]
-    assert (k.group(1), int(k.group(5)), int(k.group(6))) == (name, mode, fill), (fam, text)
-    src = k.group(7)
-    assert src.split(",")[0] == FAMILIES[fam]["src"], (fam, text)
-    if fam == "per-candidate":
-        assert src == "f32,slide", text
-    if fam == "per-candidate-noslide":
-        assert src == "f32", text
+        bands = eng.tone_bands([p[0] for p in pairs], [p[1] for p in pairs], device=dev())
+    r = rxfam.call(eng, c.fam, rows_, [x.size for x in rows_], bands=bands, rec_band=True)
+    assert (r.st["done"] == 1).all()
+    return [r.fr[s, :int(r.st["nframes"][s])] for s in range(len(rows_))], r.st, r.rec_band, r.k["text"]
 
 
 def compare(c, i, recs, st, bands, what):
-    import test_gpu_parity as T
     want, robust = c.screened[i]
-    got = T.as_oracle_frames(recs)
+    got = as_oracle_frames(recs)
     if not robust:
         assert abs(len(got) - len(want["frames"])) <= 1, (what, len(got), len(want["frames"]))
         return False
-    T.compare_frames(got, want["frames"], what)
-    T.compare_reports(T.reports_of(recs, st), want["reports"], what)
+    compare_frames(got, want["frames"], what)
+    compare_reports(reports_of(recs, st), want["reports"], what)
     if bands is not None:
         fb = [int(b) for r, b in zip(recs, bands) if int(r["frame_start"]) != mm().FRAME_REPORT]
         assert fb == want["frame_band"], (what, fb, want["frame_band"])
@@ -442,15 +398,14 @@ FAM_ROWS = list(FAMILIES)
 def test_bad_samples_in_every_family(fam, monkeypatch):
     """Per family: the poisoned streams (every kind at every place) against the screened FLAT oracle; the clean
     streams of the launch byte for byte those of a launch whose other rows are the unpoisoned streams."""
-    if I.emulated() and FAMILIES[fam]["kern"][2] == 1:
-        pytest.skip("the host emulation does not model cp.async.bulk / mbarrier")
+    rxfam.skip_tma(fam)
     c = case_of(fam)
     eng = engine_for(fam, c, monkeypatch)
     src = lambda a: pcm(a) if c.s16 else a
     rows = [src(a) for a in c.clean] + [x for _, _, _, x in c.items]
     bases = list(range(len(c.clean))) + [b for b, _, _, _ in c.items]
     recs, st, bands, k = launch(eng, c, rows, bases)
-    check_family(fam, k)
+    rxfam.check_family(fam, rxfam.parse_launch(k))
     ref_rows = [src(a) for a in c.clean] + [src(c.clean[b]) for b, _, _, _ in c.items]
     recs0, st0, bands0, k0 = launch(eng, c, ref_rows, bases)
     assert k0 == k
@@ -475,15 +430,13 @@ def test_a_poisoned_row_in_tone_pair_channels():
     burst in a frame of its originate channel, one with a 1e30 click; both channels of each row against the
     screened oracle on their pair, and the clean row's channels byte for byte those of the launch without the
     poisoned rows."""
-    import test_gpu_stream_tones as TT
-    import test_gpu_channels as TC
     rng = np.random.default_rng(3103)
     pairs = [(1270.0, 1070.0), (2225.0, 2025.0)]
     lines = []
     for r in range(3):
         x = np.zeros(0, np.float32)
         for fm, fs in pairs:
-            m = TT.on_pair("300", 48000, fm, fs)
+            m = on_pair("300", 48000, fm, fs)
             a = clean_stream(m, 50 + 2 * r + len(x), nwords=8, amplitude=float(rng.uniform(0.3, 0.8)))
             a = np.concatenate([np.zeros(int(rng.integers(0, 2000)), np.float32), a])
             if a.size > x.size:
@@ -491,7 +444,7 @@ def test_a_poisoned_row_in_tone_pair_channels():
             x = x.copy()
             x[:a.size] += a
         lines.append((x + f32(1e-3) * rng.standard_normal(x.size).astype(np.float32)).astype(np.float32))
-    m0 = TT.on_pair("300", 48000, *pairs[0])
+    m0 = on_pair("300", 48000, *pairs[0])
     p1, bn = places(m0, lines[1], 1)
     p2, _ = places(m0, lines[2], 2)
     bad = [lines[0], poison(lines[1], "nan-burst", p1["window"], bn), poison(lines[2], "click-1e30", p2["slide"], bn)]
@@ -501,23 +454,23 @@ def test_a_poisoned_row_in_tone_pair_channels():
         rows_bad = [conv(a) for a in bad]
         fl = [widen(r) for r in rows_bad] if src == "s16" else rows_bad
         if src == "f32":
-            texts = TC.check_channels_against_oracle(eng, "300", 48000, fl, [pairs] * 3, 2, ("channels", src))
+            texts = check_channels_against_oracle(eng, "300", 48000, fl, [pairs] * 3, 2, ("channels", src))
             assert all(len(t) >= 3 for t in texts), texts
-        buf, n = TT.rows(rows_bad, rows_bad[0].dtype, 8)
-        buf0, _ = TT.rows([conv(a) for a in lines], rows_bad[0].dtype, 8)
+        buf, n = gpudev.rows(rows_bad, rows_bad[0].dtype, 8)
+        buf0, _ = gpudev.rows([conv(a) for a in lines], rows_bad[0].dtype, 8)
         flat = [p for _ in range(3) for p in pairs]
-        tb = eng.tone_bands([p[0] for p in flat], [p[1] for p in flat], device=I.dev())
+        tb = eng.tone_bands([p[0] for p in flat], [p[1] for p in flat], device=dev())
         lens = np.array([a.size for a in lines], np.int32)
-        fa, sa = TC.run_channels(eng, buf, n, lens, tb, 2)
+        fa, sa = run_channels(eng, buf, n, lens, tb, 2)
         assert eng.last_kernel().startswith("k_rx_tones") and eng.last_kernel().endswith("channels=2")
         assert ("src=" + src) in eng.last_kernel(), eng.last_kernel()
-        fb, sb = TC.run_channels(eng, buf0, n, lens, tb, 2)
-        ra, sa = TC.records(fa, sa)
-        rb, sb = TC.records(fb, sb)
+        fb, sb = run_channels(eng, buf0, n, lens, tb, 2)
+        ra, sa = records(fa, sa)
+        rb, sb = records(fb, sb)
         assert ra[:2] == rb[:2] and sa[:2].tobytes() == sb[:2].tobytes(), src
         if src == "s16":
-            ff, sf = TC.run_channels(eng, I._rows(fl, n, np.float32, 8), n, lens, tb, 2)
-            rf, sf = TC.records(ff, sf)
+            ff, sf = run_channels(eng, gpudev.rows(fl, np.float32, 8, n=n)[0], n, lens, tb, 2)
+            rf, sf = records(ff, sf)
             assert rf == ra and sf.tobytes() == sa.tobytes()
 
 
@@ -539,24 +492,23 @@ DEVICE_FRAMES = {"1200": [0, 0, 8, 8, 8, 8, 0, 0, 0], "300": [0, 0, 8, 8, 8, 0, 
 def test_scaled_streams_stop_decoding_at_the_documented_bound(mode, rate):
     """A clean stream scaled by 1e-45 (the smallest subnormal) to 1e37 on the default kernel: wherever the
     device decodes, its records are the oracle's; where `re*re + im*im` overflows fp32 it gives no frame."""
-    import test_gpu_parity as T
     m = orc.Mode(mode, sample_rate=rate)
     eng = mm().RxEngine.for_mode(mode, rate)
     rows = [scaled(m, s) for s in SCALES]
-    t = I.torch()
+    t = torch()
     n = max(r.size for r in rows)
-    fr, st = eng.rx_batch(t.from_numpy(I._rows(rows, n, np.float32, 8)).to(I.dev()), nsamples=n)
-    I.sync()
+    fr, st = eng.rx_batch(upload(gpudev.rows(rows, np.float32, 8, n=n)[0]), nsamples=n)
+    sync()
     fr, st = mm().frames_to_numpy(fr), mm().states_to_numpy(st)
     got = []
     for i, s in enumerate(SCALES):
         recs = fr[i, :int(st["nframes"][i])]
-        g = T.as_oracle_frames(recs)
+        g = as_oracle_frames(recs)
         got.append(len(g))
         want = orc.rx_run(m, rows[i])
         if g:
-            T.compare_frames(g, want["frames"], (mode, s))
-            T.compare_reports(T.reports_of(recs, st[i]), want["reports"], (mode, s))
+            compare_frames(g, want["frames"], (mode, s))
+            compare_reports(reports_of(recs, st[i]), want["reports"], (mode, s))
     print("%s: %s frames per scale %s (reference %s)" % (eng.last_kernel(), got, SCALES, REF_FRAMES[mode]))
     assert got == DEVICE_FRAMES[mode], (mode, got)
 
@@ -585,7 +537,7 @@ def test_int16_full_scale_equals_the_float_path(fam, monkeypatch):
     rows = full_scale_rows(c)
     bases = list(range(len(c.clean))) + [0]
     a, sa, ba, ka = launch(eng, c, rows, bases)
-    check_family(fam, ka)
+    rxfam.check_family(fam, rxfam.parse_launch(ka))
     b, sb, bb, kb = launch(eng, c, [widen(r) for r in rows], bases)
     assert kb.split(",src=")[0] == ka.split(",src=")[0], (ka, kb)
     assert sa.tobytes() == sb.tobytes(), fam
@@ -600,7 +552,7 @@ def test_int16_full_scale_through_the_host_slab_call():
     eng = mm().RxEngine.for_mode(c.mode, c.rate)
     rows = full_scale_rows(c)
     n = max(r.size for r in rows)
-    q = I._rows(rows, n, np.int16, 8)
+    q = gpudev.rows(rows, np.int16, 8, n=n)[0]
     fa, sa = eng.rx_batch_host_s16(q, nsamples=n)
     fb, sb = eng.rx_batch_host(widen(q), nsamples=n)
     assert sa.tobytes() == sb.tobytes()
@@ -635,15 +587,14 @@ def live_rows(form):
 def channel_lines():
     """Bell103 lines carrying originate and answer, k = 2: a clean line, a NaN burst, an inf and a 1e30 click
     in a frame of the originate channel"""
-    import test_gpu_stream_tones as TT
     rng = np.random.default_rng(3104)
     pairs = [(1270.0, 1070.0), (2225.0, 2025.0)]
-    m0 = TT.on_pair("300", 48000, *pairs[0])
+    m0 = on_pair("300", 48000, *pairs[0])
     lines = []
     for r in range(4):
         x = np.zeros(0, np.float32)
         for fm, fs in pairs:
-            a = clean_stream(TT.on_pair("300", 48000, fm, fs), 70 + 2 * r + len(x), nwords=8,
+            a = clean_stream(on_pair("300", 48000, fm, fs), 70 + 2 * r + len(x), nwords=8,
                              amplitude=float(rng.uniform(0.3, 0.8)))
             a = np.concatenate([np.zeros(int(rng.integers(0, 2000)), np.float32), a])
             if a.size > x.size:
@@ -658,69 +609,6 @@ def channel_lines():
         if kind == "nan-burst":
             bursts.append((r, pm["window"]))
     return "300", 48000, lines, [p for _ in lines for p in pairs], 2, bursts
-
-
-def one_pass_text(mode, rate, rows, pairs, k, auto):
-    """one rx call of the live receiver's family over the whole rows, decoded from fresh decoder state"""
-    t = I.torch()
-    eng = mm().RxEngine.for_mode(mode, rate)
-    buf = I._rows(rows, max(r.size for r in rows), rows[0].dtype, 8)
-    x = t.from_numpy(buf).to(I.dev())
-    lens = t.from_numpy(np.array([r.size for r in rows], np.int32)).to(I.dev())
-    if pairs is not None:
-        tb = eng.tone_bands([p[0] for p in pairs], [p[1] for p in pairs], device=I.dev())
-        fr, st = eng.rx_batch_tones(x, tb, nsamples=buf.shape[1], nsamples_each=lens, channels_per_row=k)
-    elif auto:
-        eng.set_auto_carrier(autoorc.DEFAULT_THRESHOLD)
-        fr, st, _ = eng.rx_batch_auto(x, nsamples=buf.shape[1], nsamples_each=lens)
-    else:
-        fr, st = eng.rx_batch(x, nsamples=buf.shape[1], nsamples_each=lens)
-    out, cnt = eng.decode_batch(mm().decoder_for_mode(mode, int(eng.params.n_data_bits)), fr, st)
-    I.sync()
-    out, cnt = out.cpu().numpy(), cnt.cpu().numpy()
-    return [out[s, :int(cnt[s])].tobytes() for s in range(len(cnt))]
-
-
-def live_text(mode, rate, rows, pairs, k, auto, max_chunk, seed, cuts_at=(), pcm16=False):
-    """LiveReceiver fed the rows in random chunks (a cut at every sample of `cuts_at`: (row, sample))"""
-    from minimodem_b200.serving import LiveReceiver
-    t = I.torch()
-    kw = {}
-    if pairs is not None:
-        eng = mm().RxEngine.for_mode(mode, rate)
-        kw = dict(tones=eng.tone_bands([p[0] for p in pairs], [p[1] for p in pairs], device=I.dev()),
-                  channels_per_row=k)
-    if auto:
-        kw = dict(auto_carrier=autoorc.DEFAULT_THRESHOLD)
-    lr = LiveReceiver(mode, rate, len(rows), max_chunk=max_chunk, device=I.dev(), pcm16=pcm16, **kw)
-    rng = np.random.default_rng(seed)
-    cuts = []
-    for r, x in enumerate(rows):
-        c = set(int(v) for v in np.cumsum(rng.integers(1, max_chunk + 1, x.size // 2 + 2)) if v < x.size)
-        c |= {p for rr, p in cuts_at if rr == r}
-        c = sorted(c | {x.size})
-        cuts.append([b - a for a, b in zip([0] + c, c)])
-    assert all(max(v) <= max_chunk for v in cuts)
-    nch = len(rows) * k
-    texts = [b""] * nch
-
-    def take(res):
-        o, n = res
-        o, n = o.cpu().numpy(), n.cpu().numpy()
-        for s in range(nch):
-            texts[s] += o[s, :int(n[s])].tobytes()
-    fed = [0] * len(rows)
-    for step in range(max(len(v) for v in cuts)):
-        chunk = np.zeros((len(rows), max_chunk), rows[0].dtype)
-        k_ = np.zeros(len(rows), np.int32)
-        for r, x in enumerate(rows):
-            if step < len(cuts[r]):
-                k_[r] = cuts[r][step]
-                chunk[r, :k_[r]] = x[fed[r]:fed[r] + k_[r]]
-                fed[r] += int(k_[r])
-        take(lr.feed(t.from_numpy(chunk).to(I.dev()), t.from_numpy(k_).to(I.dev())))
-    take(lr.finish())
-    return texts
 
 
 @pytest.mark.gpu

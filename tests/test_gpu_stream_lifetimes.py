@@ -22,15 +22,16 @@ import pytest
 
 import autoorc
 import orc
-import test_gpu_channels as TC
-import test_gpu_launch_shapes as LS
-import test_gpu_stream_tones as TT
+import rxfam
+from gpudev import bands_tensor, dev, emulated, mm, pcm, records, rows, state_rows, sync, torch, upload
+import rxcases
+from rxcases import (ANSWER, ORIGINATE, call_audio, channel_rows, cuts, duplex_audio, random_states,
+                     shape_case)
 
 EINVAL = 22
 ENDED = 2
 OPEN, END = 1, 2
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-mm, torch, dev, sync, t_ = TT.mm, TT.torch, TT.dev, TT.sync, TC.t_
 SESSION = ("carrier", "noconfidence", "track_amplitude", "peak_confidence", "carrier_nsamples",
            "confidence_total", "amplitude_total", "nframes_decoded", "done")
 
@@ -41,8 +42,8 @@ SESSION = ("carrier", "noconfidence", "track_amplitude", "peak_confidence", "car
 @pytest.mark.parametrize("async_mode", ["eager", "late"])
 def test_stream_lifetimes_on_the_emulated_kernels(async_mode):
     """The `gpu` tests below on the host SIMT emulation of the kernels (the TMA bulk fill excepted)."""
-    import test_emu_parity
-    tail = test_emu_parity.run_emulated("gpu", async_mode, 3000, module="test_gpu_stream_lifetimes.py")
+    from gpudev import run_emulated
+    tail = run_emulated("gpu", async_mode, 3000, module="test_gpu_stream_lifetimes.py")
     assert " passed" in tail and "failed" not in tail
 
 
@@ -76,14 +77,14 @@ def flagged(n, spw=8):
 def with_flags(nstreams, flags, st=None):
     st = np.zeros(nstreams, mm().STATE_DTYPE) if st is None else st.copy()
     st["done"] = np.where(flags, ENDED, st["done"])
-    return TT.state_rows(st)
+    return state_rows(st)
 
 
 def window_of(eng, call):
     return eng.auto_stream_window() if call == "auto" else eng.stream_window()
 
 
-FLAG_FAMS = [f for f in LS.FAMILIES] + ["channels-2", "channels-3", "generic", "generic-s16"]
+FLAG_FAMS = list(rxfam.FAMILIES)
 
 
 def flag_case(fam):
@@ -91,7 +92,7 @@ def flag_case(fam):
     of most launches, the last one partial), the six of the family's case repeated"""
     if fam.startswith("channels"):
         k = int(fam[-1])
-        streams, lens, b = TC.channel_rows("1200", 48000, 7, k, 77 + k)
+        streams, lens, b = channel_rows("1200", 48000, 7, k, 77 + k)
         return (lambda: mm().RxEngine.for_mode("1200", 48000)), "tones", "f32", streams, lens * 7 // 8, b, k
     if fam.startswith("generic"):
         rng = np.random.default_rng(25)
@@ -104,52 +105,21 @@ def flag_case(fam):
         lens = np.array([x.size * 7 // 8 for x in streams], np.int32)
         return ((lambda: mm().RxEngine.for_mode("25", 48000)), "rx", "s16" if fam.endswith("s16") else "f32",
                 streams, lens, None, 1)
-    f = LS.FAMILIES[fam]
+    f = rxfam.FAMILIES[fam]
     preset = ("300", 48000) if fam.startswith("prefix") else ("1200", 48000)
-    make, streams, lens, bands, _ = LS.case(fam, preset)
+    make, streams, lens, bands, _ = shape_case(fam, preset)
     idx = [i % len(streams) for i in range(19)]
     b = None if bands is None else np.array([bands[i] for i in idx], np.uint32)
     # every row cut inside its transmission, so that the holdback holds records back
     return make, f["call"], f["src"], [streams[i] for i in idx], lens[idx] * 7 // 8, b, 1
 
 
-def rx_any(eng, call, src, streams, lens, bands, k, states=None, auto_states=None, max_frames=None):
-    """one rx call of the family; returns (records per channel, states, auto states bytes or None)"""
-    t = torch()
-    buf, n = TT.rows([TT.pcm(a) for a in streams] if src == "s16" else streams,
-                     np.int16 if src == "s16" else np.float32, 8)
-    x, le = t_(buf), t_(np.asarray(lens, np.int32))
-    ast = None
-    if call == "rx":
-        fr, st = eng.rx_batch(x, nsamples=n, nsamples_each=le, states=states, max_frames=max_frames)
-    elif call == "tones":
-        fr, st = eng.rx_batch_tones(x, TC.bands_tensor(bands), nsamples=n, nsamples_each=le, states=states,
-                                    max_frames=max_frames, channels_per_row=k)
-    else:
-        fr, st, ast = eng.rx_batch_auto(x, nsamples=n, nsamples_each=le, states=states, auto_states=auto_states,
-                                        max_frames=max_frames)
-    sync()
-    recs, sn = TC.records(fr, st)
-    return recs, sn, st, (None if ast is None else ast.cpu().numpy().copy())
-
-
-def new_engine(monkeypatch, fam, make, call):
-    LS.set_env(monkeypatch, LS.FAMILIES[fam]["env"] if fam in LS.FAMILIES else {})
-    eng = make()
-    if call == "auto":
-        eng.set_auto_carrier(autoorc.DEFAULT_THRESHOLD)
-    return eng
-
-
-def check_launch(eng, fam):
-    if fam in LS.FAMILIES:
-        LS.check_family(fam, LS.launch(eng))
-    elif fam.startswith("generic"):
-        s = eng.last_kernel()
-        assert s.startswith("k_rx<") and "mode=1(" in s and ("src=s16" in s) == fam.endswith("s16"), s
-    else:
-        s = eng.last_kernel()
-        assert s.startswith("k_rx_tones<") and s.endswith(" channels=%s" % fam[-1]), s
+def rx_any(eng, fam, src, streams, lens, bands, states=None, auto_states=None, max_frames=None, k=None):
+    """one rx call of the family on the streams as `src` rows; returns (records per channel, states, device
+    states, auto states as numpy or None)"""
+    r = rxfam.call(eng, fam, [pcm(a) for a in streams] if src == "s16" else streams, lens, bands=bands,
+                   states=states, auto_states=auto_states, max_frames=max_frames, k=k)
+    return r.recs, r.st, r.states, (None if r.auto is None else r.auto.cpu().numpy().copy())
 
 
 # --------------------------------------------------------------------------
@@ -160,20 +130,19 @@ def check_launch(eng, fam):
 def test_the_flag_ends_a_stream_in_every_rx_family(fam, monkeypatch):
     """Holdback stream_window(), about half the states flagged: a flagged stream gives the records and state
     (flag aside) of the same engine at holdback 0, an unflagged one those of the batch with no flag."""
-    if fam in LS.FAMILIES:
-        LS.skip_tma(fam)
+    rxfam.skip_tma(fam)
     make, call, src, streams, lens, bands, k = flag_case(fam)
-    eng = new_engine(monkeypatch, fam, make, call)
+    eng = rxfam.new_engine(monkeypatch, fam, make)
     nch = len(streams) * k
     flags = flagged(nch)
     eng.set_holdback(0)
-    r0, s0, _, a0 = rx_any(eng, call, src, streams, lens, bands, k)
-    check_launch(eng, fam)
+    r0, s0, _, a0 = rx_any(eng, fam, src, streams, lens, bands)
+    rxfam.check_launch(eng, fam)
     eng.set_holdback(window_of(eng, call))
-    rh, sh, _, ah = rx_any(eng, call, src, streams, lens, bands, k)
-    check_launch(eng, fam)
-    rf, sf, _, af = rx_any(eng, call, src, streams, lens, bands, k, states=with_flags(nch, flags))
-    check_launch(eng, fam)
+    rh, sh, _, ah = rx_any(eng, fam, src, streams, lens, bands)
+    rxfam.check_launch(eng, fam)
+    rf, sf, _, af = rx_any(eng, fam, src, streams, lens, bands, states=with_flags(nch, flags))
+    rxfam.check_launch(eng, fam)
     for c in range(nch):
         want_r, want_s = (r0[c], s0[c]) if flags[c] else (rh[c], sh[c])
         assert rf[c] == want_r, (fam, c, bool(flags[c]))
@@ -198,12 +167,12 @@ def test_skip_rule_and_overflow_of_a_flagged_stream(src):
     eng = make()
     streams, lens = streams[:6], lens[:6]
     eng.set_holdback(0)
-    whole, sw, _, _ = rx_any(eng, "rx", src, streams, lens, None, 1)
+    whole, sw, _, _ = rx_any(eng, "per-candidate", src, streams, lens, None)
     eng.set_holdback(eng.stream_window())
     st0 = np.zeros(6, mm().STATE_DTYPE)
     st0["done"] = [1, 1 | ENDED, 1 | 4, ENDED, ENDED, 4]
     st0["pos"][:3] = 77
-    recs, st, _, _ = rx_any(eng, "rx", src, streams, lens, None, 1, states=TT.state_rows(st0))
+    recs, st, _, _ = rx_any(eng, "per-candidate", src, streams, lens, None, states=state_rows(st0))
     for s in (0, 1, 2, 5):
         assert recs[s] == b"" and st[s].tobytes() == st0[s].tobytes(), s
     assert recs[3] == whole[3] and recs[4] == whole[4]
@@ -211,7 +180,7 @@ def test_skip_rule_and_overflow_of_a_flagged_stream(src):
     states = with_flags(6, np.ones(6, bool))
     got = [b""] * 6
     for call in range(10000):
-        recs, st, states, _ = rx_any(eng, "rx", src, streams, lens, None, 1, states=states, max_frames=3)
+        recs, st, states, _ = rx_any(eng, "per-candidate", src, streams, lens, None, states=states, max_frames=3)
         got = [g + r for g, r in zip(got, recs)]
         if (st["done"] == (1 | ENDED)).all():
             break
@@ -219,7 +188,7 @@ def test_skip_rule_and_overflow_of_a_flagged_stream(src):
         with pytest.raises(RuntimeError):
             mm().check_not_truncated(states, 3)
         st["nframes"][:] = 0
-        states = TT.state_rows(st)
+        states = state_rows(st)
     assert call >= 2 and got == whole
     st["nframes"], st["done"] = sw["nframes"], sw["done"]
     assert st.tobytes() == sw.tobytes()
@@ -237,17 +206,17 @@ class Live:
         self.fill, self.dropped = z((nrows,)), z((nrows,))
         self.states = z((nrows * k, mm().STATE_WORDS))
         self.auto = t.zeros((nrows, mm().AUTO_STATE_BYTES), dtype=t.uint8).to(dev()) if call == "auto" else None
-        self.bands = None if bands is None else TC.bands_tensor(bands)
+        self.bands = None if bands is None else bands_tensor(bands)
         self.nb = int(eng.params.nbands)
         self.max_frames = eng.max_frames(stride)
 
     def tick(self, chunk, clen, events):
         """returns the records of this tick per channel and the states"""
         t = torch()
-        ev = t_(np.asarray(events, np.uint8))
+        ev = upload(np.asarray(events, np.uint8))
         if self.auto is not None:
-            self.auto.masked_fill_(t_((np.asarray(events) & OPEN) != 0)[:, None], 0)
-        mm().stream_push(self.rows, self.fill, self.states, t_(chunk), t_(np.asarray(clen, np.int32)),
+            self.auto.masked_fill_(upload((np.asarray(events) & OPEN) != 0)[:, None], 0)
+        mm().stream_push(self.rows, self.fill, self.states, upload(chunk), upload(np.asarray(clen, np.int32)),
                          dropped=self.dropped, channels_per_row=self.k, tone_bands=self.bands, nbands=self.nb,
                          row_events=ev)
         n = self.stride
@@ -263,17 +232,7 @@ class Live:
                                                                 max_frames=self.max_frames, states=self.states,
                                                                 auto_states=self.auto)
         sync()
-        return TC.records(fr, self.states)
-
-
-def cuts(rng, n, max_chunk):
-    """random chunk sizes summing to n, some of them a handful of samples"""
-    out = []
-    while n > 0:
-        c = int(rng.integers(1, 9)) if rng.random() < 0.25 else int(rng.integers(1, max_chunk + 1))
-        out.append(min(c, n))
-        n -= out[-1]
-    return out
+        return records(fr, self.states)
 
 
 def live_geometry(eng, call):
@@ -306,9 +265,9 @@ def test_staggered_ends_through_the_events(what, monkeypatch):
         bands = np.array([p for b in bands for p in (list(b), [nb, 3], list(b))], np.uint32)
         k = 3
         call = "tones"
-    eng = new_engine(monkeypatch, fam, make, call)
+    eng = rxfam.new_engine(monkeypatch, fam, make)
     eng.set_holdback(0)
-    whole, sw, _, _ = rx_any(eng, call, "f32", streams, [a.size for a in streams], bands, k)
+    whole, sw, _, _ = rx_any(eng, fam, "f32", streams, [a.size for a in streams], bands, k=k)
     window, max_chunk, stride = live_geometry(eng, call)
     eng.set_holdback(window)
     rng = np.random.default_rng(zlib.crc32(what.encode()))
@@ -365,7 +324,7 @@ def test_reopen_abandon_whole_stream_and_dropped_chunks():
     bands = bands[:6]
     window, max_chunk, stride = live_geometry(eng, "tones")
     eng.set_holdback(0)
-    whole, _, _, _ = rx_any(eng, "tones", "f32", streams, [a.size for a in streams], bands, 1)
+    whole, _, _, _ = rx_any(eng, "tones", "f32", streams, [a.size for a in streams], bands)
     eng.set_holdback(window)
     # the first stream of every row runs on another row's pair: rows are reopened on their own pair
     first_bands = np.roll(bands, 1, axis=0)
@@ -397,7 +356,7 @@ def test_reopen_abandon_whole_stream_and_dropped_chunks():
     assert (live.fill.cpu().numpy()[:3] == fill0[:3]).all() and (live.rows.cpu().numpy()[:3] == rows0[:3]).all()
     assert st[:3].tobytes() == st0[:3].tobytes() and (st["done"][:3] == 1 | ENDED).all()
     # phase 2: every row reopened on its own pair; row 0 takes its whole stream in one OPEN | END push
-    live.bands.copy_(TC.bands_tensor(bands))
+    live.bands.copy_(bands_tensor(bands))
     plans = [[streams[0].size]] + [cuts(rng, streams[r].size, max_chunk) for r in range(1, 6)]
     fed = [0] * 6
     got = [b""] * 6
@@ -467,7 +426,7 @@ def test_push_follows_the_event_rule():
         for with_bands in (False, True):
             fill = rng.integers(0, stride + 1, nrows).astype(np.int32)
             rows0 = rng.standard_normal((nrows, stride)).astype(np.float32)
-            st0 = TC.random_states(rng, nrows * k, fill, k)
+            st0 = random_states(rng, nrows * k, fill, k)
             pre = rng.integers(0, 3, nrows)                       # 0: no flag, 1: some channels, 2: all
             for r in range(nrows):
                 for c in range(r * k, r * k + k):
@@ -482,10 +441,10 @@ def test_push_follows_the_event_rule():
             chunk = rng.standard_normal((nrows, 200)).astype(np.float32)
             clen = rng.integers(0, 201, nrows).astype(np.int32)
             want = push_model(rows0, fill.astype(np.int64), st0, k, bands, nb, chunk, clen, events)
-            R, F, S, D = t_(rows0), t_(fill), TT.state_rows(st0), t_(np.full(nrows, -1, np.int32))
-            bt = t_(bands.view(np.int32)) if bands is not None else None
-            mm().stream_push(R, F, S, t_(chunk), t_(clen), dropped=D, channels_per_row=k, tone_bands=bt, nbands=nb,
-                             row_events=t_(events))
+            R, F, S, D = upload(rows0), upload(fill), state_rows(st0), upload(np.full(nrows, -1, np.int32))
+            bt = upload(bands.view(np.int32)) if bands is not None else None
+            mm().stream_push(R, F, S, upload(chunk), upload(clen), dropped=D, channels_per_row=k, tone_bands=bt, nbands=nb,
+                             row_events=upload(events))
             sync()
             what = (k, with_bands)
             assert (R.cpu().numpy() == want[0]).all(), what
@@ -495,9 +454,9 @@ def test_push_follows_the_event_rule():
                 assert got[c].tobytes() == want[2][c].tobytes(), (what, c, events[c // k], pre[c // k])
             assert (D.cpu().numpy() == want[3]).all(), what
             # row_events NULL: the channel push as it was (done = 0, no row dropped for its flags)
-            want = TC.push_model(rows0, fill.astype(np.int64), st0, k, bands, nb, chunk, clen)
-            R, F, S, D = t_(rows0), t_(fill), TT.state_rows(st0), t_(np.full(nrows, -1, np.int32))
-            mm().stream_push(R, F, S, t_(chunk), t_(clen), dropped=D, channels_per_row=k, tone_bands=bt, nbands=nb)
+            want = rxcases.push_model(rows0, fill.astype(np.int64), st0, k, bands, nb, chunk, clen)
+            R, F, S, D = upload(rows0), upload(fill), state_rows(st0), upload(np.full(nrows, -1, np.int32))
+            mm().stream_push(R, F, S, upload(chunk), upload(clen), dropped=D, channels_per_row=k, tone_bands=bt, nbands=nb)
             sync()
             assert (R.cpu().numpy() == want[0]).all() and (F.cpu().numpy() == want[1]).all(), what
             assert S.cpu().numpy().tobytes() == want[2].tobytes() and (D.cpu().numpy() == want[3]).all(), what
@@ -506,25 +465,6 @@ def test_push_follows_the_event_rule():
 # --------------------------------------------------------------------------
 # 6. LiveReceiver with churn
 # --------------------------------------------------------------------------
-def call_audio(rng, m, nwords):
-    if m.mode == "callerid":        # an SDMF message: type, length, date and time, number (decoded on its last byte)
-        digits = [ord("0") + int(d) for d in rng.integers(0, 10, 8 + 10)]
-        words = np.array([0x04, 18] + digits, np.uint32)
-    else:
-        words = rng.integers(0, 1 << m.n_data_bits, nwords, dtype=np.uint64).astype(np.uint32)
-    x = np.concatenate([np.zeros(int(rng.integers(0, 3 * m.derived().frame_nsamples)), np.float32),
-                        orc.tx_words(m, words, float(rng.uniform(0.3, 0.9)), 4096, True),
-                        np.zeros(int(rng.integers(0, 2 * m.derived().frame_nsamples)), np.float32)])
-    return (x + np.float32(3e-3) * rng.standard_normal(x.size)).astype(np.float32)
-
-
-def duplex_audio(rng, nwords):
-    mo, ma = TT.on_pair("300", 48000, *TT.ORIGINATE), TT.on_pair("300", 48000, *TT.ANSWER)
-    a, b = call_audio(rng, mo, nwords), call_audio(rng, ma, nwords)
-    x = np.zeros(max(a.size, b.size), np.float32)
-    x[:a.size] += a
-    x[:b.size] += b
-    return x
 
 
 CHURN = {
@@ -542,16 +482,16 @@ def one_pass_texts(c, calls, kind):
     k = c.get("k", 1)
     if c.get("auto"):
         eng.set_auto_carrier(autoorc.DEFAULT_THRESHOLD)
-    buf, n = TT.rows(calls, np.float32, 4)
-    lens = t_(np.array([a.size for a in calls], np.int32))
+    buf, n = rows(calls, np.float32, 4)
+    lens = upload(np.array([a.size for a in calls], np.int32))
     if k > 1:
-        bands = eng.tone_bands([TT.ORIGINATE[0], TT.ANSWER[0]] * len(calls), [TT.ORIGINATE[1], TT.ANSWER[1]] * len(calls),
+        bands = eng.tone_bands([ORIGINATE[0], ANSWER[0]] * len(calls), [ORIGINATE[1], ANSWER[1]] * len(calls),
                                device=dev())
-        fr, st = eng.rx_batch_tones(t_(buf), bands, nsamples=n, nsamples_each=lens, channels_per_row=k)
+        fr, st = eng.rx_batch_tones(upload(buf), bands, nsamples=n, nsamples_each=lens, channels_per_row=k)
     elif c.get("auto"):
-        fr, st, _ = eng.rx_batch_auto(t_(buf), nsamples=n, nsamples_each=lens)
+        fr, st, _ = eng.rx_batch_auto(upload(buf), nsamples=n, nsamples_each=lens)
     else:
-        fr, st = eng.rx_batch(t_(buf), nsamples=n, nsamples_each=lens)
+        fr, st = eng.rx_batch(upload(buf), nsamples=n, nsamples_each=lens)
     out, cnt = eng.decode_batch(kind, fr, st)
     sync()
     out, cnt = out.cpu().numpy(), cnt.cpu().numpy()
@@ -568,13 +508,13 @@ def test_live_receiver_with_calls_that_come_and_go(name):
     t = torch()
     c = CHURN[name]
     k = c.get("k", 1)
-    nrows = 8 if TT.emulated() else 200
+    nrows = 8 if emulated() else 200
     rng = np.random.default_rng(zlib.crc32(name.encode()))
     m = orc.Mode(c["mode"], sample_rate=c["rate"])
     kw = {}
     if k > 1:
         e0 = mm().RxEngine.for_mode(c["mode"], c["rate"])
-        kw = dict(tones=e0.tone_bands([TT.ORIGINATE[0], TT.ANSWER[0]] * nrows, [TT.ORIGINATE[1], TT.ANSWER[1]] * nrows,
+        kw = dict(tones=e0.tone_bands([ORIGINATE[0], ANSWER[0]] * nrows, [ORIGINATE[1], ANSWER[1]] * nrows,
                                       device=dev()), channels_per_row=k)
     if c.get("auto"):
         kw = dict(auto_carrier=autoorc.DEFAULT_THRESHOLD)
@@ -616,8 +556,8 @@ def test_live_receiver_with_calls_that_come_and_go(name):
             if cur[r] is None and ended_once[r] and rng.random() < 0.5:
                 clen[r] = int(rng.integers(1, max_chunk + 1))     # noise after the end: dropped
                 chunk[r, :clen[r]] = rng.standard_normal(clen[r]).astype(np.float32)
-        text, cnt = rx.feed(t.from_numpy(chunk).to(dev()), t.from_numpy(clen).to(dev()),
-                            opened=t.from_numpy(opened).to(dev()), ended=t.from_numpy(ended).to(dev()))
+        text, cnt = rx.feed(upload(chunk), upload(clen),
+                            opened=upload(opened), ended=upload(ended))
         sync()
         text, cnt = text.cpu().numpy(), cnt.cpu().numpy()
         dropped = rx.dropped.cpu().numpy()
@@ -644,7 +584,7 @@ def test_host_calls_honour_the_flag(src):
     make, _, _, streams, lens, _, _ = flag_case("per-candidate")
     streams = [a[:int(n) * 4 // 5] for a, n in zip(streams, lens)]     # cut inside the transmission
     eng = make()
-    buf, n = TT.rows([TT.pcm(a) for a in streams] if src == "s16" else streams,
+    buf, n = rows([pcm(a) for a in streams] if src == "s16" else streams,
                      np.int16 if src == "s16" else np.float32, 8)
     fn = eng.rx_batch_host_s16 if src == "s16" else eng.rx_batch_host
     eng.set_holdback(0)

@@ -11,8 +11,6 @@ others the same frame count within one.
 The CPU tests pin fsk_b200_tone_bands to fsk_b200_rx_params_derive and run the `gpu` tests of this file
 on the host SIMT emulation of the kernels (tests/emu)."""
 import ctypes as C
-import os
-import re
 import zlib
 
 import numpy as np
@@ -22,52 +20,13 @@ import golden_util as gu
 import orc
 import refcases
 import tie_screen
+from gpudev import dev, mm, pcm, rows, state_rows, sync, torch, upload
+from rxcases import (ANSWER, COVER, KEYS, ORIGINATE, TONE_PRESETS, auto_combos, duplex_case, lay_out, on_pair,
+                     random_pair, transmission)
+from rxfam import as_oracle_frames, check_against_oracle, compare_frames, reports_of
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-KERNELS = os.path.join(ROOT, "minimodem_b200", "csrc", "fsk_b200_kernels.cu")
 EINVAL, ENOTSUP = 22, 95
 f32 = np.float32
-
-# (G, W, L) of AUTO_COMBOS -> a preset (mode, sample rate) whose per-stream-table launch shape it is
-COVER = {
-    (8, 3, 2): ("1200", 48000),
-    (16, 2, 4): ("rtty", 8000),
-    (16, 3, 4): ("300", 48000),
-    (16, 3, 1): ("uic-train", 8000),
-    (32, 1, 4): ("rtty", 48000),
-    (32, 2, 4): ("110", 48000),
-    (32, 3, 2): ("uic-ground", 48000),
-}
-KEYS = sorted(COVER)
-PRESETS = ["rtty", "tdd", "same", "callerid", "uic-train", "uic-ground", "V.21", "2400", "1200", "600", "300",
-           "110", "12000", "45.45"]
-
-
-def mm():
-    import minimodem_b200
-    return minimodem_b200
-
-
-def torch():
-    return pytest.importorskip("torch")
-
-
-def emulated():
-    import conftest
-    return conftest.EMU_DEVICE is not None
-
-
-def dev():
-    import conftest
-    if conftest.EMU_DEVICE is not None:
-        return conftest.EMU_DEVICE
-    assert torch().cuda.is_available(), "GPU tests need a CUDA device"
-    return torch().device("cuda:0")
-
-
-def sync():
-    if not emulated():
-        torch().cuda.synchronize()
 
 
 # --------------------------------------------------------------------------
@@ -93,7 +52,7 @@ def test_tone_bands_equal_the_derived_bands():
     rng = np.random.default_rng(20261016)
     ndraw = nfail = nedge = 0
     for _ in range(3000):
-        mode = PRESETS[int(rng.integers(len(PRESETS)))]
+        mode = TONE_PRESETS[int(rng.integers(len(TONE_PRESETS)))]
         rate = float([8000, 11025, 22050, 44100, 48000, int(rng.integers(4000, 96001))][int(rng.integers(6))])
         bw = 0.0 if rng.random() < 0.4 else float(f32(rng.choice([rng.uniform(1, 400), rng.integers(1, 400)])))
         base = mm().rx_config_for_mode(mode, rate, band_width=bw)
@@ -147,12 +106,6 @@ def test_tone_bands_reject_negative_and_non_finite_tones():
     assert mm().lib().fsk_b200_tone_bands(C.byref(params), f32(1200), f32(2200), None) == -EINVAL
 
 
-def auto_combos():
-    src = open(KERNELS).read()
-    m = re.search(r"#define AUTO_COMBOS\(X\)((?:[^\n]*\\\n)*[^\n]*)", src)
-    return {tuple(int(v) for v in t) for t in re.findall(r"X\((\d+), (\d+), (\d+)\)", m.group(1))}
-
-
 def test_the_cover_table_is_the_auto_combo_list():
     assert set(COVER) == auto_combos()
 
@@ -166,78 +119,21 @@ def test_live_receiver_refuses_tones_with_auto_carrier():
 def test_gpu_stream_tones_file_on_the_emulated_kernels():
     """The `gpu` tests below on the host SIMT emulation of the kernels: copies landing late, the
     approximate units moved by up to 64 ulp."""
-    import test_emu_parity
-    tail = test_emu_parity.run_emulated("gpu", "late", 2400, module="test_gpu_stream_tones.py",
-                                        extra_env={"FSK_EMU_ULP": "64"})
+    from gpudev import run_emulated
+    tail = run_emulated("gpu", "late", 2400, module="test_gpu_stream_tones.py",
+                        extra_env={"FSK_EMU_ULP": "64"})
     assert " passed" in tail and "failed" not in tail
 
 
 def test_reference_vectors_on_the_emulated_kernels_eager_copies():
-    import test_emu_parity
-    tail = test_emu_parity.run_emulated("reference_vectors", "eager", 900, module="test_gpu_stream_tones.py")
+    from gpudev import run_emulated
+    tail = run_emulated("reference_vectors", "eager", 900, module="test_gpu_stream_tones.py")
     assert " passed" in tail and "failed" not in tail
 
 
 # --------------------------------------------------------------------------
 # streams
 # --------------------------------------------------------------------------
-def rows(streams, dtype, align):
-    n = max(len(a) for a in streams)
-    stride = (n + align - 1) & ~(align - 1)
-    buf = np.zeros((len(streams), stride), dtype)
-    for i, a in enumerate(streams):
-        buf[i, :len(a)] = a
-    return buf, n
-
-
-def pcm(a):
-    return np.clip(np.round(a * 32768.0), -32768, 32767).astype(np.int16)
-
-
-def on_pair(mode, rate, mark, space):
-    """orc.Mode of `mode` on the tone pair (mark, space), also for the presets whose tones the CLI fixes"""
-    m = orc.Mode(mode, sample_rate=rate)
-    m.mark_f, m.space_f = f32(mark), f32(space)
-    return m
-
-
-def fsk_audio(bits, spb, mark, space, rate, amplitude):
-    """Phase-continuous FSK: sample i carries bit floor(i / spb), at the exact (fractional) bit period."""
-    n = int(len(bits) * spb)
-    b = np.asarray(bits, np.int64)[np.minimum((np.arange(n) / spb).astype(np.int64), len(bits) - 1)]
-    f = np.where(b == 1, mark, space)
-    return (amplitude * np.sin(2 * np.pi * np.cumsum(f) / rate)).astype(np.float32)
-
-
-def transmission(rng, m, nwords, amplitude):
-    """nwords random data words on m's tones: the oracle's transmitter, or for UIC (expect string 11110010
-    and 39 data bits, no start or stop bits) synthesised frames after a mark leader"""
-    if m.expect_data_string is not None:
-        bits = [1] * 10
-        for _ in range(nwords):
-            bits += [1, 1, 1, 1, 0, 0, 1, 0] + [int(v) for v in rng.integers(0, 2, 39)]
-        bits += [1] * 2
-        return fsk_audio(bits, float(m.sample_rate) / float(m.data_rate), float(m.mark_f), float(m.space_f),
-                         m.sample_rate, amplitude)
-    words = rng.integers(0, 1 << m.n_data_bits, nwords, dtype=np.uint64).astype(np.uint32)
-    return orc.tx_words(m, words, amplitude, 4096, True)
-
-
-def random_pair(rng, bw, nbands):
-    """independent mark and space bands, either order, at least two bands apart; each tone up to 0.3 band
-    off its band's centre"""
-    while True:
-        bm, bs = (int(v) for v in rng.integers(2, nbands - 2, 2))
-        if abs(bm - bs) >= 2:
-            break
-    return float(f32((bm + rng.uniform(-0.3, 0.3)) * bw)), float(f32((bs + rng.uniform(-0.3, 0.3)) * bw))
-
-
-def lay_out(rng, m, audio, sigma):
-    lead = np.zeros(int(rng.integers(0, 3 * m.derived().frame_nsamples)), np.float32)
-    tail = np.zeros(int(rng.integers(0, m.derived().frame_nsamples)), np.float32)
-    x = np.concatenate([lead, audio, tail])
-    return (x + f32(sigma) * rng.standard_normal(x.size).astype(np.float32)).astype(np.float32), lead.size
 
 
 _CASES = {}
@@ -272,30 +168,11 @@ def random_case(mode, rate):
 
 def run_tones(eng, buf, n, lens, bands, states=None, max_frames=None):
     t = torch()
-    frames, st = eng.rx_batch_tones(t.from_numpy(buf).to(dev()), bands, nsamples=n,
-                                    nsamples_each=t.from_numpy(np.asarray(lens, np.int32)).to(dev()),
+    frames, st = eng.rx_batch_tones(upload(buf), bands, nsamples=n,
+                                    nsamples_each=upload(np.asarray(lens, np.int32)),
                                     states=states, max_frames=max_frames)
     sync()
     return frames, st
-
-
-def state_rows(st):
-    return torch().from_numpy(st.view(np.int32).reshape(len(st), -1).copy()).to(dev())
-
-
-def check_against_oracle(screened, fr, st, what):
-    import test_gpu_parity as T
-    nok = 0
-    for s, (w, robust) in enumerate(screened):
-        recs = fr[s, :int(st["nframes"][s])]
-        got = T.as_oracle_frames(recs)
-        if not robust:
-            assert abs(len(got) - len(w["frames"])) <= 1, (what, s, len(got), len(w["frames"]))
-            continue
-        nok += 1
-        T.compare_frames(got, w["frames"], "%s stream %d" % (what, s))
-        T.compare_reports(T.reports_of(recs, st[s]), w["reports"], "%s stream %d" % (what, s))
-    assert 2 * nok >= len(screened), (what, "screened out", len(screened) - nok)
 
 
 # --------------------------------------------------------------------------
@@ -344,12 +221,11 @@ def test_reference_vectors_each_on_its_own_pair_in_one_call():
     out, cnt = out.cpu().numpy(), cnt.cpu().numpy()
     fr, st = mm().frames_to_numpy(frames), mm().states_to_numpy(states)
     assert (st["done"] == 1).all()
-    import test_gpu_parity as T
     for s, name in enumerate(VECTORS):
         case, g, _ = vector_audio(name)
         _, rx = gu.modes(case)
         assert out[s, :cnt[s]].tobytes() == bytes(g["stdout"]), name
-        lines = [orc.report_line(rx, r) for r in T.reports_of(fr[s, :int(st["nframes"][s])], st[s])]
+        lines = [orc.report_line(rx, r) for r in reports_of(fr[s, :int(st["nframes"][s])], st[s])]
         want = gu.stat_lines(g)
         assert len(lines) >= len(want) >= 1, (name, lines, want)
         for x, y in zip(lines, want):
@@ -447,7 +323,7 @@ def test_the_engine_pair_gives_the_fixed_tone_records(key, monkeypatch):
     lens = np.array([a.size for a in streams], np.int32)
     fa, sa = run_tones(eng, buf, n, lens, bands)
     t = torch()
-    fb, sb = fixed.rx_batch(t.from_numpy(buf).to(dev()), nsamples=n, nsamples_each=t.from_numpy(lens).to(dev()))
+    fb, sb = fixed.rx_batch(upload(buf), nsamples=n, nsamples_each=upload(lens))
     sync()
     G, W, L = key
     assert fixed.last_kernel().startswith("k_rx<G=%d,W=%d,L=%d,mode=0(per-candidate)" % (G, W, L)), fixed.last_kernel()
@@ -459,41 +335,11 @@ def test_the_engine_pair_gives_the_fixed_tone_records(key, monkeypatch):
         assert k >= 3 and fa[s, :k].tobytes() == fb[s, :k].tobytes(), (key, s)
 
 
-# --------------------------------------------------------------------------
-# Bell103 full duplex
-# --------------------------------------------------------------------------
-ORIGINATE, ANSWER = (1270.0, 1070.0), (2225.0, 2025.0)
-
-
-def duplex_case():
-    if "duplex" in _CASES:
-        return _CASES["duplex"]
-    rng = np.random.default_rng(103)
-    mo, ma = on_pair("300", 48000, *ORIGINATE), on_pair("300", 48000, *ANSWER)
-    streams, pairs = [], []
-    for s in range(6):
-        m = mo if s % 2 == 0 else ma
-        x, _ = lay_out(rng, m, transmission(rng, m, int(rng.integers(5, 9)), float(rng.uniform(0.3, 1.0))), 1e-3)
-        streams.append(x)
-        pairs.append(ORIGINATE if s % 2 == 0 else ANSWER)
-    # one line carrying both directions at once, given twice: once with each pair
-    a, b = transmission(rng, mo, 8, 0.5), transmission(rng, ma, 8, 0.5)
-    both = np.zeros(max(a.size, b.size) + 2000, np.float32)
-    both[1000:1000 + a.size] += a
-    both[1500:1500 + b.size] += b
-    streams += [both, both]
-    pairs += [ORIGINATE, ANSWER]
-    want = [orc.rx_run(on_pair("300", 48000, *p), x, literal=False) for x, p in zip(streams, pairs)]
-    _CASES["duplex"] = (streams, pairs, want)
-    return _CASES["duplex"]
-
-
 @pytest.mark.gpu
 def test_bell103_originate_and_answer_in_one_call():
     """Bell103 originate (1270/1070 Hz) and answer (2225/2025 Hz) streams in one call give the oracle's
     records on their pairs; a line carrying both directions summed, given once with each pair, gives both
     texts as the oracle decodes them."""
-    import test_gpu_parity as T
     streams, pairs, want = duplex_case()
     eng = mm().RxEngine.for_mode("300", 48000)
     bands = eng.tone_bands([p[0] for p in pairs], [p[1] for p in pairs], device=dev())
@@ -507,7 +353,7 @@ def test_bell103_originate_and_answer_in_one_call():
     rx = orc.Mode("300", sample_rate=48000)
     for s, w in enumerate(want):
         recs = fr[s, :int(st["nframes"][s])]
-        T.compare_frames(T.as_oracle_frames(recs), w["frames"], "duplex stream %d" % s)
+        compare_frames(as_oracle_frames(recs), w["frames"], "duplex stream %d" % s)
         text = orc.decode_records(rx, "ascii8", orc.frame_records(w["frames"]))
         assert len(text) >= 5 and out[s, :cnt[s]].tobytes() == text, s
     assert out[6, :cnt[6]].tobytes() != out[7, :cnt[7]].tobytes()
@@ -535,8 +381,8 @@ def test_a_stream_without_a_valid_pair_is_skipped():
         st0["pos"][1], st0["carrier"][1], st0["track_amplitude"][1], st0["nframes"][1] = 1234, 1, 0.5, 2
         states = state_rows(st0)
         frames = t.full((3, eng.max_frames(n), 5), 0x5A5A5A5A, dtype=t.int32).to(dev())
-        frames, sb = eng.rx_batch_tones(t.from_numpy(buf).to(dev()), bands, nsamples=n, states=states,
-                                        frames=frames, nsamples_each=t.from_numpy(np.array(lens, np.int32)).to(dev()))
+        frames, sb = eng.rx_batch_tones(upload(buf), bands, nsamples=n, states=states,
+                                        frames=frames, nsamples_each=upload(np.array(lens, np.int32)))
         sync()
         sb = mm().states_to_numpy(sb)
         assert sb[1].tobytes() == st0[1].tobytes(), bad
@@ -623,7 +469,7 @@ def test_a_new_pair_takes_effect_at_the_call_position(monkeypatch):
     s1["nframes"][:] = 0
     f2, s2 = run_tones(eng, buf, n, [x.size] * 2, ba, states=state_rows(s1))
     fixed = fixed_per_candidate(monkeypatch, "300", 48000, f_mark=ANSWER[0], f_space=ANSWER[1])
-    f3, s3 = fixed.rx_batch(t.from_numpy(buf).to(dev()), nsamples=n, states=state_rows(s1))
+    f3, s3 = fixed.rx_batch(upload(buf), nsamples=n, states=state_rows(s1))
     sync()
     s2, s3 = mm().states_to_numpy(s2), mm().states_to_numpy(s3)
     assert s2.tobytes() == s3.tobytes()
@@ -670,7 +516,7 @@ def test_live_receiver_with_tones_does_not_depend_on_the_cut():
             chunk = np.zeros((len(streams), max_chunk), np.float32)
             for s in range(len(streams)):
                 chunk[s, :k[s]] = buf[s, fed[s]:fed[s] + k[s]]
-            texts = take(lr.feed(t.from_numpy(chunk).to(dev()), t.from_numpy(k.astype(np.int32)).to(dev())))
+            texts = take(lr.feed(upload(chunk), upload(k.astype(np.int32))))
             fed += k
         texts = take(lr.finish())
         assert texts == whole, max_chunk

@@ -14,27 +14,10 @@ import pytest
 
 import minimodem_b200 as mm
 import orc
+from gpudev import dev, emulated, sync, upload
 import txorc
 
 torch = pytest.importorskip("torch")
-
-
-def dev():
-    import conftest
-    if conftest.EMU_DEVICE is not None:
-        return conftest.EMU_DEVICE
-    assert torch.cuda.is_available(), "GPU tests need a CUDA device"
-    return torch.device("cuda:0")
-
-
-def emulated():
-    import conftest
-    return conftest.EMU_DEVICE is not None
-
-
-def sync():
-    if not emulated():
-        torch.cuda.synchronize()
 
 
 def text_rows(texts):
@@ -42,7 +25,7 @@ def text_rows(texts):
     buf = np.zeros((len(texts), stride), np.uint8)
     for i, t in enumerate(texts):
         buf[i, :len(t)] = np.frombuffer(bytes(t), np.uint8)
-    return torch.from_numpy(buf).to(dev()), torch.tensor([len(t) for t in texts], dtype=torch.int32).to(dev())
+    return upload(buf), torch.tensor([len(t) for t in texts], dtype=torch.int32).to(dev())
 
 
 def expected(te, text, lens, tones, lead, k, nout):
@@ -99,7 +82,7 @@ def test_rows_are_the_sum_of_their_channels(fmt, align, lut):
             pos = [0, k // 2, k - 1, None][r % 4]
             if pos is not None and k > 1 or (k == 1 and r % 4 == 0):
                 spaces[r * k + pos] = BAD[r % len(BAD)]
-        tones = torch.from_numpy(np.stack([marks, spaces], axis=1)).to(dev())
+        tones = upload(np.stack([marks, spaces], axis=1))
         full = te.max_samples(maxlen, mm.TX_FINAL)
         nout = int(rng.integers(full // 3, full + 1)) | (1 if align == "odd-stride" else 0)
         lead = rng.integers(0, nout // 2, n).astype(np.int32)
@@ -110,7 +93,7 @@ def test_rows_are_the_sum_of_their_channels(fmt, align, lut):
         sentinel = -5.5 if float_samples else -555
         out = torch.full((nrows, stride), sentinel, dtype=torch.float32 if float_samples else torch.int16, device=dev())
         assert (out.data_ptr() % 16 == 0 and stride * out.element_size() % 16 == 0) == (align == "aligned")
-        lead_t = torch.from_numpy(lead).to(dev())
+        lead_t = upload(lead)
         _, cnt = te.text_channels(text, lens, tones, k, nout, lead_in=lead_t, out=out)
         sync()
         want, want_len = expected(te, text, lens, tones, lead, k, nout)
@@ -132,7 +115,7 @@ def test_int16_rows_saturate_the_exact_sum():
     text, lens = text_rows(texts)
     pairs = np.tile(np.array([[1200.0, 2200.0]], np.float32), (k * nrows, 1))
     pairs[k + 2] = [2200.0, 1200.0]                     # row 1: one channel with the tones swapped
-    tones = torch.from_numpy(pairs).to(dev())
+    tones = upload(pairs)
     nout = te.max_samples(len(texts[0]), mm.TX_FINAL)
     lead = np.zeros(k * nrows, np.int32)
     rows, _ = te.text_channels(text, lens, tones, k, nout)
@@ -199,14 +182,14 @@ def test_mixed_rows_decode_back(case, fmt):
     s = np.tile(np.array(spaces, np.float32), nrows)
     if case == "rtty-passband":
         s[[r * k + k - 1 for r in range(1, nrows, 2)]] = np.nan
-    tones = torch.from_numpy(np.stack([m, s], axis=1)).to(dev())
-    lead = torch.from_numpy(rng.integers(0, rate // 4, n).astype(np.int32)).to(dev())
+    tones = upload(np.stack([m, s], axis=1))
+    lead = upload(rng.integers(0, rate // 4, n).astype(np.int32))
     nout = te.max_samples(text.shape[1], mm.TX_FINAL) + rate // 4 + rate // 2
     rows, _ = te.text_channels(text, lens, tones, k, nout, lead_in=lead)
     rx = mm.RxEngine.for_mode(mode, rate)
     disabled = ~np.isfinite(s)
     bands = rx.tone_bands(m, np.where(disabled, m + 170.0, s), device=dev())
-    bands[torch.from_numpy(disabled).to(dev())] = rx.params.nbands      # disabled on the receive side too
+    bands[upload(disabled)] = rx.params.nbands      # disabled on the receive side too
     kind = mm.decoder_for_mode(mode, rx.params.n_data_bits)
     frames, states = rx.rx_batch_tones(rows, bands, channels_per_row=k)
     out, cnt = rx.decode_batch(kind, frames, states)
@@ -275,6 +258,6 @@ def test_errors_launch_nothing():
 # ---- CPU: the gpu tests above on the emulated kernel -------------------------------------------------------------
 def test_tx_channels_gpu_tests_on_the_emulated_kernel():
     """This file's gpu tests against the emulation build of the same kernel source, at reduced sizes."""
-    from test_emu_parity import run_emulated
+    from gpudev import run_emulated
     tail = run_emulated("", "late", 1500, module="test_gpu_tx_channels.py")
     assert " passed" in tail and "failed" not in tail

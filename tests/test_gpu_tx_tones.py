@@ -16,29 +16,12 @@ import pytest
 
 import minimodem_b200 as mm
 import orc
+from gpudev import dev, emulated, sync, upload
 import txorc
 
 torch = pytest.importorskip("torch")
 
 F32 = np.float32
-
-
-def dev():
-    import conftest
-    if conftest.EMU_DEVICE is not None:
-        return conftest.EMU_DEVICE
-    assert torch.cuda.is_available(), "GPU tests need a CUDA device"
-    return torch.device("cuda:0")
-
-
-def emulated():
-    import conftest
-    return conftest.EMU_DEVICE is not None
-
-
-def sync():
-    if not emulated():
-        torch.cuda.synchronize()
 
 
 NAMES = dict(mark="f_mark", space="f_space", startbits="nstartbits", stopbits="nstopbits")
@@ -103,7 +86,7 @@ def text_rows(texts, stride=None):
     for i, t in enumerate(texts):
         buf[i, :len(t)] = np.frombuffer(bytes(t), np.uint8)
     lens = torch.tensor([len(t) for t in texts], dtype=torch.int32).to(dev())
-    return torch.from_numpy(buf).to(dev()), lens
+    return upload(buf), lens
 
 
 def as_f32(a):
@@ -439,6 +422,6 @@ def test_tx_oracle_matches_the_reference_cli_at_random_pairs(flt, tmp_path):
 # ---- 7. CPU: the gpu tests above on the emulated kernel ---------------------------------------------------------
 def test_tx_tones_gpu_tests_on_the_emulated_kernel():
     """This file's gpu tests against the emulation build of the same kernel source, at reduced sizes."""
-    from test_emu_parity import run_emulated
+    from gpudev import run_emulated
     tail = run_emulated("", "late", 1500, module="test_gpu_tx_tones.py")
     assert " passed" in tail and "failed" not in tail

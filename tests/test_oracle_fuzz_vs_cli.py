@@ -14,54 +14,12 @@ import pytest
 
 import golden_util as gu
 import orc
+from clicases import random_invocation
 
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden"))
 from make_golden import read_wav  # noqa: E402
 
 pytestmark = pytest.mark.ref
-
-
-def random_invocation(rng):
-    while True:
-        baud = int(rng.choice([75, 110, 150, 300, 600, 1200, 2400, 4800]))
-        rate = int(rng.choice([8000, 11025, 16000, 22050, 44100, 48000]))
-        if not (6 <= rate / baud <= 700):
-            continue
-        args, kw = [str(baud), "--samplerate", str(rate)], dict(sample_rate=rate)
-        if rng.random() < 0.3:
-            args = ["-7"] + args
-            kw["n_data_bits"] = 7
-        if rng.random() < 0.4:
-            sb = int(rng.choice([1, 2, 3]))
-            args += ["--startbits", str(sb)]
-            kw["startbits"] = sb
-        if rng.random() < 0.5:
-            st = float(rng.choice([1.0, 1.5, 2.0]))
-            args += ["--stopbits", str(st)]
-            kw["stopbits"] = st
-        for flag, key in (("--msb-first", "msb_first"), ("--invert-start-stop", "invert_start_stop"),
-                          ("--inverted", "inverted")):
-            if rng.random() < 0.25:
-                args.append(flag)
-                kw[key] = True
-        if rng.random() < 0.3 and baud >= 400:
-            mark = float(rng.choice([1000, 1300, 1500, 1800]))
-            space = mark + float(rng.choice([400, 600, 1000]))
-            if space < rate / 2 - 300:
-                args += ["-M", str(mark), "-S", str(space)]
-                kw["mark"], kw["space"] = mark, space
-        flt = rng.random() < 0.3
-        vol = float(rng.choice([1.0, 0.5, 0.1]))
-        tx = args + (["--float-samples"] if flt else []) + (["--volume", str(vol)] if vol != 1.0 else [])
-        try:
-            m = orc.Mode(str(baud), **kw)
-            m.derived()
-            orc.Plan(m.sample_rate, m.mark_f, m.space_f, m.band_width)
-        except Exception:
-            continue
-        if m.frame_n_bits > 12:            # longer frames hit the reference's ring limit (DESIGN.md 5, item 2)
-            continue
-        return str(baud), kw, tx, args, flt, vol
 
 
 @pytest.mark.parametrize("seed", range(60))

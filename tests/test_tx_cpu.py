@@ -13,7 +13,7 @@ import golden_util as gu
 import orc
 import refcases
 import txorc
-from test_emu_parity import run_emulated
+from gpudev import run_emulated
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 CASES = refcases.EVERY + refcases.MORE

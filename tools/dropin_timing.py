@@ -6,11 +6,11 @@ import os, subprocess, sys, tempfile, time
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT); sys.path.insert(0, os.path.join(ROOT, "tests"))
 import golden_util as gu, refcases, orc
-import test_gpu_parity as T
+from clicases import write_wav
 case = refcases.BY_NAME["01-self-test-1200"]
 g = gu.load(case["name"]); a = gu.audio(case, g)
 d = tempfile.mkdtemp(); wav = os.path.join(d, "x.wav")
-T._write_wav(wav, a, int(g["audio_len"][1]), bool(g["audio_len"][2]))
+write_wav(wav, a, int(g["audio_len"][1]), bool(g["audio_len"][2]))
 out = {}
 for name in ("minimodem_ref", "minimodem_dropin"):
     exe = os.path.join(os.path.dirname(orc.LIBREF), name)
