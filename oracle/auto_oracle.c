@@ -13,10 +13,25 @@
  *                   count v that follows the reference's fill (DESIGN.md section 5): at the loop top
  *                   v = advance >= v ? 0 : v - advance, then, while v < S/2, v grows by
  *                   min(S/2, samples left after pos + v).
- * Every record carries the mark band it was decoded on.  Built by tests/autoorc.py; nothing in the
- * product links it.
+ * Every record carries the mark band it was decoded on, and on request every scan is logged (where, which
+ * window decided, the band, none / accepted / rejected, and why the loop scanned).  Built by
+ * tests/autoorc.py; nothing in the product links it.
  */
 #include "fsk_oracle.c"
+
+/* one carrier scan (:1181-1220) */
+enum { ORC_SCAN_NONE = 0, ORC_SCAN_ACCEPTED = 1, ORC_SCAN_REJECTED = 2 };	/* outcome */
+enum { ORC_SCAN_START = 0, ORC_SCAN_AGAIN = 1, ORC_SCAN_AFTER_DROP = 2, ORC_SCAN_AFTER_STRIKE = 3 }; /* cause */
+typedef struct {
+    unsigned long long pos;	/* the loop's position */
+    unsigned long long nvalid;	/* the samples from pos on that the loop holds */
+    int window;			/* the window that found a band; for none, the number of windows scanned */
+    int band;			/* the band found, or -1 */
+    int outcome;
+    int cause;			/* the first scan, one after a scan without a band, after a carrier drop, or
+				 * after a strike past the 20th without a carrier */
+    unsigned nframes, nreports;	/* records before the scan */
+} orc_auto_scan;
 
 typedef struct {
     unsigned *frame_band;	/* [nframes] of the orc_rx_result */
@@ -26,6 +41,32 @@ typedef struct {
      * magnitudes, and between its largest and the threshold (a screen for near-ties) */
     float min_margin;
 } orc_auto_bands;
+
+/* the optional scan log of orc_rx_run_auto_log (kept out of orc_auto_bands, whose layout its callers share) */
+typedef struct {
+    orc_auto_scan *scans;	/* [nscans] */
+    size_t nscans, cap;
+} orc_auto_scan_log;
+
+static int auto_log(orc_auto_scan_log *l, const orc_auto_scan *e)
+{
+    if (l->nscans >= l->cap) {
+	size_t c = l->cap ? l->cap * 2 : 256;
+	orc_auto_scan *p = realloc(l->scans, c * sizeof(*p));
+	if (!p)
+	    return -1;
+	l->scans = p;
+	l->cap = c;
+    }
+    l->scans[l->nscans++] = *e;
+    return 0;
+}
+
+void orc_auto_scan_log_free(orc_auto_scan_log *l)
+{
+    free(l->scans);
+    memset(l, 0, sizeof(*l));
+}
 
 static int auto_push(unsigned **arr, size_t *cap, size_t n, unsigned v)
 {
@@ -102,10 +143,11 @@ int orc_auto_b_shift(float band_width, int autodetect_shift, int inverted)
 /* orc_rx_run (fsk_oracle.c) with carrier_autodetect_threshold = threshold > 0, without --Xrxnoise or
  * call records.  find_frame (NULL: orc_find_frame) is called with ctx = the loop's orc_plan, whose
  * b_mark / b_space are the tones of the moment (the near-tie screen of tests/autoorc.py reads them).
- * res must be zero-initialised before its first use, as there. */
-int orc_rx_run_auto(const orc_rx_config *cfg, const float *samples, size_t nsamples, int mode,
+ * res and bands must be zero-initialised before their first use, as there; so must log, which (when not
+ * NULL) receives every scan. */
+int orc_rx_run_auto_log(const orc_rx_config *cfg, const float *samples, size_t nsamples, int mode,
 	float threshold, int autodetect_shift, int inverted, orc_find_frame_fn find_frame,
-	orc_rx_result *res, orc_auto_bands *bands)
+	orc_rx_result *res, orc_auto_bands *bands, orc_auto_scan_log *log)
 {
     if (!find_frame)
 	find_frame = default_find_frame;
@@ -114,6 +156,8 @@ int orc_rx_run_auto(const orc_rx_config *cfg, const float *samples, size_t nsamp
     res->nframes = res->nreports = res->ncalls = 0;
     res->n_find_frame_calls = 0;
     bands->min_margin = INFINITY;
+    if (log)
+	log->nscans = 0;
     orc_rx_derive(cfg, &d);
     if (d.expect_n_bits == 0 || d.expect_n_bits > 64 || !(threshold > 0.0f))
 	return -1;
@@ -149,6 +193,7 @@ int orc_rx_run_auto(const orc_rx_config *cfg, const float *samples, size_t nsamp
     size_t nf = 0, nr = 0;
 
     int carrier_band = -1;				/* :1180 */
+    int scan_cause = ORC_SCAN_START;
     int carrier = 0;
     float confidence_total = 0, amplitude_total = 0;
     unsigned nframes_decoded = 0;
@@ -214,9 +259,18 @@ int orc_rx_run_auto(const orc_rx_config *cfg, const float *samples, size_t nsamp
 	    advance = i + nsamples_per_scan;
 	    if (advance > scan_n)
 		advance = scan_n;
+	    int b_space = carrier_band + b_shift;
+	    if (log) {
+		orc_auto_scan e = { pos, nvalid, (int)(i / (unsigned)nsamples_per_scan), carrier_band,
+		    carrier_band < 0 ? ORC_SCAN_NONE
+			    : b_space < 1 || b_space >= (int)plan.nbands ? ORC_SCAN_REJECTED : ORC_SCAN_ACCEPTED,
+		    scan_cause, (unsigned)res->nframes, (unsigned)res->nreports };
+		if (auto_log(log, &e))
+		    rc = -1;
+	    }
+	    scan_cause = ORC_SCAN_AGAIN;
 	    if (carrier_band < 0)
 		continue;
-	    int b_space = carrier_band + b_shift;
 	    if (b_space < 1 || b_space >= (int)plan.nbands) {
 		carrier_band = -1;
 		continue;
@@ -274,6 +328,7 @@ int orc_rx_run_auto(const orc_rx_config *cfg, const float *samples, size_t nsamp
 	if (confidence <= cfg->confidence_threshold) {
 	    if (++noconfidence > 20) {
 		carrier_band = -1;				/* :1297 */
+		scan_cause = carrier ? ORC_SCAN_AFTER_DROP : ORC_SCAN_AFTER_STRIKE;
 		if (carrier) {
 		    orc_rx_report rp = { nframes_decoded, carrier_nsamples,
 			confidence_total, amplitude_total, (unsigned)res->nframes };
@@ -347,4 +402,13 @@ int orc_rx_run_auto(const orc_rx_config *cfg, const float *samples, size_t nsamp
     free(scratch);
     free(cs);
     return rc;
+}
+
+/* orc_rx_run_auto_log without the scan log */
+int orc_rx_run_auto(const orc_rx_config *cfg, const float *samples, size_t nsamples, int mode,
+	float threshold, int autodetect_shift, int inverted, orc_find_frame_fn find_frame,
+	orc_rx_result *res, orc_auto_bands *bands)
+{
+    return orc_rx_run_auto_log(cfg, samples, nsamples, mode, threshold, autodetect_shift, inverted, find_frame,
+	    res, bands, NULL);
 }

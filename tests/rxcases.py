@@ -185,26 +185,37 @@ def duplex_case():
     return _DUPLEX[0]
 
 
-def tone_stream(rng, m, b_shift, nbands, nwords):
-    """One transmission of random data words on a random tone pair of this mode's band grid, the mark
-    tone off its band centre by up to 0.3 band.  UIC frames (the expect string 11110010 and 39 data bits,
-    no start or stop bits) come from fsk_audio after a mark leader; everything else from the oracle's
-    transmitter."""
+def tone_mark(rng, m, b_shift, nbands):
+    """a random mark tone of this mode's band grid whose space band (b_shift away) lies inside it, off its band
+    centre by up to 0.3 band"""
     bw = float(m.band_width)
     lo, hi = max(2, 2 - b_shift), min(nbands - 3, nbands - 3 - b_shift)
     bm = int(rng.integers(lo, max(lo + 1, hi)))
-    mark = float(bm * bw + rng.uniform(-0.3, 0.3) * bw)
-    amplitude = float(rng.uniform(0.3, 1.0))
+    return float(bm * bw + rng.uniform(-0.3, 0.3) * bw)
+
+
+def tone_burst(rng, m, mark, b_shift, nwords, amplitude, space=None):
+    """nwords random data words on (mark, space = mark + b_shift bands).  UIC frames (the expect string
+    11110010 and 39 data bits, no start or stop bits) come from fsk_audio after a mark leader; everything
+    else from the oracle's transmitter."""
+    space = mark + b_shift * float(m.band_width) if space is None else space
     if m.expect_data_string is not None:
         bits = [1] * 10
         for _ in range(nwords):
             bits += [1, 1, 1, 1, 0, 0, 1, 0] + [int(v) for v in rng.integers(0, 2, 39)]
         bits += [1] * 2
-        return fsk_audio(bits, float(m.sample_rate) / float(m.data_rate), mark, mark + b_shift * bw,
-                         m.sample_rate, amplitude)
-    tx = orc.Mode(m.mode, sample_rate=m.sample_rate, mark=mark, space=mark + b_shift * bw)
+        return fsk_audio(bits, float(m.sample_rate) / float(m.data_rate), mark, space, m.sample_rate, amplitude)
+    tx = orc.Mode(m.mode, sample_rate=m.sample_rate, mark=mark, space=space)
+    tx.do_tx_sync_bytes = min(tx.do_tx_sync_bytes, m.do_tx_sync_bytes)
     words = rng.integers(0, 1 << m.n_data_bits, nwords, dtype=np.uint64).astype(np.uint32)
     return orc.tx_words(tx, words, amplitude, 4096, True)
+
+
+def tone_stream(rng, m, b_shift, nbands, nwords):
+    """One transmission of random data words on a random tone pair of this mode's band grid (tone_mark,
+    tone_burst)."""
+    mark = tone_mark(rng, m, b_shift, nbands)
+    return tone_burst(rng, m, mark, b_shift, nwords, float(rng.uniform(0.3, 1.0)))
 
 
 # ---------------------------------------------------------------------------------------------------
@@ -371,34 +382,55 @@ def shape_case(fam, which):
 
 
 SIGMA_BG = 0.003
+# the auto call's background: a gap stays silent to the carrier scan (at 0.003 a scan window's largest band
+# sits near the 0.001 threshold, and a gap turns into a run of threshold near-ties)
+SIGMA_BG_AUTO = 1e-4
 NOISE_SIGMAS = (0.05, 0.2, 0.5)
 NSTREAMS = 8
 KINDS = ("burst", "gap", "noise", "fade", "sag", "cut")
+# the auto call's own: a burst on one pair followed directly by one on another pair, and a burst whose space
+# band lies outside the band grid (the scan finds it and rejects it)
+AUTO_KINDS = ("retune", "low")
 
 
-def session_stream(rng, m, end_in_gap):
+def session_stream(rng, m, end_in_gap, auto=None):
     """(samples, noise-only ranges [(start, end)]): every kind of segment once (noise twice) and up to two more, in
-    random order, under sigma = 0.003 background"""
+    random order, under sigma = 0.003 background.  auto = (b_shift, nbands): the auto call's stream -- every
+    burst on its own random pair of the band grid, the AUTO_KINDS too, sigma = 1e-4 background."""
     spb = float(m.derived().nsamples_per_bit)
     words = lambda k: rng.integers(0, 1 << m.n_data_bits, k, dtype=np.uint64).astype(np.uint32)
     # a burst of 3..10 frames; SAME's counts its one sync byte (the transmitter's preamble is 16 of them)
     tm = copy.copy(m)
     tm.do_tx_sync_bytes = min(m.do_tx_sync_bytes, 1)
-    burst = lambda amp: orc.tx_words(tm, words(int(rng.integers(3, 11)) - tm.do_tx_sync_bytes), amp, 4096, True)
+    if auto is None:
+        burst = lambda amp: orc.tx_words(tm, words(int(rng.integers(3, 11)) - tm.do_tx_sync_bytes), amp, 4096, True)
+        kinds = KINDS + ("noise",)
+    else:
+        bs, nb = auto
+        pair_burst = lambda mark, amp: tone_burst(rng, tm, mark, bs, int(rng.integers(3, 11)) - tm.do_tx_sync_bytes,
+                                                  amp)
+        burst = lambda amp: pair_burst(tone_mark(rng, m, bs, nb), amp)
+        kinds = KINDS + ("noise",) + AUTO_KINDS
     parts, noise, at = [], [], 0
-    kinds = list(rng.permutation(KINDS + ("noise",))) + list(rng.choice(KINDS, int(rng.integers(0, 3))))
+    kinds = list(rng.permutation(kinds)) + list(rng.choice(KINDS, int(rng.integers(0, 3))))
     kinds.append("gap" if end_in_gap else "burst")
     for kind in kinds:
         amp = float(rng.uniform(0.2, 1.0))
         if kind == "gap":
             a = np.zeros(int(rng.uniform(1, 60) * spb), np.float32)
         elif kind == "noise":           # long enough to acquire a false carrier in every preset's case; longer
-            # ones pile up near-ties of the threshold and the search limit on noise candidates
-            a = (float(rng.choice(NOISE_SIGMAS)) * rng.standard_normal(int(rng.uniform(20, 120) * spb))).astype(np.float32)
+            # ones pile up near-ties of the threshold and the search limit on noise candidates (the auto call's
+            # at most 60 bits: every strike there rescans, and 120 screened out more than one stream in ten)
+            a = (float(rng.choice(NOISE_SIGMAS)) * rng.standard_normal(int(rng.uniform(20, 120 if auto is None else 60)
+                                                                           * spb))).astype(np.float32)
             noise.append((at, at + a.size))
         elif kind == "fade":            # squelched at 1/8..1/5 of the level, held at 1/3
             ratio = float(rng.uniform(1 / 8, 1 / 5)) if rng.random() < 0.6 else 1 / 3
-            a = np.concatenate([burst(amp), burst(amp * ratio)])
+            if auto is None:
+                a = np.concatenate([burst(amp), burst(amp * ratio)])
+            else:                       # on one pair
+                mark = tone_mark(rng, m, bs, nb)
+                a = np.concatenate([pair_burst(mark, amp), pair_burst(mark, amp * ratio)])
         elif kind == "sag":             # a noise burst at the signal's level inside a running burst
             a = burst(amp)
             n = int(rng.uniform(2, 6) * spb)
@@ -407,18 +439,40 @@ def session_stream(rng, m, end_in_gap):
         elif kind == "cut":
             a = burst(amp)
             a = a[:int(rng.integers(a.size // 3, a.size))]
+        elif kind == "retune":
+            a = np.concatenate([burst(amp), burst(float(rng.uniform(0.2, 1.0)))])
+        elif kind == "low":             # the space band below band 1, or past the last band
+            bw = float(m.band_width)
+            bm = int(rng.integers(1, 1 - bs + 1)) if bs < 0 else int(rng.integers(nb - bs, nb - 1))
+            mark = float(bm * bw + rng.uniform(-0.3, 0.3) * bw)
+            space = min(max(mark + bs * bw, -mark), float(m.sample_rate) / 2 - bw)
+            a = tone_burst(rng, tm, mark, bs, int(rng.integers(3, 11)) - tm.do_tx_sync_bytes, amp, space=space)
         else:
             a = burst(amp)
         parts.append(a)
         at += a.size
     x = np.concatenate(parts)
-    return (x + f32(SIGMA_BG) * rng.standard_normal(x.size).astype(np.float32)).astype(np.float32), noise
+    sigma = SIGMA_BG if auto is None else SIGMA_BG_AUTO
+    return (x + f32(sigma) * rng.standard_normal(x.size).astype(np.float32)).astype(np.float32), noise
 
 
-def drops(m, x):
-    """carrier drops (session reports before the end of the stream) of the oracle on x"""
-    r = orc.rx_run(m, x, literal=False)
+def drops(m, x, auto=False, inverted=False):
+    """carrier drops (session reports before the end of the stream) of the oracle (the auto oracle) on x"""
+    r = autoorc.rx_run(m, x, inverted=inverted) if auto else orc.rx_run(m, x, literal=False)
     return len(r["reports"]) - (1 if r["reports"] and r["reports"][-1][4] == len(r["frames"]) else 0)
+
+
+def bisect_gap(make, dropped, hi):
+    """the two gap lengths one sample either side of the drop: (make(lo), make(lo + 1))"""
+    lo = 0
+    assert not dropped(0) and dropped(hi)
+    while hi - lo > 1:
+        mid = (lo + hi) // 2
+        if dropped(mid):
+            hi = mid
+        else:
+            lo = mid
+    return make(lo), make(hi)
 
 
 def boundary_streams(m, seed):
@@ -430,15 +484,32 @@ def boundary_streams(m, seed):
     hi = int(80 * float(m.derived().nsamples_per_bit))
     bg = (f32(SIGMA_BG) * rng.standard_normal(a.size + b.size + hi)).astype(np.float32)
     make = lambda gap: (np.concatenate([a, np.zeros(gap, np.float32), b]) + bg[:a.size + gap + b.size]).astype(np.float32)
-    lo = 0
-    assert drops(m, make(lo)) == 0 and drops(m, make(hi)) > 0
-    while hi - lo > 1:
-        mid = (lo + hi) // 2
-        if drops(m, make(mid)):
-            hi = mid
-        else:
-            lo = mid
-    return make(lo), make(hi)
+    return bisect_gap(make, lambda gap: drops(m, make(gap)) > 0, hi)
+
+
+def auto_drop_in_gap(m, x, gap_end, inverted=False):
+    """the auto oracle on x drops a carrier (the 21st strike) and rescans before sample gap_end"""
+    r = autoorc.rx_run(m, x, inverted=inverted, scans=True)
+    return any(e["cause"] == "after-drop" and e["pos"] <= gap_end for e in r["scans"])
+
+
+def auto_boundary_streams(m, b_shift, nbands, inverted, seed, same_pair):
+    """boundary_streams for the auto call, the second burst on the first one's pair or on another: the gaps one
+    sample either side of the one whose carrier drop comes before the second burst starts.  Returns the two
+    streams and where their gaps end."""
+    rng = np.random.default_rng(seed)
+    ma = tone_mark(rng, m, b_shift, nbands)
+    while True:
+        mb = ma if same_pair else tone_mark(rng, m, b_shift, nbands)
+        if same_pair or abs(mb - ma) > 2 * float(m.band_width):
+            break
+    a, b = tone_burst(rng, m, ma, b_shift, 4, 0.6), tone_burst(rng, m, mb, b_shift, 3, 0.6)
+    hi = int(80 * float(m.derived().nsamples_per_bit))
+    bg = (f32(SIGMA_BG_AUTO) * rng.standard_normal(a.size + b.size + hi)).astype(np.float32)
+    make = lambda gap: (np.concatenate([a, np.zeros(gap, np.float32), b]) + bg[:a.size + gap + b.size]).astype(np.float32)
+    short, past = bisect_gap(make, lambda gap: auto_drop_in_gap(m, make(gap), a.size + gap, inverted), hi)
+    gap = short.size - a.size - b.size
+    return short, past, a.size + gap, a.size + gap + 1
 
 
 class Case:
@@ -451,6 +522,8 @@ def session_case(f, which):
     and a preset (mode, rate) or "random"; computed once per (call, src, which)"""
     call = "tones" if f["call"] == "channels" else f["call"]
     key = (f["call"], f["src"], which) if which != "random" else (f["call"], f["src"], f["cls"], f["n"])
+    if f.get("inverted"):
+        key += ("inverted",)
     if key in _SESSION_CASES:
         return _SESSION_CASES[key]
     seed = key[:1] + key[2:]                    # int16 rows: the float streams, quantized
@@ -464,9 +537,15 @@ def session_case(f, which):
     else:
         c.mode, c.rate = which
         m = orc.Mode(c.mode, sample_rate=c.rate)
-        c.make = lambda: mm.RxEngine.for_mode(which[0], which[1])
+        inv = dict(inverted=True) if f.get("inverted") else {}
+        c.make = lambda: mm.RxEngine.for_mode(which[0], which[1], **inv)
     k = 2 if f["call"] == "channels" else 1
-    nch = NSTREAMS + 2 if k == 1 else 2 * (NSTREAMS // 2 + 2)
+    c.inverted = bool(f.get("inverted", False))
+    auto = None
+    if call == "auto":
+        p = mm.rx_params(mm.rx_config_for_mode(c.mode, c.rate))
+        auto = (autoorc.b_shift(m, c.inverted), int(p.nbands))
+    nch = NSTREAMS + (2 if auto is None else 4) if k == 1 else 2 * (NSTREAMS // 2 + 2)
     c.modes, c.hz, c.bands, c.noise, chans = [], [], [], [], []
     if call == "tones":
         p = mm.rx_params(mm.rx_config_for_mode(c.mode, c.rate))
@@ -480,14 +559,25 @@ def session_case(f, which):
             c.modes.append(tm)
     else:
         c.modes = [m] * nch
-    for j in range(nch):
-        chans.append(session_stream(rng, c.modes[j], j % 2 == 0))
-    # the boundary streams: channels 8 and 9 (k = 1), or alone on rows 4 and 5 (k = 2)
-    nb_at = [NSTREAMS, NSTREAMS + 1] if k == 1 else [NSTREAMS, NSTREAMS + 3]
-    short, _ = boundary_streams(c.modes[nb_at[0]], zlib.crc32(repr(seed).encode()))
-    _, past = boundary_streams(c.modes[nb_at[1]], zlib.crc32(repr(seed).encode()) + 1)
-    chans[nb_at[0]] = (short, [])
-    chans[nb_at[1]] = (past, [])
+    for j in range(NSTREAMS if auto else nch):
+        chans.append(session_stream(rng, c.modes[j], j % 2 == 0, auto))
+    if auto is not None:
+        # the boundary streams: channels 8, 9 (the second burst on the first one's pair) and 10, 11 (on another)
+        c.boundary, c.gap_end = [], {}
+        for same in (True, False):
+            short, past, e0, e1 = auto_boundary_streams(m, auto[0], auto[1], c.inverted,
+                                                        zlib.crc32(repr(seed).encode()) + same, same)
+            c.boundary += [(len(chans), 0), (len(chans) + 1, 1)]
+            c.gap_end.update({len(chans): e0, len(chans) + 1: e1})
+            chans += [(short, []), (past, [])]
+    else:
+        # the boundary streams: channels 8 and 9 (k = 1), or alone on rows 4 and 5 (k = 2)
+        nb_at = [NSTREAMS, NSTREAMS + 1] if k == 1 else [NSTREAMS, NSTREAMS + 3]
+        short, _ = boundary_streams(c.modes[nb_at[0]], zlib.crc32(repr(seed).encode()))
+        _, past = boundary_streams(c.modes[nb_at[1]], zlib.crc32(repr(seed).encode()) + 1)
+        chans[nb_at[0]] = (short, [])
+        chans[nb_at[1]] = (past, [])
+        c.boundary = [(nb_at[0], 0), (nb_at[1], 1)]
     if k == 2:
         for j in (NSTREAMS + 1, NSTREAMS + 2):      # the other channel of those rows carries nothing
             chans[j] = (np.zeros(1, np.float32), [])
@@ -504,8 +594,11 @@ def session_case(f, which):
     c.noise = [ch[1] for ch in chans]
     c.lens = np.array([x.size for x in c.rows], np.int32)
     c.row_of = [j // k for j in range(nch)]
-    c.screened = [tie_screen.screen(c.modes[j], c.rows[c.row_of[j]]) for j in range(nch)]
-    c.boundary = [(nb_at[0], 0), (nb_at[1], 1)]
+    c.auto = auto
+    if auto is None:
+        c.screened = [tie_screen.screen(c.modes[j], c.rows[c.row_of[j]]) for j in range(nch)]
+    else:
+        c.screened = [autoorc.screen(m, x, c.inverted) for x in c.rows]
     _SESSION_CASES[key] = c
     return c
 
@@ -603,6 +696,49 @@ def live_text(mode, rate, rows, pairs, k, auto, max_chunk, seed, cuts_at=(), pcm
         take(lr.feed(upload(chunk), upload(k_)))
     take(lr.finish())
     return texts
+
+
+def records_of(frames, states, bands):
+    """per stream: [(record bytes, band)] of the records an auto call wrote"""
+    fr, st, b = mm.frames_to_numpy(frames), mm.states_to_numpy(states), bands.cpu().numpy()
+    return [[(fr[s, i].tobytes(), int(b[s, i])) for i in range(int(st["nframes"][s]))] for s in range(len(st))]
+
+
+def live_records(eng, streams, cut, cuts_at=()):
+    """The live-stream recipe of include/fsk_b200.h with auto-carrier (eng: set_auto_carrier done):
+    fsk_b200_stream_push, then fsk_b200_rx_batch_auto with the auto holdback, chunk by chunk -- chunks of
+    `cut` samples, also cut at every sample of `cuts_at` --, the holdback off for the last call.  streams:
+    float32 or int16.  Returns every stream's records and bands in order."""
+    t = gpudev.torch()
+    window = eng.auto_stream_window()
+    eng.set_holdback(window)
+    stride = (window + eng.params.frame_nsamples + cut + 7) & ~7
+    max_frames = eng.max_frames(stride)
+    S = len(streams)
+    dt = t.int16 if streams[0].dtype == np.int16 else t.float32
+    buf, n = gpudev.rows(streams, streams[0].dtype, 8)
+    lens = np.array([len(a) for a in streams], np.int64)
+    z = lambda shape, d: t.zeros(shape, dtype=d).to(dev())
+    rows_, fill = z((S, stride), dt), z((S,), t.int32)
+    states, auto = z((S, mm.STATE_WORDS), t.int32), z((S, mm.AUTO_STATE_BYTES), t.uint8)
+    dropped = z((S,), t.int32)
+    got = [[] for _ in streams]
+
+    def step(chunk, valid):
+        mm.stream_push(rows_, fill, states, chunk, valid, dropped=dropped)
+        frames, _, _, bands = eng.rx_batch_auto(rows_, nsamples=stride, nsamples_each=fill, max_frames=max_frames,
+                                                states=states, auto_states=auto, rec_band=True)
+        sync()
+        for s, r in enumerate(records_of(frames, states, bands)):
+            got[s] += r
+    at = sorted(set(range(0, n, cut)) | {int(p) for p in cuts_at if 0 < p < n})
+    for o, e in zip(at, at[1:] + [n]):
+        w = e - o
+        step(upload(np.ascontiguousarray(buf[:, o:o + w])), upload(np.clip(lens - o, 0, w).astype(np.int32)))
+    eng.set_holdback(0)
+    step(z((S, 8), dt), 0)
+    assert int(dropped.cpu().numpy().sum()) == 0
+    return got
 
 
 # ---------------------------------------------------------------------------------------------------

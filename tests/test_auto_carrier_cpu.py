@@ -18,6 +18,7 @@ import autoorc
 import golden_util as gu
 import orc
 import refcases
+import rxcases
 
 # (mode, sample rates): the three preset classes of src/minimodem.c:900-934
 CLASSES = [("1200", (48000, 22050, 11025)), ("600", (48000, 8000)), ("300", (48000, 8000)),
@@ -65,6 +66,7 @@ def ring_limited(m):
 
 
 def random_case(seed, classes=CLASSES):
+    """(oracle mode, audio, rate, CLI arguments, inverted) of a random invocation"""
     rng = np.random.default_rng(7000 + seed)
     mode, rates = classes[int(rng.integers(len(classes)))]
     rate = int(rng.choice(rates))
@@ -100,29 +102,55 @@ def compare_lines(got, want, ctx):
         assert gu.close(float(fa[3].split("=")[1]), float(fb[3].split("=")[1]), 2e-3, cond=gu.CONF_COND)
 
 
+# the carrier-session streams of the auto call (tests/test_gpu_carrier_sessions.py): every AUTO_COMBOS preset,
+# and --inverted at 1200 baud
+SESSIONS = ["session:%s@%d" % w for w in sorted(set(rxcases.COVER.values()))] + ["session:1200@48000:inverted"]
+
+
+def session_preset(name):
+    """(mode, rate, inverted) of a SESSIONS name"""
+    mode, rest = name.split(":")[1].split("@")
+    return mode, int(rest), name.endswith(":inverted")
+
+
+def session_streams(name):
+    """(mode, audio, rate, rx_args, inverted) of every stream of a carrier-session case"""
+    import rxfam
+    mode, rate, inv = session_preset(name)
+    c = rxcases.session_case(dict(rxfam.FAMILIES["auto"], inverted=bool(inv)), (mode, rate))
+    rx_args = [mode, "--samplerate", str(rate), "-a"] + (["--inverted"] if inv else [])
+    return [(orc.Mode(mode, sample_rate=rate, inverted=bool(inv)), x, rate, rx_args, bool(inv)) for x in c.rows]
+
+
+def inputs(seed, classes=CLASSES):
+    return [random_case(seed, classes)] if isinstance(seed, int) else session_streams(seed)
+
+
 @pytest.mark.ref
-@pytest.mark.parametrize("seed", range(60))
+@pytest.mark.parametrize("seed", list(range(60)) + SESSIONS)
 def test_auto_oracle_matches_the_reference_cli(seed, tmp_path):
-    m, audio, rate, rx_args, inverted = random_case(seed)
-    wav = str(tmp_path / "x.wav")
-    write_wav_float(wav, audio, rate)
-    r = subprocess.run([orc.REF_CLI, "--rx", "--file", wav] + rx_args, stdout=subprocess.PIPE,
-                       stderr=subprocess.PIPE, check=True)
-    res = autoorc.rx_run(m, audio, literal=True, inverted=inverted)
-    assert orc.ref_decode(m, res["frames"]) == r.stdout, (rx_args, r.stdout[:60])
-    want = [ln.strip() for ln in r.stderr.decode().splitlines() if ln.startswith("### ")]
-    compare_lines(autoorc.stat_lines(m, res), want, rx_args)
+    """LITERAL prints what the CLI prints, on the random cases and the carrier-session streams"""
+    for m, audio, rate, rx_args, inverted in inputs(seed):
+        wav = str(tmp_path / "x.wav")
+        write_wav_float(wav, audio, rate)
+        r = subprocess.run([orc.REF_CLI, "--rx", "--file", wav] + rx_args, stdout=subprocess.PIPE,
+                           stderr=subprocess.PIPE, check=True)
+        res = autoorc.rx_run(m, audio, literal=True, inverted=inverted)
+        assert orc.ref_decode(m, res["frames"]) == r.stdout, (seed, rx_args, r.stdout[:60])
+        want = [ln.strip() for ln in r.stderr.decode().splitlines() if ln.startswith("### ")]
+        compare_lines(autoorc.stat_lines(m, res), want, (seed, rx_args))
 
 
-@pytest.mark.parametrize("seed", range(60))
+@pytest.mark.parametrize("seed", list(range(60)) + [s for s in SESSIONS if not ring_limited(
+    orc.Mode(session_preset(s)[0], sample_rate=session_preset(s)[1]))])
 def test_flat_auto_oracle_matches_literal(seed):
-    m, audio, rate, rx_args, inverted = random_case(seed, CLASSES[:2])
-    assert not ring_limited(m)
-    lit = autoorc.rx_run(m, audio, literal=True, inverted=inverted)
-    flat = autoorc.rx_run(m, audio, literal=False, inverted=inverted)
-    assert flat["frames"] == lit["frames"], rx_args
-    assert flat["reports"] == lit["reports"] and flat["frame_band"] == lit["frame_band"], rx_args
-    assert flat["report_band"] == lit["report_band"], rx_args
+    for m, audio, rate, rx_args, inverted in inputs(seed, CLASSES[:2]):
+        assert not ring_limited(m)
+        lit = autoorc.rx_run(m, audio, literal=True, inverted=inverted)
+        flat = autoorc.rx_run(m, audio, literal=False, inverted=inverted)
+        assert flat["frames"] == lit["frames"], (seed, rx_args)
+        assert flat["reports"] == lit["reports"] and flat["frame_band"] == lit["frame_band"], (seed, rx_args)
+        assert flat["report_band"] == lit["report_band"], (seed, rx_args)
 
 
 def test_the_cases_cover_every_path():
@@ -192,3 +220,64 @@ def test_the_auto_screen_replays_the_oracle_exactly():
         got = autoorc.rx_run(m, audio, inverted=inverted, find_frame=s.find_frame)
         for k in ("frames", "reports", "frame_band", "report_band"):
             assert got[k] == want[k], (rx_args, k)
+
+
+def test_the_auto_replay_reproduces_the_oracle_exactly():
+    """tie_screen.replay over the auto oracle's search calls (autoorc.calls) restates its frames and reports
+    bit for bit, on every random case (the carrier-session streams: test_every_case_reaches_every_loop_event)."""
+    import tie_screen
+    for seed in range(60):
+        m, audio, rate, rx_args, inverted = random_case(seed)
+        want = autoorc.rx_run(m, audio, inverted=inverted)
+        frames, reports, ties = tie_screen.replay(m, autoorc.calls(m, audio, inverted))
+        assert frames == [f[:5] for f in want["frames"]] and reports == want["reports"] and not ties, rx_args
+
+
+def _auto_fade(r):
+    """1200 baud under auto-carrier: a burst at 0.8, then with no gap one at 0.8 r, sigma = 1e-4; the scan takes
+    bands 5 and 9 (test_gpu_auto_carrier's test_a_stream_on_the_configured_tones_gives_the_fixed_tone_records),
+    so up to a drop the loop is the fixed-tone loop on 1000 / 1800 Hz"""
+    m = orc.Mode("1200")
+    rng = np.random.default_rng(5)
+    a = orc.tx_words(m, rng.integers(0, 256, 6).astype(np.uint32), 0.8, 4096, True)
+    b = orc.tx_words(m, rng.integers(0, 256, 6).astype(np.uint32), 1.0, 4096, True)
+    bg = (1e-4 * rng.standard_normal(a.size + b.size)).astype(np.float32)
+    return m, orc.Mode("1200", mark=1000.0, space=1800.0), a.size, \
+        (np.concatenate([a, np.float32(0.8 * r) * b]) + bg).astype(np.float32)
+
+
+def _auto_squelch_ratio(r):
+    """amplitude / (0.25 track_amplitude) - 1 at the first search that reaches into the fade"""
+    m, fixed, at, x = _auto_fade(r)
+    res = orc.rx_run(fixed, x, literal=False, want_calls=True)
+    j = next(i for i, cl in enumerate(res["calls"]) if cl[8] > 0 and cl[10] + cl[9] >= at)
+    track = np.float32(0)
+    for f in res["frames"]:
+        if f[5] + f[3] >= res["calls"][j][10]:
+            break
+        track = np.float32((track + f[2]) / np.float32(2))
+    return float(res["calls"][j][8]) / float(np.float32(0.25) * track) - 1
+
+
+@pytest.mark.parametrize("eps", [-1e-5, -1e-6, -1e-7, 1e-7, 1e-6, 1e-5])
+def test_the_auto_screen_flags_a_squelch_tie(eps):
+    """A fade under auto-carrier tuned (secant on its amplitude ratio) so that the squelch `amplitude <
+    track_amplitude * 0.25` sits within eps of a tie: autoorc.screen flags it (the replay's margin, decided
+    the other way by autoorc.flipped); a fade clear of the tie stays robust."""
+    r0, r1 = 0.25, 0.26
+    g0, g1 = _auto_squelch_ratio(r0) - eps, _auto_squelch_ratio(r1) - eps
+    for _ in range(30):
+        if abs(g1) < abs(eps) / 2 + 6e-8 or g1 == g0:
+            break
+        r0, r1, g0 = r1, r1 - g1 * (r1 - r0) / (g1 - g0), g1
+        g1 = _auto_squelch_ratio(r1) - eps
+    assert abs(g1) < abs(eps) / 2 + 6e-8, (eps, r1, g1)
+    m, fixed, at, x = _auto_fade(r1)
+    auto = autoorc.rx_run(m, x)
+    k = sum(1 for f in auto["frames"] if f[5] + f[3] < at)
+    assert k >= 5 and auto["frames"][:k] == orc.rx_run(fixed, x, literal=False)["frames"][:k]
+    assert set(auto["frame_band"]) == {5}
+    _, robust = autoorc.screen(m, x)
+    assert not robust, (eps, r1)
+    _, robust = autoorc.screen(m, _auto_fade(0.3)[3])
+    assert robust

@@ -7,8 +7,12 @@ streams that each carry their own tone pairs, behind silent lead-ins, with a gap
 and a second transmission on other tones.  Every stream is screened first (autoorc.screen): a scan decision
 within 1e-5 (relative) of a tie -- its two largest band magnitudes, or its largest and the threshold -- or a
 frame search that tests/tie_screen.py's perturbed runs can tip marks the stream as not robust.  Robust
-streams must give the oracle's records and bands exactly (confidences within the usual bar); the device's
-band magnitudes are the fsk_b200_detect_carrier_batch ones, within about 1e-6 of the oracle's."""
+streams must give the oracle's records and bands exactly (confidences within the usual bar).
+
+SCAN_TIE rests on test_band_decisions_match_a_float64_dft: every consumer of band_mag (FskPlan.detect_carrier,
+detect_carrier_batch and the scan inside the rx loop, float and int16 rows) takes a float64 DFT's decision
+between two bands 2e-6 apart, in every lane placement of every AUTO_COMBOS instance, at the exact threshold
+and on a tie of every band."""
 import zlib
 
 import numpy as np
@@ -19,7 +23,7 @@ import golden_util as gu
 import orc
 import refcases
 from gpudev import dev, mm, pcm, rows, sync, torch, upload
-from rxcases import COVER, KEYS, auto_combos, tone_stream
+from rxcases import COVER, KEYS, auto_combos, live_records, records_of, tone_stream
 from rxfam import as_oracle_frames, compare_frames, compare_reports, reports_of
 
 
@@ -162,12 +166,6 @@ def test_auto_instance_int16_rows_equal_the_float_rows(key):
         assert sa["nframes"].sum() >= len(streams)
 
 
-def records_of(frames, states, bands):
-    """per stream: [(record bytes, band)] of the records a call wrote"""
-    fr, st, b = mm().frames_to_numpy(frames), mm().states_to_numpy(states), bands.cpu().numpy()
-    return [[(fr[s, i].tobytes(), int(b[s, i])) for i in range(int(st["nframes"][s]))] for s in range(len(st))]
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize("src", ["f32", "s16"])
 @pytest.mark.parametrize("key", KEYS, ids=[str(k) for k in KEYS])
@@ -258,42 +256,6 @@ def test_cli_auto_carrier_vectors_decode_on_the_device(name):
     assert got == want
 
 
-def live_records(mode, rate, streams, cut):
-    """The live-stream recipe of include/fsk_b200.h with auto-carrier: fsk_b200_stream_push, then
-    fsk_b200_rx_batch_auto with the auto holdback, chunk by chunk; the holdback off for the last call.
-    Returns every stream's records and bands in order."""
-    t = torch()
-    eng = engine(mode, rate)
-    window = eng.auto_stream_window()
-    eng.set_holdback(window)
-    stride = (window + eng.params.frame_nsamples + cut + 3) & ~3
-    max_frames = eng.max_frames(stride)
-    S = len(streams)
-    buf, n = rows(streams, np.float32, 4)
-    lens = np.array([len(a) for a in streams], np.int64)
-    z = lambda shape, dt: t.zeros(shape, dtype=dt).to(dev())
-    rows_, fill = z((S, stride), t.float32), z((S,), t.int32)
-    states, auto = z((S, mm().STATE_WORDS), t.int32), z((S, mm().AUTO_STATE_BYTES), t.uint8)
-    dropped = z((S,), t.int32)
-    got = [[] for _ in streams]
-
-    def step(chunk, valid):
-        mm().stream_push(rows_, fill, states, chunk, valid, dropped=dropped)
-        frames, _, _, bands = eng.rx_batch_auto(rows_, nsamples=stride, nsamples_each=fill, max_frames=max_frames,
-                                                states=states, auto_states=auto, rec_band=True)
-        sync()
-        for s, r in enumerate(records_of(frames, states, bands)):
-            got[s] += r
-    for o in range(0, n, cut):
-        w = min(cut, n - o)
-        step(upload(np.ascontiguousarray(buf[:, o:o + w])),
-             upload(np.clip(lens - o, 0, w).astype(np.int32)))
-    eng.set_holdback(0)
-    step(z((S, 4), t.float32), 0)
-    assert int(dropped.cpu().numpy().sum()) == 0
-    return got
-
-
 @pytest.mark.gpu
 def test_live_stream_records_do_not_depend_on_the_cut():
     """Live streams with auto-carrier: the records and bands do not depend on how the streams are cut,
@@ -308,7 +270,7 @@ def test_live_stream_records_do_not_depend_on_the_cut():
     r = run_auto(eng, buf, n, np.array([len(a) for a in streams], np.int32))
     whole = records_of(r[0], r[1], r[3])
     for cut in (997, 4096, 20000):
-        assert live_records(mode, rate, streams, cut) == whole, cut
+        assert live_records(engine(mode, rate), streams, cut) == whole, cut
     buf, n = rows(streams, np.float32, 4)
     lens = np.array([len(a) for a in streams], np.int64)
     outs = []
@@ -370,3 +332,245 @@ def test_every_preset_runs_and_the_errors_launch_nothing():
         with pytest.raises(RuntimeError, match="-95"):
             e.rx_batch_auto(x, nsamples=4096)
         assert mm().launch_count() == n0
+
+
+# ---------------------------------------------------------------------------------------------------
+# band decisions against a float64 DFT: every consumer of band_mag
+# ---------------------------------------------------------------------------------------------------
+EPSILONS = (2e-6, -2e-6, 1e-5, -1e-5, 1e-4, -1e-4)
+
+
+class Window:
+    """one preset's carrier-scan window: n samples zero-padded to fftsize F, bands 1 .. nbands-1; G the lanes
+    of its AUTO_COMBOS instance; L = ceil(nsamples_per_scan), the shortest stream whose scan reads it"""
+
+    def __init__(self, key):
+        self.key = key
+        self.mode, self.rate = COVER[key]
+        self.G = key[0]
+        m = orc.Mode(self.mode, sample_rate=self.rate)
+        p = mm().rx_params(mm().rx_config_for_mode(self.mode, self.rate))
+        self.F, self.nbands = int(p.fftsize), int(p.nbands)
+        sf = np.float32(min(np.float32(m.derived().nsamples_per_bit), np.float32(self.F)))
+        self.n, self.L = int(sf), int(np.ceil(sf))
+        self.b_shift = autoorc.b_shift(m)
+        self.m = m
+        k = np.arange(self.nbands)[:, None] * np.arange(self.n)[None, :] % self.F
+        self.w = np.exp(-2j * np.pi * k / self.F)          # [band, sample], exact integer phase
+
+    def mags(self, x):
+        """float64 band magnitudes of the exact samples x[:n], band_mag's scale (2 / n); band 0 is -1"""
+        m = np.abs(self.w @ np.asarray(x[:self.n], np.float64)) * (2.0 / self.n)
+        m[0] = -1.0
+        return m
+
+    def accepts(self, b):
+        return 1 <= b + self.b_shift < self.nbands
+
+    def placements(self):
+        """(name, k1, k2): the two bands in one lane of a group (k2 = k1 + G), in neighbouring lanes, across the
+        G-lane group (lane G-1, then lane 0), and, for the warp-wide scan of detect_carrier_batch, in one lane
+        of the 32-lane stride and across it; both bands accepted by the scan"""
+        lo = max(1, 1 - self.b_shift)
+        hi = min(self.nbands - 1, self.nbands - 1 - self.b_shift)
+        mid = (lo + hi) // 2
+        G = self.G
+        want = [("same-lane", mid - G // 2, mid - G // 2 + G), ("neighbour-lanes", mid, mid + 1),
+                ("across-group", (mid // G) * G, (mid // G) * G + 1), ("same-lane-32", mid - 16, mid + 16),
+                ("across-32", 32, 33), ("across-32", 64, 65)]
+        return [(nm, a, b) for nm, a, b in want if lo <= a < b <= hi]
+
+    def duel(self, rng, k1, k2, eps, s16):
+        """x [L] float32 (s16: int16) whose window's float64 magnitudes have bands k1 and k2 on top, |k2| / |k1| - 1
+        within 10 % of eps, and every other band below both by more than 1e-3 of them; (x, the eps it has)"""
+        i = np.arange(self.n)
+        q = 1.0 / 32768.0
+        for _ in range(64):
+            p1, p2 = rng.uniform(0, 2 * np.pi, 2)
+            build = lambda a2: 0.4 * np.cos(2 * np.pi * (k1 * i % self.F) / self.F + p1) + \
+                a2 * np.cos(2 * np.pi * (k2 * i % self.F) / self.F + p2)
+            r = lambda a2: (lambda mg: mg[k2] / mg[k1] - 1.0)(self.mags(build(a2)))
+            lo, hi = 0.05, 0.55             # |x| < 1: int16 holds it
+            if not r(lo) < eps < r(hi):
+                continue
+            for _ in range(80):
+                mid = (lo + hi) / 2
+                lo, hi = (mid, hi) if r(mid) < eps else (lo, mid)
+            x = build((lo + hi) / 2)
+            x = np.round(x / q).astype(np.float64) * q if s16 else x.astype(np.float32).astype(np.float64)
+            # single-step nudges (one LSB or one ulp of one sample) toward eps
+            D1, D2 = self.w[k1] @ x, self.w[k2] @ x
+            for _ in range(200):
+                e = abs(D2) / abs(D1) - 1.0
+                if abs(e - eps) <= 0.05 * abs(eps):
+                    break
+                step = np.full(self.n, q) if s16 else np.spacing(np.abs(x).astype(np.float32)).astype(np.float64)
+                cand = []
+                for sgn in (1.0, -1.0):
+                    d1 = D1 + sgn * step * self.w[k1]
+                    d2 = D2 + sgn * step * self.w[k2]
+                    cand.append(np.abs(np.abs(d2) / np.abs(d1) - 1.0 - eps))
+                cand = np.array(cand)
+                j = np.unravel_index(np.argmin(cand), cand.shape)
+                if cand[j] >= abs(e - eps):
+                    break
+                sgn = 1.0 if j[0] == 0 else -1.0
+                x[j[1]] += sgn * step[j[1]]
+                D1, D2 = self.w[k1] @ x, self.w[k2] @ x
+            mg = self.mags(x)
+            e = mg[k2] / mg[k1] - 1.0
+            others = np.delete(mg, [0, k1, k2])
+            if abs(e - eps) <= 0.1 * abs(eps) and others.max() < (1 - 1e-3) * min(mg[k1], mg[k2]) \
+                    and min(mg[k1], mg[k2]) > 10 * autoorc.DEFAULT_THRESHOLD:
+                out = np.zeros(self.L, np.float64)
+                out[:self.n] = x
+                if s16:
+                    return np.round(out * 32768).astype(np.int16), e
+                return out.astype(np.float32), e
+        raise AssertionError(("no duel", self.key, k1, k2, eps))
+
+    def impulse(self, a, s16=False):
+        x = np.zeros(self.L, np.int16 if s16 else np.float32)
+        x[0] = a
+        return x
+
+    def threshold_amplitude(self):
+        """the float32 a > 0 with fl(a * magscalar) == threshold exactly (magscalar = 1 / (n / 2), src/fsk.c:553),
+        or None; an impulse of a at the window start gives every band that magnitude"""
+        ms = np.float32(1) / (np.float32(self.n) / np.float32(2))
+        thr = np.float32(autoorc.DEFAULT_THRESHOLD)
+        a = np.float32(thr / ms)
+        for k in range(-64, 65):
+            b = np.float32(a + np.float32(k) * np.spacing(a))
+            if np.float32(b * ms) == thr:
+                return b
+        return None
+
+
+WINDOWS = {}
+
+
+def window(key):
+    if key not in WINDOWS:
+        WINDOWS[key] = Window(key)
+    return WINDOWS[key]
+
+
+def band_cases(key):
+    """[(name, x float32 [L] or int16, the float64 decision: a band or -1, the band decision's eps or None)] of
+    one preset: every placement at every eps (float32 and int16 samples), the exact threshold and 2e-6 either
+    side, and the tie of every band (an impulse at the window start)"""
+    w = window(key)
+    rng = np.random.default_rng(zlib.crc32(repr(("duels",) + key).encode()))
+    out = []
+    for nm, k1, k2 in w.placements():
+        for eps in EPSILONS:
+            for s16 in (False, True):
+                x, e = w.duel(rng, k1, k2, eps, s16)
+                out.append(("%s %d/%d eps=%g%s" % (nm, k1, k2, eps, " s16" if s16 else ""), x, k2 if e > 0 else k1, e))
+    a = w.threshold_amplitude()
+    if a is not None:
+        out.append(("threshold", w.impulse(a), 1, None))
+        out.append(("threshold-2e-6", w.impulse(np.float32(a * np.float32(1 - 2e-6))), -1, None))
+        out.append(("threshold+2e-6", w.impulse(np.float32(a * np.float32(1 + 2e-6))), 1, None))
+    # every band at fl(|a| magscalar): band 1 where that reaches the threshold
+    ms = np.float32(1) / (np.float32(w.n) / np.float32(2))
+    tie = lambda a: 1 if np.float32(np.float32(a) * ms) >= np.float32(autoorc.DEFAULT_THRESHOLD) else -1
+    out.append(("tie", w.impulse(0.875), tie(0.875), None))
+    out.append(("tie s16", w.impulse(28672, s16=True), tie(0.875), None))
+    return out
+
+
+def widened(x):
+    return x.astype(np.float32) * np.float32(1.0 / 32768.0) if x.dtype == np.int16 else x
+
+
+def scan_band(w, want):
+    """what the scan leaves in the auto state for the float64 decision `want`: the band if the scan accepts it, 0
+    for none or a rejected band"""
+    return want if want > 0 and w.accepts(want) else 0
+
+
+def test_band_cases_are_what_they_claim():
+    """The duels' float64 winners and margins, the exact threshold (every band's float32 magnitude equals it),
+    the tie; and the auto oracle's scan (its scan log) takes the float64 decision on every one."""
+    nthr = 0
+    for key in KEYS:
+        w = window(key)
+        assert w.placements(), key
+        for name, x, want, e in band_cases(key):
+            y = widened(x)
+            mg = w.mags(y)
+            if e is not None:
+                assert int(np.argmax(mg)) == want, (key, name)
+            elif name.startswith("threshold"):
+                nthr += 1
+                ms = np.float32(1) / (np.float32(w.n) / np.float32(2))
+                got = np.float32(abs(np.float32(y[0])) * ms)
+                thr = np.float32(autoorc.DEFAULT_THRESHOLD)
+                assert (got == thr) if name == "threshold" else (got < thr) == name.endswith("-2e-6"), (key, name)
+            r = autoorc.rx_run(w.m, y, scans=True)
+            assert r["scans"][0]["band"] == want and r["scans"][0]["window"] == (0 if want > 0 else 1), (key, name)
+        if w.nbands > 33:
+            assert any(nm.startswith("across-32") for nm, _, _ in w.placements()), key
+    assert nthr >= 3 * (len(KEYS) - 1), nthr
+    assert any(window(k).nbands > 32 for k in KEYS) and any(window(k).b_shift < 0 for k in KEYS)
+
+
+@pytest.mark.ref
+def test_the_reference_fft_ties_every_band_on_an_impulse():
+    """The reference's own fsk_detect_carrier (oracle/_ref) on the impulse windows: the tie and the exact
+    threshold pick band 1, 2e-6 below the threshold nothing."""
+    import ctypes as C
+    fn = orc.ref().fsk_detect_carrier
+    fn.argtypes = [C.c_void_p, C.POINTER(C.c_float), C.c_uint, C.c_float]
+    fn.restype = C.c_int
+    for key in KEYS:
+        w = window(key)
+        rp = orc.RefPlan(w.rate, w.m.mark_f, w.m.space_f, w.m.band_width)
+        for name, x, want, e in band_cases(key):
+            if e is None:
+                y = np.ascontiguousarray(widened(x)[:w.n])
+                assert fn(rp.h, orc.fptr(y), w.n, autoorc.DEFAULT_THRESHOLD) == want, (key, name)
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("key", KEYS, ids=[str(k) for k in KEYS])
+def test_band_decisions_match_a_float64_dft(key):
+    """Every consumer of band_mag takes the float64 DFT's decision: FskPlan.detect_carrier (k_band_mags),
+    detect_carrier_batch (k_detect_carrier) and the scan of rx_batch_auto on float and int16 rows (detect_group;
+    the stream is shorter than a frame, so the loop scans once and stops, its decision in the auto state) --
+    on duels of two bands eps apart, the exact threshold and the tie of every band."""
+    w = window(key)
+    cases = band_cases(key)
+    t = torch()
+    plan = mm().FskPlan(w.rate, float(w.m.mark_f), float(w.m.space_f), float(w.m.band_width))
+    assert (plan.fftsize, plan.nbands) == (w.F, w.nbands)
+    eng = engine(w.mode, w.rate)
+    bad = []
+    fl = [(nm, widened(x), want, e) for nm, x, want, e in cases]
+    buf, _ = rows([x for _, x, _, _ in fl], np.float32, 4)
+    got_b = mm().detect_carrier_batch(w.F, upload(buf), w.n, autoorc.DEFAULT_THRESHOLD).cpu().numpy()
+    for i, (nm, x, want, e) in enumerate(fl):
+        got = plan.detect_carrier(np.ascontiguousarray(x[:w.n]), autoorc.DEFAULT_THRESHOLD)
+        if got != want:
+            bad.append(("detect_carrier", nm, e, got, want))
+        if int(got_b[i]) != want:
+            bad.append(("detect_carrier_batch", nm, e, int(got_b[i]), want))
+    for src in ("f32", "s16"):
+        sub = [(nm, x, want, e) for nm, x, want, e in cases if (x.dtype == np.int16) == (src == "s16")]
+        xs = [x for _, x, _, _ in sub]
+        buf, _ = rows(xs, xs[0].dtype, 8)
+        lens = np.full(len(xs), w.L, np.int32)
+        _, st, ast, _ = run_auto(eng, buf, w.L, lens)
+        assert "k_rx_auto<G=%d,W=%d,L=%d," % key in eng.last_kernel() and "src=%s" % src in eng.last_kernel()
+        assert (mm().states_to_numpy(st)["nframes"] == 0).all()
+        band = ast.cpu().numpy().view(np.uint32)[:, 0]
+        for (nm, x, want, e), b in zip(sub, band):
+            if int(b) != scan_band(w, want):
+                bad.append(("scan " + src, nm, e, int(b), scan_band(w, want)))
+    plan.destroy()
+    eps = [abs(b[2]) for b in bad if b[2] is not None]
+    print("%s: %d decisions, %d disagree with the float64 DFT; smallest |eps| disagreeing: %s" % (
+        key, 3 * len(cases), len(bad), "%.2g" % min(eps) if eps else "none"))
+    assert not bad, bad[:8]
