@@ -539,15 +539,9 @@ fsk_b200_engine *fsk_b200_engine_new(const fsk_b200_rx_params *params)
 	errno = EINVAL;
 	return NULL;
     }
-    {	/* phase advance of the two tones over one bit period, argument reduced exactly in integers */
-	const unsigned long long F = (unsigned long long)(params->fftsize > 0 ? params->fftsize : 1);
-	const double am = 2.0 * M_PI * (double)(((unsigned long long)params->b_mark * e->geom.bit_nsamples) % F) / (double)F;
-	const double as = 2.0 * M_PI * (double)(((unsigned long long)params->b_space * e->geom.bit_nsamples) % F) / (double)F;
-	e->geom.rot[0] = (float)cos(am);
-	e->geom.rot[1] = (float)-sin(am);
-	e->geom.rot[2] = (float)cos(as);
-	e->geom.rot[3] = (float)-sin(as);
-    }
+    /* phase advance of the two tones over one bit period */
+    fsk_b200_tone_pair_phase(params->b_mark, params->b_space, e->geom.bit_nsamples,
+	    (unsigned long long)(params->fftsize > 0 ? params->fftsize : 1), e->geom.rot);
     e->autoc.fftsize = params->fftsize;		/* the tone calls read these two as well */
     e->autoc.nbands = params->nbands;
     e->loopc.frame_nsamples = params->frame_nsamples;

@@ -6,11 +6,30 @@
 #ifndef FSK_B200_INTERNAL_H
 #define FSK_B200_INTERNAL_H
 
+#include <math.h>
+
 #include "fsk_b200.h"
 
 #ifdef __cplusplus
 extern "C" {
 #endif
+
+/* exp(-2 pi i b n / F) as (re, im): the argument reduced exactly in integers, evaluated in double and rounded
+ * to float.  Every tone table of the library is built from it, so an entry is the same wherever it is built. */
+static inline void fsk_b200_tone_phase(unsigned long long b, unsigned long long n, unsigned long long F, float out[2])
+{
+    const double a = 2.0 * M_PI * (double)((b * n) % F) / (double)F;
+    out[0] = (float)cos(a);
+    out[1] = (float)-sin(a);
+}
+
+/* the same for a tone pair: (re, im) of b_mark, then of b_space */
+static inline void fsk_b200_tone_pair_phase(unsigned b_mark, unsigned b_space, unsigned long long n,
+	unsigned long long F, float out[4])
+{
+    fsk_b200_tone_phase(b_mark, n, F, out);
+    fsk_b200_tone_phase(b_space, n, F, out + 2);
+}
 
 /* Geometry of one frame candidate as the kernels consume it (passed by value
  * as a kernel parameter, so changing it costs nothing). */

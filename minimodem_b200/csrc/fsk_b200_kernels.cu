@@ -1571,7 +1571,8 @@ struct CudaEngine {
     int smem_optin;
     /* twiddle table */
     float4 *d_tw;
-    unsigned tw_cap, tw_n;
+    size_t tw_cap;		/* bytes */
+    unsigned tw_n;
     int tw_fftsize;
     unsigned tw_bm, tw_bs;
     /* tuning (0 = automatic) */
@@ -1581,7 +1582,8 @@ struct CudaEngine {
     int pfx_fill;		/* mode 3, float rows: 1 (default) TMA bulk fill, 0 cp.async fill */
     int prefix;			/* chunk-prefix table search (mode 3): -1 (default) where it pays, 0 never, 1 wherever it fits */
     float4 *d_twc;		/* mode 3: chunk-rotation table, twc_n = fftsize / gcd(4, fftsize) entries (0: not built) */
-    unsigned twc_n, twc_cap;
+    unsigned twc_n;
+    size_t twc_cap;		/* bytes */
     /* single-stream staging */
     float *d_one;
     size_t d_one_cap;
@@ -1600,6 +1602,7 @@ struct CudaEngine {
     cudaStream_t st[2];
     float2 *d_unit;			/* --auto-carrier: unit-circle table of unit_f entries (AutoArgs.unit) */
     int unit_f;
+    size_t unit_cap;			/* bytes */
 };
 
 extern "C" unsigned long long fsk_b200_cuda_launch_count(void) { return g_launches; }
@@ -1720,8 +1723,28 @@ extern "C" int fsk_b200_cuda_tune(void *p, int lanes, int wpb, int ring)
 				 * (176) take it, SAME (92) and Bell202 (40) stay on the per-candidate kernel */
 #endif
 
-/* exp(-2 pi i k n / fftsize) for k = b_mark, b_space; the argument is reduced
- * exactly in integers and evaluated in double before rounding to float */
+/* the host table h of `bytes` into the engine buffer *d, reallocated first when its capacity *cap is smaller:
+ * 0, -ENOMEM when the allocation failed (the buffer is then gone; the CUDA error is left to the caller) or
+ * -EIO when the copy failed (*err) */
+static int upload_table(void **d, size_t *cap, const void *h, size_t bytes, cudaError_t *err)
+{
+    if (*cap < bytes) {
+	cudaFree(*d);
+	*d = NULL;
+	*cap = 0;
+	if (cudaMalloc(d, bytes) != cudaSuccess)
+	    return -ENOMEM;
+	*cap = bytes;
+    }
+    /* synchronous copy from pageable memory, then a device-wide synchronise: the library's own
+     * streams and the caller's may be cudaStreamNonBlocking, which the legacy stream does not order */
+    *err = cudaMemcpy(*d, h, bytes, cudaMemcpyHostToDevice);
+    if (*err == cudaSuccess)
+	*err = cudaDeviceSynchronize();
+    return *err == cudaSuccess ? 0 : -EIO;
+}
+
+/* exp(-2 pi i k n / fftsize) for k = b_mark, b_space */
 extern "C" int fsk_b200_cuda_set_table(void *p, int fftsize, unsigned b_mark, unsigned b_space,
 	unsigned bit_nsamples)
 {
@@ -1736,35 +1759,14 @@ extern "C" int fsk_b200_cuda_set_table(void *p, int fftsize, unsigned b_mark, un
     float4 *h = (float4 *)malloc(sizeof(float4) * bit_nsamples);
     if (!h)
 	return -ENOMEM;
-    const unsigned long long F = (unsigned long long)fftsize;
-    for (unsigned n = 0; n < bit_nsamples; n++) {
-	const double am = 2.0 * M_PI * (double)(((unsigned long long)b_mark * n) % F) / (double)F;
-	const double as = 2.0 * M_PI * (double)(((unsigned long long)b_space * n) % F) / (double)F;
-	h[n].x = (float)cos(am);
-	h[n].y = (float)-sin(am);
-	h[n].z = (float)cos(as);
-	h[n].w = (float)-sin(as);
-    }
-    if (ce->tw_cap < bit_nsamples) {
-	cudaFree(ce->d_tw);
-	ce->d_tw = NULL;
-	ce->tw_cap = 0;
-	if (cudaMalloc(&ce->d_tw, sizeof(float4) * bit_nsamples) != cudaSuccess) {
-	    fsk_b200_set_error("set_table: %s", cudaGetErrorString(cudaGetLastError()));
-	    free(h);
-	    return -ENOMEM;
-	}
-	ce->tw_cap = bit_nsamples;
-    }
-    /* synchronous copy from pageable memory, then a device-wide synchronise: the library's own
-     * streams and the caller's may be cudaStreamNonBlocking, which the legacy stream does not order */
-    cudaError_t err = cudaMemcpy(ce->d_tw, h, sizeof(float4) * bit_nsamples, cudaMemcpyHostToDevice);
-    if (err == cudaSuccess)
-	err = cudaDeviceSynchronize();
+    for (unsigned n = 0; n < bit_nsamples; n++)
+	fsk_b200_tone_pair_phase(b_mark, b_space, n, (unsigned)fftsize, &h[n].x);
+    cudaError_t err;
+    int rc = upload_table((void **)&ce->d_tw, &ce->tw_cap, h, sizeof(float4) * bit_nsamples, &err);
     free(h);
-    if (err != cudaSuccess) {
-	fsk_b200_set_error("set_table: %s", cudaGetErrorString(err));
-	return -EIO;
+    if (rc) {
+	fsk_b200_set_error("set_table: %s", cudaGetErrorString(rc == -ENOMEM ? cudaGetLastError() : err));
+	return rc;
     }
     ce->tw_n = bit_nsamples;
     ce->tw_fftsize = fftsize;
@@ -1774,47 +1776,29 @@ extern "C" int fsk_b200_cuda_set_table(void *p, int fftsize, unsigned b_mark, un
      * only takes multiples of gcd(4, fftsize), so the table has fftsize / gcd entries, entry e for the
      * sample index e * gcd.  Kept only while it is small enough to be staged per block. */
     ce->twc_n = 0;
-    {
-	const unsigned g4 = (fftsize % 4 == 0) ? 4u : (fftsize % 2 == 0) ? 2u : 1u;
-	const unsigned fp = (unsigned)fftsize / g4;
-	if ((size_t)fp * sizeof(float4) <= FSK_PFX_MAX_TABLE_BYTES) {
-	    /* (FSK_PFX_TABLE_EXTRA entries more than one period: a lane-run of the table build walks it
-	     * linearly from anywhere inside the period) */
-	    const unsigned fp1 = fp, fpx = fp + FSK_PFX_TABLE_EXTRA;
-	    float4 *hc = (float4 *)malloc(sizeof(float4) * fpx);
-	    if (!hc)
-		return -ENOMEM;
-	    for (unsigned i = 0; i < fpx; i++) {
-		const unsigned long long n = (unsigned long long)(i % fp1) * g4;
-		const double am = 2.0 * M_PI * (double)(((unsigned long long)b_mark * n) % F) / (double)F;
-		const double as = 2.0 * M_PI * (double)(((unsigned long long)b_space * n) % F) / (double)F;
-		hc[i].x = (float)cos(am);
-		hc[i].y = (float)-sin(am);
-		hc[i].z = (float)cos(as);
-		hc[i].w = (float)-sin(as);
-	    }
-	    if (ce->twc_cap < fpx) {
-		cudaFree(ce->d_twc);
-		ce->d_twc = NULL;
-		ce->twc_cap = 0;
-		if (cudaMalloc(&ce->d_twc, sizeof(float4) * fpx) != cudaSuccess) {
-		    (void)cudaGetLastError();
-		    free(hc);
-		    return 0;			/* mode 3 is simply not offered */
-		}
-		ce->twc_cap = fpx;
-	    }
-	    cudaError_t err2 = cudaMemcpy(ce->d_twc, hc, sizeof(float4) * fpx, cudaMemcpyHostToDevice);
-	    if (err2 == cudaSuccess)
-		err2 = cudaDeviceSynchronize();
-	    free(hc);
-	    if (err2 != cudaSuccess) {
-		fsk_b200_set_error("set_table: %s", cudaGetErrorString(err2));
-		return -EIO;
-	    }
-	    ce->twc_n = fp;
-	}
+    const unsigned g4 = (fftsize % 4 == 0) ? 4u : (fftsize % 2 == 0) ? 2u : 1u;
+    const unsigned fp = (unsigned)fftsize / g4;
+    if ((size_t)fp * sizeof(float4) > FSK_PFX_MAX_TABLE_BYTES)
+	return 0;
+    /* (FSK_PFX_TABLE_EXTRA entries more than one period: a lane-run of the table build walks it
+     * linearly from anywhere inside the period) */
+    const unsigned fpx = fp + FSK_PFX_TABLE_EXTRA;
+    float4 *hc = (float4 *)malloc(sizeof(float4) * fpx);
+    if (!hc)
+	return -ENOMEM;
+    for (unsigned i = 0; i < fpx; i++)
+	fsk_b200_tone_pair_phase(b_mark, b_space, (unsigned long long)(i % fp) * g4, (unsigned)fftsize, &hc[i].x);
+    rc = upload_table((void **)&ce->d_twc, &ce->twc_cap, hc, sizeof(float4) * fpx, &err);
+    free(hc);
+    if (rc == -ENOMEM) {
+	(void)cudaGetLastError();
+	return 0;			/* mode 3 is simply not offered */
     }
+    if (rc) {
+	fsk_b200_set_error("set_table: %s", cudaGetErrorString(err));
+	return rc;
+    }
+    ce->twc_n = fp;
     return 0;
 }
 
@@ -1898,13 +1882,21 @@ static bool split_for(int G, unsigned n_bits, int force_L, int *W, int *L)
     return best > 0.0;
 }
 
-/* per_stream_tw (--auto-carrier): the per-candidate kernel only, with a tone table per stream instead of
- * one per block */
-static int pick_shape(const CudaEngine *ce, const fsk_b200_geom *g, unsigned need_floats,
-	unsigned max_advance, size_t nstreams, Shape *sh, const fsk_b200_loopc *lc = NULL, bool per_stream_tw = false)
+/* the ring of the widest search window (whole blocks, room for it to start anywhere inside a block): it
+ * already leaves 1..2 blocks of look-ahead, and a deeper ring means fewer resident streams */
+static unsigned ring_min_for(unsigned need_floats)
 {
-    sh->geo = *g;
-    memset(&sh->mplan, 0, sizeof(sh->mplan));
+    return (need_floats + 8u + 2u * RING_BLOCK - 1u) / RING_BLOCK * RING_BLOCK;
+}
+
+/* mode 0, the per-candidate kernel: a ring per stream (the minimum, or the one asked for), G lanes per stream
+ * and the (W, L) split of the windows, then the most warps per block -- failing that, more lanes per stream --
+ * that fit.  per_stream_tw (--auto-carrier, the tone calls): a tone table per stream instead of one per block.
+ * False where the kernel cannot run the mode: no split, bit periods too long, the table not in shared memory,
+ * or no ring fits (sh->ring is then 0). */
+static bool plan_per_candidate(const CudaEngine *ce, const fsk_b200_geom *g, unsigned need_floats,
+	bool per_stream_tw, Shape *sh)
+{
     const size_t smem_max = (size_t)ce->smem_optin;
     const size_t tw_bytes = (size_t)g->bit_nsamples * sizeof(float4);	/* the sliding search's extension is added at the end */
     sh->tw_in_smem = tw_bytes <= 24 * 1024;
@@ -1912,21 +1904,10 @@ static int pick_shape(const CudaEngine *ce, const fsk_b200_geom *g, unsigned nee
     const size_t pad_bytes = (size_t)((g->bit_nsamples + 3u) & ~3u) * 4;
     /* per stream, besides the ring: scratch, mirror, 2 mbarriers (and its tone table) */
     const size_t scr_bytes = (size_t)g->n_bits * sizeof(float2) + pad_bytes + 16 + (per_stream_tw ? tw_bytes : 0);
-
-    /* ring: the widest search window plus (ideally) one full advance of look-ahead */
-    /* whole blocks; room for the widest window starting anywhere inside a block */
-    const unsigned ring_min = (need_floats + 8u + 2u * RING_BLOCK - 1u) / RING_BLOCK * RING_BLOCK;
-    (void)max_advance;
-    /* default: the minimum, which already leaves 1..2 blocks of look-ahead; a deeper ring means
-     * fewer resident streams */
+    const unsigned ring_min = ring_min_for(need_floats);
     unsigned ring = ce->ring ? ((unsigned)ce->ring + RING_BLOCK - 1u) / RING_BLOCK * RING_BLOCK : ring_min;
     if (ring < ring_min)
 	ring = ring_min;
-    /* keep at least ~24 streams per SM resident if that is possible at all */
-    if (!ce->ring) {
-	while (ring > ring_min && (smem_max - fixed) / ((size_t)ring * 4 + scr_bytes) < 24)
-	    ring -= RING_BLOCK;
-    }
 
     int G = ce->lanes;
     if (!G) {
@@ -1944,207 +1925,255 @@ static int pick_shape(const CudaEngine *ce, const fsk_b200_geom *g, unsigned nee
 	G <<= 1;
 	fast = split_for(G, g->n_bits, ce->split, &W, &L);
     }
-    if (g->bit_nsamples > FAST_MAX_N * (unsigned)L || !sh->tw_in_smem)
-	fast = false;
-
     int wpb = ce->wpb ? ce->wpb : 2;
-    for (;;) {
-	const size_t spw = 32 / G;
-	const size_t smem = (fixed + (size_t)wpb * spw * ((size_t)ring * 4 + scr_bytes) + 15) & ~(size_t)15;
-	if (smem <= smem_max) {
-	    sh->smem = smem;
-	    break;
-	}
-	if (wpb > 1) { wpb--; continue; }
-	if (G < 32) {
+    size_t smem;
+    while ((smem = (fixed + (size_t)wpb * (32 / G) * ((size_t)ring * 4 + scr_bytes) + 15) & ~(size_t)15) > smem_max) {
+	if (wpb > 1) {
+	    wpb--;
+	} else if (G < 32) {
 	    G <<= 1;
-	    fast = split_for(G, g->n_bits, ce->split, &W, &L) && g->bit_nsamples <= FAST_MAX_N * (unsigned)L && sh->tw_in_smem;
-	    continue;
-	}
-	if (ring) { ring = 0; fast = false; continue; }	/* not even one ring fits: read global memory */
-	sh->tw_in_smem = 0;
-	sh->smem = ((size_t)g->n_bits * sizeof(float2) + 16 + 15) & ~(size_t)15;
-	break;
-    }
-    if (!fast) {
-	/* generic kernels are instantiated for G = 32 only and do not use a ring */
-	G = 32;
-	ring = 0;
-	L = 1;
-	while ((unsigned)(L * 2) * g->n_bits <= 32u)
-	    L *= 2;
-	W = (int)((g->n_bits + 32 / L - 1) / (32 / L));
-	const size_t fixed2 = sh->tw_in_smem ? tw_bytes : 0;
-	const size_t scr_only = (size_t)g->n_bits * sizeof(float2) + 16;
-	wpb = ce->wpb ? ce->wpb : 4;
-	sh->smem = (fixed2 + (size_t)wpb * scr_only + 15) & ~(size_t)15;
-	if (sh->smem > smem_max) {
-	    sh->tw_in_smem = 0;
-	    sh->smem = ((size_t)wpb * scr_only + 15) & ~(size_t)15;
-	}
-    }
-    sh->mode = fast ? 0 : 1;
-    if (fast && lc && !per_stream_tw && ce->multi && (ce->multi > 0 || g->bit_nsamples >= FSK_MULTI_MIN_N)) {
-	/* the rx loop's searches from shared segment sums, if this mode's windows tile and all of its
-	 * searches fit the period slots of a (W, L) split of this group size */
-	int W2 = 0, L2 = 0;
-	if (split_for_multi(G, g->n_bits + 1u, &W2, &L2) && g->bit_nsamples <= FAST_MAX_N * (unsigned)L2
-		&& fsk_b200_mplan_build(g, lc, (unsigned)(W2 * (G / L2)), &sh->mplan) == 0) {
-	    sh->mode = 2;
-	    sh->mplan.always = ce->multi >= 2 || ce->multi < 0;
-	    W = W2;
-	    L = L2;
-	}
-    }
-    memset(&sh->pfx, 0, sizeof(sh->pfx));
-    if (lc && !per_stream_tw && ce->prefix && ce->twc_n && ring_min >= 128u
-	    && (ce->prefix > 0 || g->bit_nsamples >= FSK_PREFIX_MIN_N)) {
-	/* the rx loop's searches from a chunk-prefix table (mode 3): one stream per warp, one lane per
-	 * window boundary of a candidate, the ring without its mirror plus the table per stream */
-	fsk_b200_pfx &pf = sh->pfx;
-	const unsigned nb = g->n_bits, N = g->bit_nsamples;
-	pf.tiles = 1;
-	for (unsigned w = 0; w + 1 < nb; w++)
-	    if (g->bit_begin[w + 1] != g->bit_begin[w] + N)
-		pf.tiles = 0;
-	pf.nbnd = pf.tiles ? nb + 1u : 2u * nb;
-	/* candidate slots: aligned power-of-two slots reduce by butterflies; slots of exactly nbnd lanes packed
-	 * back to back are used only where they hold more candidates per round (9 boundaries: 3 instead of 2) */
-	unsigned bs2 = 8;
-	int lb = 3;
-	while (bs2 < pf.nbnd) {
-	    bs2 <<= 1;
-	    lb++;
-	}
-	if (pf.nbnd <= 32u && 32u / bs2 == 32u / pf.nbnd) {
-	    pf.bs = bs2;
-	    pf.pow2 = 1;
+	    fast = split_for(G, g->n_bits, ce->split, &W, &L);
 	} else {
-	    pf.bs = pf.nbnd;
-	    pf.pow2 = 0;
-	    lb = 1;			/* the kernel's template code for packed slots */
-	}
-	pf.cpr = pf.bs ? 32u / pf.bs : 0u;
-	/* 16-byte pieces of the widest search span (it may start up to 3 samples into its first piece), dealt
-	 * to the 32 lanes in runs of S pieces.  S odd: the lanes walk their runs in step, S pieces apart, and
-	 * only an odd stride spreads a quarter-warp's 16-byte accesses over all banks; the same for the table
-	 * rows (tstride) */
-	const unsigned npieces = (3u + need_floats) / 4u + 1u;
-	pf.S = ((npieces + 31u) / 32u) | 1u;
-	pf.inv_S = 1.0f / (float)pf.S;
-	pf.tstride = ((pf.S + 1u) / 2u) | 1u;
-	const unsigned F = (unsigned)ce->tw_fftsize;
-	const unsigned g4 = (F % 4u == 0) ? 4u : (F % 2u == 0) ? 2u : 1u;
-	pf.fp = F / g4;
-	pf.s4 = 4u / g4;
-	pf.inv_fp = 1.0f / (float)pf.fp;
-	for (unsigned j = 0; j <= 7; j++) {
-	    const double am = 2.0 * M_PI * (double)(((unsigned long long)ce->tw_bm * j) % F) / (double)F;
-	    const double as = 2.0 * M_PI * (double)(((unsigned long long)ce->tw_bs * j) % F) / (double)F;
-	    pf.loc[j >> 1][0][j & 1u] = j ? (float)cos(am) : 1.0f;
-	    pf.loc[j >> 1][1][j & 1u] = j ? (float)-sin(am) : 0.0f;
-	    pf.loc[j >> 1][2][j & 1u] = j ? (float)cos(as) : 1.0f;
-	    pf.loc[j >> 1][3][j & 1u] = j ? (float)-sin(as) : 0.0f;
-	}
-	for (unsigned k = 0; k < 4; k++) {		/* the rx loop's four searches, src/minimodem.c:1236-1263, :1357-1368 */
-	    const unsigned carrier = k & 1u, fine = k >> 1;
-	    const unsigned tmax_k = carrier ? lc->try_max_carrier : lc->try_max_nocarrier;
-	    const unsigned first = carrier ? lc->nsamples_overscan : 0u;
-	    unsigned step = tmax_k / (fine ? 8u : 3u);
-	    if (step == 0)
-		step = 1;
-	    fsk_b200_pfx_kind &kd = pf.kind[k];
-	    kd.step = step;
-	    kd.k_up = tmax_k > first ? (tmax_k - 1u - first) / step : 0u;
-	    kd.k_dn = first / step < kd.k_up ? first / step : kd.k_up;
-	    kd.ncands = tmax_k > first ? 1u + kd.k_up + kd.k_dn : 0u;
-	}
-	const unsigned ring3 = ce->ring ? ring : ring_min;
-	const unsigned tw_stage = pf.fp + (pf.S + 2u) * pf.s4;	/* one period and a lane-run */
-	const size_t table = (size_t)tw_stage * sizeof(float4);
-	const size_t per_stream = ((size_t)ring3 + 4u * pf.S + 8u) * 4 + (size_t)nb * sizeof(float2) + 16
-	    + (32u * (size_t)pf.tstride + 32u + (pf.pow2 ? 0u : 32u)) * sizeof(float4);	/* ring + mirror, scratch, barriers, table + totals (+ slot-sum scratch) */
-	/* warps (= streams) per block: the most resident streams per SM (each block pays the table and 1 KiB) */
-	const size_t sm_total = (size_t)ce->smem_optin + 1024;
-	int best_wpb = 0;
-	size_t best_streams = 0;
-	for (int w = 1; w <= FSK_PFX_MAXTHREADS / 32; w++) {
-	    const size_t blk = ((table + (size_t)w * per_stream + 16 + 128 + 15) & ~(size_t)15);
-	    if (blk > smem_max)
-		break;
-	    size_t nblk = sm_total / (blk + 1024);
-	    if (nblk > 32)
-		nblk = 32;
-	    size_t streams = nblk * (size_t)w;
-	    if (streams > 64)
-		streams = 64;
-	    if (streams > best_streams) {
-		best_streams = streams;
-		best_wpb = w;
-	    }
-	}
-	if (ce->wpb && ce->prefix > 0) {
-	    const size_t blk = ((table + (size_t)ce->wpb * per_stream + 16 + 128 + 15) & ~(size_t)15);
-	    if (blk <= smem_max)
-		best_wpb = ce->wpb;
-	}
-	if (pf.nbnd <= 32u && best_wpb > 0 && pf.S <= 512u && g->bit_nsamples <= ring3 && ce->twc_n) {
-	    sh->mode = 3;
-	    G = 32;
-	    W = lb;
-	    L = 1;
-	    sh->pfx_tw_stage = tw_stage;
-	    wpb = best_wpb;
-	    ring = ring3;
-	    sh->tw_in_smem = 1;
-	    sh->smem = ((table + (size_t)wpb * per_stream + 16 + 128 + 15) & ~(size_t)15);
+	    sh->ring = 0;			/* not even one ring fits */
+	    return false;
 	}
     }
-    /* the table as staged: the window-relative entries, or (per-candidate kernel with the sliding fine
-     * search) the absolute-index extension the host layer prepared, if it still fits */
-    sh->geo.tw_entries = sh->mode == 3 ? sh->pfx_tw_stage : g->bit_nsamples;
-    sh->slide = 0;
-    if (sh->mode == 0 && lc && lc->slide && g->tw_entries > g->bit_nsamples && sh->tw_in_smem) {
-	const size_t extra = (size_t)(g->tw_entries - g->bit_nsamples) * sizeof(float4)
-	    * (per_stream_tw ? (size_t)wpb * (32 / G) : 1u);
-	if (sh->smem + extra <= smem_max) {
-	    sh->smem += extra;
-	    sh->geo.tw_entries = g->tw_entries;
-	    sh->slide = 1;
-	}
-    }
+    sh->mode = 0;
     sh->G = G;
     sh->W = W;
     sh->L = L;
     sh->wpb = wpb;
     sh->ring = ring;
-    {
-	const unsigned base_need = need_floats + 8u + RING_BLOCK;
-	const unsigned slack = ring > base_need ? ring - base_need : 0u;
-	sh->lookahead = slack < max_advance ? slack : max_advance;
+    sh->smem = smem;
+    return fast && g->bit_nsamples <= FAST_MAX_N * (unsigned)L && sh->tw_in_smem;
+}
+
+/* mode 1, the generic kernel: G = 32, no ring (it reads global memory), the table in shared memory if it fits */
+static void plan_generic(const CudaEngine *ce, const fsk_b200_geom *g, Shape *sh)
+{
+    const size_t tw_bytes = (size_t)g->bit_nsamples * sizeof(float4);
+    const size_t scr_only = (size_t)g->n_bits * sizeof(float2) + 16;
+    int L = 1;
+    while ((unsigned)(L * 2) * g->n_bits <= 32u)
+	L *= 2;
+    sh->mode = 1;
+    sh->G = 32;
+    sh->W = (int)((g->n_bits + 32 / L - 1) / (32 / L));
+    sh->L = L;
+    sh->wpb = ce->wpb ? ce->wpb : 4;
+    sh->ring = 0;
+    sh->tw_in_smem = tw_bytes <= 24 * 1024;
+    sh->smem = ((sh->tw_in_smem ? tw_bytes : 0) + (size_t)sh->wpb * scr_only + 15) & ~(size_t)15;
+    if (sh->smem > (size_t)ce->smem_optin) {
+	sh->tw_in_smem = 0;
+	sh->smem = ((size_t)sh->wpb * scr_only + 15) & ~(size_t)15;
     }
-    sh->geo.lanes_per_window = (unsigned)L;
-    /* one block per wpb*(32/G) streams: the hardware block scheduler hands out
-     * streams as SM resources free up (streams differ in length and work) */
-    const size_t streams_per_block = (size_t)wpb * (32 / G);
+}
+
+/* mode 2, the shared-segment kernel, on the per-candidate plan pc (its G, ring, warps and shared memory): the
+ * (W, L) split whose period slots hold all of this mode's searches, if its windows tile */
+static bool plan_shared(const CudaEngine *ce, const fsk_b200_geom *g, const fsk_b200_loopc *lc, const Shape &pc,
+	Shape *sh)
+{
+    int W = 0, L = 0;
+    fsk_b200_mplan mp;
+    if (!split_for_multi(pc.G, g->n_bits + 1u, &W, &L) || g->bit_nsamples > FAST_MAX_N * (unsigned)L
+	    || fsk_b200_mplan_build(g, lc, (unsigned)(W * (pc.G / L)), &mp) != 0)
+	return false;
+    *sh = pc;
+    sh->mode = 2;
+    sh->W = W;
+    sh->L = L;
+    sh->mplan = mp;
+    sh->mplan.always = ce->multi >= 2 || ce->multi < 0;
+    return true;
+}
+
+/* shared memory of a mode-3 block of w streams: the rotation table, the streams, 16 + 128 bytes of barriers */
+static size_t pfx_block_bytes(size_t table, size_t per_stream, int w)
+{
+    return (table + (size_t)w * per_stream + 16 + 128 + 15) & ~(size_t)15;
+}
+
+/* mode 3, the chunk-prefix table kernel on a ring of `ring` floats: one stream per warp, one lane per window
+ * boundary of a candidate, the ring without its mirror plus the table per stream; false where the mode's
+ * boundaries, its search span or the ring do not fit it */
+static bool plan_prefix(const CudaEngine *ce, const fsk_b200_geom *g, const fsk_b200_loopc *lc, unsigned need_floats,
+	unsigned ring, Shape *sh)
+{
+    fsk_b200_pfx pf;
+    memset(&pf, 0, sizeof(pf));
+    const unsigned nb = g->n_bits, N = g->bit_nsamples;
+    pf.tiles = 1;
+    for (unsigned w = 0; w + 1 < nb; w++)
+	if (g->bit_begin[w + 1] != g->bit_begin[w] + N)
+	    pf.tiles = 0;
+    pf.nbnd = pf.tiles ? nb + 1u : 2u * nb;
+    /* candidate slots: aligned power-of-two slots reduce by butterflies; slots of exactly nbnd lanes packed
+     * back to back are used only where they hold more candidates per round (9 boundaries: 3 instead of 2) */
+    unsigned bs2 = 8;
+    int lb = 3;
+    while (bs2 < pf.nbnd) {
+	bs2 <<= 1;
+	lb++;
+    }
+    if (pf.nbnd <= 32u && 32u / bs2 == 32u / pf.nbnd) {
+	pf.bs = bs2;
+	pf.pow2 = 1;
+    } else {
+	pf.bs = pf.nbnd;
+	pf.pow2 = 0;
+	lb = 1;			/* the kernel's template code for packed slots */
+    }
+    pf.cpr = pf.bs ? 32u / pf.bs : 0u;
+    /* 16-byte pieces of the widest search span (it may start up to 3 samples into its first piece), dealt
+     * to the 32 lanes in runs of S pieces.  S odd: the lanes walk their runs in step, S pieces apart, and
+     * only an odd stride spreads a quarter-warp's 16-byte accesses over all banks; the same for the table
+     * rows (tstride) */
+    const unsigned npieces = (3u + need_floats) / 4u + 1u;
+    pf.S = ((npieces + 31u) / 32u) | 1u;
+    pf.inv_S = 1.0f / (float)pf.S;
+    pf.tstride = ((pf.S + 1u) / 2u) | 1u;
+    const unsigned F = (unsigned)ce->tw_fftsize;
+    const unsigned g4 = (F % 4u == 0) ? 4u : (F % 2u == 0) ? 2u : 1u;
+    pf.fp = F / g4;
+    pf.s4 = 4u / g4;
+    pf.inv_fp = 1.0f / (float)pf.fp;
+    pf.loc[0][0][0] = pf.loc[0][2][0] = 1.0f;	/* j = 0 as (1, +0): the shared tone phase gives (1, -0) */
+    for (unsigned j = 1; j <= 7; j++) {
+	float t[4];
+	fsk_b200_tone_pair_phase(ce->tw_bm, ce->tw_bs, j, F, t);
+	for (unsigned k = 0; k < 4; k++)
+	    pf.loc[j >> 1][k][j & 1u] = t[k];
+    }
+    for (unsigned k = 0; k < 4; k++) {		/* the rx loop's four searches, src/minimodem.c:1236-1263, :1357-1368 */
+	const unsigned carrier = k & 1u, fine = k >> 1;
+	const unsigned tmax_k = carrier ? lc->try_max_carrier : lc->try_max_nocarrier;
+	const unsigned first = carrier ? lc->nsamples_overscan : 0u;
+	unsigned step = tmax_k / (fine ? 8u : 3u);
+	if (step == 0)
+	    step = 1;
+	fsk_b200_pfx_kind &kd = pf.kind[k];
+	kd.step = step;
+	kd.k_up = tmax_k > first ? (tmax_k - 1u - first) / step : 0u;
+	kd.k_dn = first / step < kd.k_up ? first / step : kd.k_up;
+	kd.ncands = tmax_k > first ? 1u + kd.k_up + kd.k_dn : 0u;
+    }
+    const unsigned tw_stage = pf.fp + (pf.S + 2u) * pf.s4;	/* one period and a lane-run */
+    const size_t table = (size_t)tw_stage * sizeof(float4);
+    const size_t per_stream = ((size_t)ring + 4u * pf.S + 8u) * 4 + (size_t)nb * sizeof(float2) + 16
+	+ (32u * (size_t)pf.tstride + 32u + (pf.pow2 ? 0u : 32u)) * sizeof(float4);	/* ring + mirror, scratch, barriers, table + totals (+ slot-sum scratch) */
+    /* warps (= streams) per block: the most resident streams per SM (each block pays the table and 1 KiB) */
+    const size_t smem_max = (size_t)ce->smem_optin;
+    const size_t sm_total = smem_max + 1024;
+    int wpb = 0;
+    size_t best_streams = 0;
+    for (int w = 1; w <= FSK_PFX_MAXTHREADS / 32 && pfx_block_bytes(table, per_stream, w) <= smem_max; w++) {
+	size_t nblk = sm_total / (pfx_block_bytes(table, per_stream, w) + 1024);
+	if (nblk > 32)
+	    nblk = 32;
+	size_t streams = nblk * (size_t)w;
+	if (streams > 64)
+	    streams = 64;
+	if (streams > best_streams) {
+	    best_streams = streams;
+	    wpb = w;
+	}
+    }
+    if (ce->wpb && ce->prefix > 0 && pfx_block_bytes(table, per_stream, ce->wpb) <= smem_max)
+	wpb = ce->wpb;
+    if (pf.nbnd > 32u || wpb == 0 || pf.S > 512u || N > ring)
+	return false;
+    sh->mode = 3;
+    sh->G = 32;
+    sh->W = lb;
+    sh->L = 1;
+    sh->wpb = wpb;
+    sh->ring = ring;
+    sh->tw_in_smem = 1;
+    sh->smem = pfx_block_bytes(table, per_stream, wpb);
+    sh->pfx = pf;
+    sh->pfx_tw_stage = tw_stage;
+    return true;
+}
+
+/* what every plan ends with: the table entries staged, the look-ahead the ring leaves (up to max_advance),
+ * and one block per wpb * (32 / G) streams -- the hardware block scheduler hands out streams as SM resources
+ * free up (streams differ in length and work) */
+static void plan_finish(const fsk_b200_geom *g, unsigned need_floats, unsigned max_advance, size_t nstreams, Shape *sh)
+{
+    sh->geo.tw_entries = sh->mode == 3 ? sh->pfx_tw_stage : g->bit_nsamples;
+    const unsigned base_need = need_floats + 8u + RING_BLOCK;
+    const unsigned slack = sh->ring > base_need ? sh->ring - base_need : 0u;
+    sh->lookahead = slack < max_advance ? slack : max_advance;
+    sh->geo.lanes_per_window = (unsigned)sh->L;
+    const size_t streams_per_block = (size_t)sh->wpb * (32 / sh->G);
     size_t blocks = (nstreams + streams_per_block - 1) / streams_per_block;
     if (blocks > 0x7fffffff)
 	blocks = 0x7fffffff;
     sh->blocks = (int)(blocks ? blocks : 1);
-    return 0;
+}
+
+/* the launch shape of an rx call over nstreams streams: the first of prefix table, shared segments,
+ * per candidate and generic that the engine's knobs allow, the mode suits and that fits */
+static void rx_shape(const CudaEngine *ce, const fsk_b200_geom *g, const fsk_b200_loopc *lc, size_t nstreams,
+	bool per_stream_tw, Shape *sh)
+{
+    const unsigned tmax = lc->try_max_nocarrier > lc->try_max_carrier ? lc->try_max_nocarrier : lc->try_max_carrier;
+    const unsigned max_advance = tmax - 1u + lc->frame_nsamples;	/* :1407, overscan >= 0 */
+    const unsigned need_floats = tmax - 1u + g->span;
+    Shape pc = {};
+    pc.geo = *g;
+    const bool per_cand = plan_per_candidate(ce, g, need_floats, per_stream_tw, &pc);
+    /* a forced ring (FSK_B200_RING, tune) sizes the prefix-table ring as the per-candidate plan left it:
+     * rounded up to whole blocks and at least the minimum, or 0 (no prefix-table kernel) where the
+     * per-candidate kernel cannot run the mode */
+    const unsigned pfx_ring = !ce->ring ? ring_min_for(need_floats) : per_cand ? pc.ring : 0u;
+    const bool prefix = !per_stream_tw && ce->prefix && ce->twc_n
+	&& (ce->prefix > 0 || g->bit_nsamples >= FSK_PREFIX_MIN_N);
+    const bool shared = !per_stream_tw && per_cand && ce->multi
+	&& (ce->multi > 0 || g->bit_nsamples >= FSK_MULTI_MIN_N);
+    *sh = Shape{};
+    sh->geo = *g;
+    if (prefix && plan_prefix(ce, g, lc, need_floats, pfx_ring, sh))
+	;			/* mode 3 */
+    else if (shared && plan_shared(ce, g, lc, pc, sh))
+	;			/* mode 2 */
+    else if (per_cand)
+	*sh = pc;
+    else
+	plan_generic(ce, g, sh);
+    plan_finish(g, need_floats, max_advance, nstreams, sh);
+    /* the per-candidate kernel's sliding fine search: the absolute-index table extension the host layer
+     * prepared, if it still fits (one per stream with per-stream tables) */
+    if (sh->mode == 0 && lc->slide && g->tw_entries > g->bit_nsamples && sh->tw_in_smem) {
+	const size_t extra = (size_t)(g->tw_entries - g->bit_nsamples) * sizeof(float4)
+	    * (per_stream_tw ? (size_t)sh->wpb * (32 / sh->G) : 1u);
+	if (sh->smem + extra <= (size_t)ce->smem_optin) {
+	    sh->smem += extra;
+	    sh->geo.tw_entries = g->tw_entries;
+	    sh->slide = 1;
+	}
+    }
+}
+
+/* kernel k launched at shape sh: its dynamic shared memory allowed, the launch counted */
+template <typename K, typename... Args>
+static cudaError_t launch_shape(K k, const Shape &sh, cudaStream_t st, const Args &...args)
+{
+    cudaError_t e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sh.smem);
+    if (e != cudaSuccess)
+	return e;
+    FSK_LAUNCH(k, sh.blocks, sh.wpb * 32, sh.smem, st, args...);
+    g_launches++;
+    return cudaGetLastError();
 }
 
 template <int G, int W, int L, int MODE>
 static cudaError_t launch_find_t(const Shape &sh, const CudaEngine *ce, const FindArgs &a, cudaStream_t st)
 {
-    cudaError_t e = cudaFuncSetAttribute(k_find_frame<G, W, L, MODE>,
-	    cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sh.smem);
-    if (e != cudaSuccess)
-	return e;
-    FSK_LAUNCH((k_find_frame<G, W, L, MODE>), sh.blocks, sh.wpb * 32, sh.smem, st, sh.geo, ce->d_tw,
-	    sh.tw_in_smem, sh.ring, a);
-    g_launches++;
-    return cudaGetLastError();
+    return launch_shape(k_find_frame<G, W, L, MODE>, sh, st, sh.geo, ce->d_tw, sh.tw_in_smem,
+	    sh.ring, a);
 }
 
 extern "C" int fsk_b200_cuda_find_frame_batch(void *p, const fsk_b200_geom *g, const float *samples,
@@ -2159,9 +2188,13 @@ extern "C" int fsk_b200_cuda_find_frame_batch(void *p, const fsk_b200_geom *g, c
     }
     if (engine_device_check(ce, "find_frame_batch"))
 	return -EINVAL;
-    Shape sh;
+    Shape sh = {};
+    sh.geo = *g;
     /* the ring is sized for the widest search of the rx loop: 1.5 bits + span */
-    pick_shape(ce, g, g->span + 2u * g->bit_nsamples + 8u, 0, nstreams, &sh);
+    const unsigned need_floats = g->span + 2u * g->bit_nsamples + 8u;
+    if (!plan_per_candidate(ce, g, need_floats, false, &sh))
+	plan_generic(ce, g, &sh);
+    plan_finish(g, need_floats, 0, nstreams, &sh);
     const FindArgs a = { samples, (unsigned)nstreams, stride, offset, nvalid, try_first, try_max,
 	try_step, limit, expect_sel, frames, reinterpret_cast<float2 *>(bit_mags) };
     cudaStream_t st = (cudaStream_t)stream;
@@ -2188,24 +2221,18 @@ template <int G, int W, int L, int MODE, int FILL, int SRC = 0, int AUTO = 0>
 static cudaError_t launch_rx_t(const Shape &sh, const CudaEngine *ce, const fsk_b200_loopc *lc,
 	const RxArgs &a, cudaStream_t st, const AutoArgs &au)
 {
-    cudaError_t e = cudaFuncSetAttribute(k_rx<G, W, L, MODE, FILL, SRC, AUTO>,
-	    cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sh.smem);
-    if (e != cudaSuccess)
-	return e;
     /* AUTO: no block-wide table is staged (tw_in_smem 0); every stream fills its own */
-    FSK_LAUNCH((k_rx<G, W, L, MODE, FILL, SRC, AUTO>), sh.blocks, sh.wpb * 32, sh.smem, st, sh.geo, *lc,
-	    MODE == 3 ? ce->d_twc : ce->d_tw, AUTO ? 0u : sh.tw_in_smem, sh.ring, sh.lookahead, a, sh.mplan, ce->d_tw, sh.pfx,
-	    au);
-    g_launches++;
-    return cudaGetLastError();
+    return launch_shape(k_rx<G, W, L, MODE, FILL, SRC, AUTO>, sh, st, sh.geo, *lc,
+	    MODE == 3 ? ce->d_twc : ce->d_tw, AUTO ? 0u : sh.tw_in_smem, sh.ring, sh.lookahead, a,
+	    sh.mplan, ce->d_tw, sh.pfx, au);
 }
 
 /* --auto-carrier: the shapes of the per-candidate kernel with a tone table per stream (AUTO 1), in float
- * and int16 builds -- what pick_shape chooses for the presets of fsk_b200_rx_config_for_mode at 8 and 48 kHz */
+ * and int16 builds -- what rx_shape chooses for the presets of fsk_b200_rx_config_for_mode at 8 and 48 kHz */
 #define AUTO_COMBOS(X) \
     X(8, 3, 2) X(16, 2, 4) X(16, 3, 4) X(16, 3, 1) X(32, 1, 4) X(32, 2, 4) X(32, 3, 2)
 
-/* (cos, -sin)(2 pi r / fftsize): the expression of fsk_b200_cuda_set_table with r = (b * n) mod fftsize, so
+/* (cos, -sin)(2 pi r / fftsize): the tone phase of fsk_b200_cuda_set_table with r = (b * n) mod fftsize, so
  * every per-stream table entry is bit-identical to the one a fixed-tone engine builds */
 extern "C" int fsk_b200_cuda_set_unit_table(void *p, int fftsize)
 {
@@ -2217,23 +2244,14 @@ extern "C" int fsk_b200_cuda_set_unit_table(void *p, int fftsize)
     float2 *h = (float2 *)malloc(sizeof(float2) * (size_t)fftsize);
     if (!h)
 	return -ENOMEM;
-    const double F = (double)fftsize;
-    for (int r = 0; r < fftsize; r++) {
-	const double a = 2.0 * M_PI * (double)r / F;
-	h[r].x = (float)cos(a);
-	h[r].y = (float)-sin(a);
-    }
-    cudaFree(ce->d_unit);
-    ce->d_unit = NULL;
+    for (int r = 0; r < fftsize; r++)
+	fsk_b200_tone_phase(1, (unsigned)r, (unsigned)fftsize, &h[r].x);
     ce->unit_f = 0;
-    cudaError_t err = cudaMalloc(&ce->d_unit, sizeof(float2) * (size_t)fftsize);
-    if (err == cudaSuccess)
-	err = cudaMemcpy(ce->d_unit, h, sizeof(float2) * (size_t)fftsize, cudaMemcpyHostToDevice);
-    if (err == cudaSuccess)
-	err = cudaDeviceSynchronize();
+    cudaError_t err;
+    const int rc = upload_table((void **)&ce->d_unit, &ce->unit_cap, h, sizeof(float2) * (size_t)fftsize, &err);
     free(h);
-    if (err != cudaSuccess) {
-	fsk_b200_set_error("set_unit_table: %s", cudaGetErrorString(err));
+    if (rc) {
+	fsk_b200_set_error("set_unit_table: %s", cudaGetErrorString(rc == -ENOMEM ? cudaGetLastError() : err));
 	return -EIO;
     }
     ce->unit_f = fftsize;
@@ -2281,15 +2299,6 @@ static RxLaunch rx_instance(const Shape &sh, const CudaEngine *ce)
 	return launch_rx_t<32, 1, 1, 1, 0, SRC, 0>;
     }
     return NULL;
-}
-
-/* the launch shape of an rx call over nstreams streams */
-static void rx_shape(const CudaEngine *ce, const fsk_b200_geom *g, const fsk_b200_loopc *lc, size_t nstreams,
-	bool per_stream_tw, Shape *sh)
-{
-    const unsigned tmax = lc->try_max_nocarrier > lc->try_max_carrier ? lc->try_max_nocarrier : lc->try_max_carrier;
-    const unsigned max_advance = tmax - 1u + lc->frame_nsamples;	/* :1407, overscan >= 0 */
-    pick_shape(ce, g, tmax - 1u + g->span, max_advance, nstreams, sh, lc, per_stream_tw);
 }
 
 extern "C" int fsk_b200_cuda_rx_s16_runs(void *p, const fsk_b200_geom *g, const fsk_b200_loopc *lc, size_t nstreams)
@@ -2503,6 +2512,18 @@ fail:
 #undef HOST_TRY
 }
 
+/* after a single-kernel launch: count it, and report a launch error as "<what> launch: <error>" */
+static int launched(const char *what)
+{
+    g_launches++;
+    const cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) {
+	fsk_b200_set_error("%s launch: %s", what, cudaGetErrorString(e));
+	return -EIO;
+    }
+    return 0;
+}
+
 extern "C" int fsk_b200_cuda_s16_to_f32(const int16_t *src, float *dst, size_t nstreams, size_t stride,
 	void *stream)
 {
@@ -2516,13 +2537,7 @@ extern "C" int fsk_b200_cuda_s16_to_f32(const int16_t *src, float *dst, size_t n
     } else {
 	FSK_LAUNCH(k_s16_to_f32_scalar, (unsigned)((n + 255) / 256), 256, 0, (cudaStream_t)stream, src, dst, n);
     }
-    g_launches++;
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) {
-	fsk_b200_set_error("s16_to_f32 launch: %s", cudaGetErrorString(e));
-	return -EIO;
-    }
-    return 0;
+    return launched("s16_to_f32");
 }
 
 /* one warp per row; k channels (states) per row, tone_bands optional ([nrows * k][2]), row_events optional
@@ -2544,13 +2559,7 @@ extern "C" int fsk_b200_cuda_stream_push(int elem, void *samples, size_t nrows, 
 	FSK_LAUNCH(k_stream_push<float>, (unsigned)blocks, threads, 0, (cudaStream_t)stream, (float *)samples,
 		(unsigned)nrows, stride, fill, k, tone_bands, nbands, states, (const float *)chunk, chunk_stride,
 		chunk_len, chunk_len_all, dropped, row_events);
-    g_launches++;
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) {
-	fsk_b200_set_error("stream_push launch: %s", cudaGetErrorString(e));
-	return -EIO;
-    }
-    return 0;
+    return launched("stream_push");
 }
 
 extern "C" int fsk_b200_cuda_decode(int kind, unsigned shift, unsigned n_data_bits, int msb_first,
@@ -2578,13 +2587,7 @@ extern "C" int fsk_b200_cuda_decode(int kind, unsigned shift, unsigned n_data_bi
 	    return -EINVAL;
     }
 #undef DECODE_CASE
-    g_launches++;
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) {
-	fsk_b200_set_error("decode launch: %s", cudaGetErrorString(e));
-	return -EIO;
-    }
-    return 0;
+    return launched("decode");
 }
 
 /* the drop-in fsk_find_frame: one stream, host samples */
@@ -2658,13 +2661,7 @@ extern "C" int fsk_b200_cuda_detect_carrier_batch(int fftsize, const float *samp
     const size_t blocks = (nstreams * 32 + threads - 1) / threads;
     FSK_LAUNCH(k_detect_carrier, (unsigned)blocks, threads, 0, (cudaStream_t)stream, samples, (unsigned)nstreams,
 	    stride, offset, nsamples, fftsize, nbands, min_mag_threshold, out_band);
-    g_launches++;
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) {
-	fsk_b200_set_error("detect_carrier_batch launch: %s", cudaGetErrorString(e));
-	return -EIO;
-    }
-    return 0;
+    return launched("detect_carrier_batch");
 }
 
 extern "C" void *fsk_b200_cuda_upload(const void *host, size_t bytes)
@@ -2740,8 +2737,7 @@ extern "C" int fsk_b200_cuda_tx_synth(const fsk_b200_tx_plan *p, const void *lut
 	    tx_launch<float, true, true>(p, lut, &m, (cudaStream_t)stream);
 	else
 	    tx_launch<int16_t, true, true>(p, lut, &m, (cudaStream_t)stream);
-	g_launches++;
-	cudaError_t e = cudaGetLastError();
+	const int rc = launched("tx");
 	if (scratch) {
 #ifdef FSK_EMU
 	    cudaFree(scratch);
@@ -2749,11 +2745,7 @@ extern "C" int fsk_b200_cuda_tx_synth(const fsk_b200_tx_plan *p, const void *lut
 	    cudaFreeAsync(scratch, (cudaStream_t)stream);
 #endif
 	}
-	if (e != cudaSuccess) {
-	    fsk_b200_set_error("tx launch: %s", cudaGetErrorString(e));
-	    return -EIO;
-	}
-	return 0;
+	return rc;
     }
     /* the pair per stream is its own instance: the fixed-pair instances keep their code */
     if (p->float_samples && io->tones)
@@ -2764,11 +2756,5 @@ extern "C" int fsk_b200_cuda_tx_synth(const fsk_b200_tx_plan *p, const void *lut
 	tx_launch<int16_t, true>(p, lut, io, (cudaStream_t)stream);
     else
 	tx_launch<int16_t, false>(p, lut, io, (cudaStream_t)stream);
-    g_launches++;
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) {
-	fsk_b200_set_error("tx launch: %s", cudaGetErrorString(e));
-	return -EIO;
-    }
-    return 0;
+    return launched("tx");
 }
