@@ -1720,6 +1720,195 @@ __device__ __forceinline__ void ring_zero(const Ring rg, unsigned pos, unsigned 
     }
 }
 
+/* a row's samples and the generic path's reader of them: float32 (SRC 0) or int16 PCM (SRC 1) */
+template <int SRC> struct RowOf { typedef float T; typedef GlobalSrc Src; };
+template <> struct RowOf<1> { typedef int16_t T; typedef GlobalSrc16 Src; };
+
+/* One stream's ring fill in the rx loop.  FILL 0: cp.async blocks by all lanes of the group (int16 rows land
+ * in the upper half of each block and are widened in place by `ready`); FILL 1: cp.async.bulk by lane 0,
+ * completion on two mbarriers used in turn.  The caller keeps `pos`; the searches read `pos_off`. */
+template <int G, int FILL, int SRC>
+struct StreamRing {
+    typedef typename RowOf<SRC>::T T;
+    static constexpr unsigned AL = SRC ? 7u : 3u;	/* 16-byte source chunks: 4 floats, or 8 int16 */
+    const Ring rg;
+    const T *const x;
+    const unsigned n, n4;		/* rows are readable up to a multiple of 4 (n <= 2^32 - 4) */
+    const unsigned need_max, span;	/* need_max: the samples past `pos` an iteration reads at most */
+    const unsigned g, gmask, bar0, bar1;
+    const unsigned dst0;		/* this lane's first 16-byte chunk of the ring */
+    unsigned pos_off;			/* the ring offset of `pos` */
+    /* the absolute index up to which the ring content has been REQUESTED (copies issued or zeros stored): 64-bit,
+     * as the requests run past the end of the row (zeros), which may lie just below 2^32 (pos < n stays 32-bit) */
+    unsigned long long filled;
+    unsigned long long conv;		/* SRC 1: blocks up to `conv` (ring offset coff) are widened */
+    unsigned coff;
+    unsigned fdst;			/* block fill: this lane's first 16-byte chunk of the block at `filled`, */
+    const T *fsrc;			/* in the ring and in the row, carried instead of recomputed */
+    unsigned kphase = 0;		/* bulk fill: number of barrier phases armed */
+    bool tail_fix = false;		/* bulk fill: [n, n4) holds row padding, not zeros */
+
+    __device__ __forceinline__ StreamRing(const Ring &r, unsigned bars, const T *row, unsigned len, unsigned pos,
+	    unsigned need, unsigned sp, unsigned lane_g, unsigned mask)
+	: rg(r), x(row), n(len), n4((len + 3u) & ~3u), need_max(need), span(sp), g(lane_g), gmask(mask),
+	  bar0(bars), bar1(bars + 8u), dst0(r.ring_s + 16u * lane_g) { start(pos); }
+
+    /* the request limit of an iteration at p: its largest window `extra` samples further on, and no more
+     * than the ring holds */
+    __device__ __forceinline__ unsigned long long reach(unsigned p, unsigned extra) const
+    {
+	return min(((unsigned long long)p + extra + need_max + 3u) & ~3ull, (unsigned long long)(p & ~AL) + rg.R);
+    }
+
+    /* the barriers (bulk fill) and the first request */
+    __device__ __forceinline__ void open(unsigned pos)
+    {
+	if (FILL == 1 && g == 0) {
+	    mbar_init(bar0, 1);
+	    mbar_init(bar1, 1);
+	    mbar_fence_init();
+	}
+	__syncwarp(gmask);
+	request(reach(pos, 0u), pos);
+    }
+
+    /* FILL 0: whole blocks while they start below `to` and still fit in a ring whose oldest live sample
+     * is `base` */
+    __device__ __forceinline__ void request_at(unsigned long long to, unsigned base)
+    {
+	const unsigned long long lim = min(to, (unsigned long long)(base & ~AL) + rg.R - (RING_BLOCK - 1u));
+	while (filled < lim) {
+	    if constexpr (SRC) {		/* int16 rows: landing zone = upper half of the block */
+		if (filled + RING_BLOCK <= n)
+		    ring_block16<G>(rg.ring_s, (fdst - dst0) >> 2, x + filled, g);
+		else
+		    ring_block16_tail<G>(rg.ring_s, (fdst - dst0) >> 2, x, n, filled, g);
+	    } else if (filled + RING_BLOCK <= n)	/* the common case: all of it valid */
+		ring_block_at<G>(fdst, fsrc, rg.ring_s + rg.pad * 4u, rg.R);
+	    else				/* end of the stream: zero fill */
+		ring_block_tail<G>(rg, rg.ring_s, (fdst - dst0) >> 2, x, n, filled, g);
+	    filled += RING_BLOCK;
+	    fsrc += RING_BLOCK;
+	    fdst += RING_BLOCK * 4u;
+	    if (fdst == dst0 + rg.R * 4u)
+		fdst = dst0;
+	}
+	cp_async_commit();
+    }
+
+    /* request the ring content up to absolute index `to` (rounded up to whole blocks) */
+    __device__ __forceinline__ void request(unsigned long long to, unsigned pos)
+    {
+	if constexpr (FILL == 0)
+	    request_at(to, pos);
+	else {
+	    static_assert(SRC == 0, "bulk fill: float rows only");
+	    const unsigned to_b = (unsigned)min(to, (unsigned long long)n4);
+	    const unsigned from_b = (unsigned)min(filled, (unsigned long long)to_b);
+	    if (g == 0)
+		ring_issue_bulk(rg, x, pos, pos_off, from_b, to_b, (kphase & 1u) ? bar1 : bar0);
+	    if (n < n4 && from_b < n4 && to_b == n4 && to_b > from_b)
+		tail_fix = true;
+	    kphase++;
+	    if (to > max(filled, (unsigned long long)n4))	/* past the end of the stream: zeros */
+		ring_zero<G>(rg, pos, pos_off, max(filled, (unsigned long long)n4), to, g);
+	    if (to > filled)
+		filled = to;
+	}
+    }
+
+    /* The top of the iteration at `pos`.  Its samples were normally requested an iteration ago (request_next);
+     * what is missing -- a launch's first iteration, a restarted ring, the bulk fill -- is requested here with
+     * what the next iteration can need (it starts at most `ahead` samples further).  Returns whether copies
+     * are pending: the search waits for float cp.async itself; int16 rows are widened, the bulk fill settles. */
+    __device__ __forceinline__ bool ready(unsigned pos, unsigned try_max, unsigned ahead)
+    {
+	const unsigned long long need_now = ((unsigned long long)pos + try_max - 1u + span + 3u) & ~3ull;
+	const bool late = filled < need_now;	/* part of this window is only now requested */
+	if (FILL != 0 || late)
+	    request(reach(pos, ahead), pos);
+	if (SRC) {
+	    cp_async_wait<0>();
+	    __syncwarp(gmask);
+	    for (; conv < filled; conv += RING_BLOCK) {
+		ring_widen16<G>(rg, coff, g, gmask);
+		coff += RING_BLOCK;
+		if (coff == rg.R)
+		    coff = 0;
+	    }
+	    return false;
+	}
+	if (FILL == 0)
+	    return true;
+	settle(late || tail_fix);
+	if (tail_fix) {
+	    __syncwarp(gmask);
+	    if (n >= (pos & ~3u))
+		ring_zero<G>(rg, pos, pos_off, n, n4, g);
+	    tail_fix = false;
+	}
+	__syncwarp(gmask);
+	return false;
+    }
+
+    /* FILL 0, once the searches are over: the samples before the next start `npos` are dead, so ask for the
+     * next iteration's now (unless the advance skips past everything requested: filled < (npos & ~AL)) */
+    __device__ __forceinline__ void request_next(unsigned npos, unsigned ahead)
+    {
+	__syncwarp(gmask);	/* every read of this window precedes the copies */
+	request_at(reach(npos, ahead), npos);
+    }
+
+    /* wait until nothing is in flight into this ring */
+    __device__ __forceinline__ void drain()
+    {
+	if (FILL == 0)
+	    cp_async_wait<0>();
+	else
+	    settle(true);
+	__syncwarp(gmask);
+    }
+
+    /* restart the ring at `pos`, as a resumed stream starts it */
+    __device__ __forceinline__ void restart(unsigned pos)
+    {
+	drain();
+	start(pos);
+    }
+
+    /* `pos` has just moved `adv` samples on (adv < R by construction) */
+    __device__ __forceinline__ void advance(unsigned pos, unsigned adv)
+    {
+	pos_off = ring_wrap(pos_off + adv, rg.R);
+	if (filled < (pos & ~AL))		/* skipped past everything requested so far */
+	    restart(pos);
+	__syncwarp(gmask);	/* every read of this window precedes the next copies */
+    }
+
+private:
+    __device__ __forceinline__ void start(unsigned pos)
+    {
+	filled = pos & ~AL;
+	pos_off = pos & AL;
+	fdst = dst0;
+	fsrc = x + filled + 4u * g;
+	conv = filled;
+	coff = 0;
+    }
+
+    /* bulk fill: wait for everything requested before the latest request (all of it if `all`) */
+    __device__ __forceinline__ void settle(bool all) const
+    {
+	if (kphase >= 2u)
+	    wait_phase(kphase - 2u);
+	if (all && kphase >= 1u)
+	    wait_phase(kphase - 1u);
+    }
+
+    /* phase k (0-based) lives on barrier k&1 with parity (k>>1)&1 */
+    __device__ __forceinline__ void wait_phase(unsigned k) const { mbar_wait((k & 1u) ? bar1 : bar0, (k >> 1) & 1u); }
+};
+
 __device__ __forceinline__ void store_frame(fsk_b200_frame *f, unsigned long long bits, float conf,
 	float ampl, unsigned start)
 {

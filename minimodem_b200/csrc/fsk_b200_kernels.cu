@@ -306,9 +306,8 @@ k_find_frame(const __grid_constant__ fsk_b200_geom geo, const float4 *__restrict
 /* K2: the rx loop (src/minimodem.c:1137-1463) for whole streams            */
 /* ------------------------------------------------------------------------ */
 
-/* FILL 0: cp.async (LDGSTS) by all lanes of the group, the next iteration's samples asked for as
- * soon as the searches of this one are over rather than at the top of the next iteration;
- * FILL 1 (MODE 3): cp.async.bulk (TMA engine) issued by lane 0 with mbarrier completion. */
+/* FILL 0: cp.async (LDGSTS) by all lanes of the group; FILL 1 (MODE 3): cp.async.bulk (TMA engine) issued
+ * by lane 0 with mbarrier completion (StreamRing) */
 /* 128 threads x 4 blocks caps the kernel at 128 registers per thread: 8 blocks of 64 threads per
  * SM, which is also what the shared-memory rings allow */
 #ifndef FSK_MINBLOCKS
@@ -374,14 +373,15 @@ k_rx(const __grid_constant__ fsk_b200_geom geo, const __grid_constant__ fsk_b200
 	auto ended = [&]() { return (a.states[s].done & FSK_B200_STREAM_ENDED) != 0u; };
 	/* AUTO 2: the k channels of a row are consecutive streams; records, states and pairs stay per stream */
 	const unsigned row = AUTO == 2 ? s / au.k : s;
-	const float *x = SRC ? (const float *)nullptr : a.samples + (size_t)row * a.stride;
-	const int16_t *x16 = SRC ? a.samples16 + (size_t)row * a.stride : (const int16_t *)nullptr;
+	const typename RowOf<SRC>::T *x;	/* float32, or int16 PCM (SRC 1) */
+	if constexpr (SRC)
+	    x = a.samples16 + (size_t)row * a.stride;
+	else
+	    x = a.samples + (size_t)row * a.stride;
 	/* a row never extends past its stride or the 32-bit position limit (per-row lengths are caller data) */
 	const unsigned n = (unsigned)min(min((size_t)(a.nsamples ? a.nsamples[row] : a.nsamples_all), a.stride),
 		(size_t)FSK_B200_MAX_ROW_SAMPLES);
 	fsk_b200_frame *out = a.frames + (size_t)s * a.max_frames;
-	/* 16-byte chunks of the source line up with 16-byte chunks of the ring: 4 floats, or 8 int16 */
-	constexpr unsigned AL = SRC ? 7u : 3u;
 
 	unsigned pos = (unsigned)st.pos;
 	unsigned nframes = st.nframes;
@@ -415,118 +415,11 @@ k_rx(const __grid_constant__ fsk_b200_geom geo, const __grid_constant__ fsk_b200
 	    set_tones(bm, bsp);
 	}
 
-	/* ring bookkeeping (MODE 0): ring offset of `pos`, and the absolute index up to
-	 * which the ring content has been REQUESTED (copies issued or zeros stored).  The
-	 * requests run past the end of the row (zeros), and a row may end just below 2^32:
-	 * the absolute indices of the requests are 64-bit; pos < n <= 2^32 - 4 stays 32-bit */
-	unsigned pos_off = pos & AL;
-	unsigned long long filled = pos & ~AL;
-	unsigned long long conv = filled;		/* SRC 1: blocks up to `conv` (ring offset coff) are widened */
-	unsigned coff = 0;
-	const unsigned need_max = lc.try_max_nocarrier - 1u + geo.span;
-	const unsigned n4 = (n + 3u) & ~3u;		/* rows are readable up to a multiple of 4 (n <= 2^32 - 4) */
-	/* the request limit of an iteration at p: its largest window `extra` samples further on, and no
-	 * more than the ring holds */
-	auto reach = [&](unsigned p, unsigned extra) {
-	    return min(((unsigned long long)p + extra + need_max + 3u) & ~3ull, (unsigned long long)(p & ~AL) + R);
-	};
-	const unsigned bar0 = smem_u32(sm.bars), bar1 = bar0 + 8u;
-	unsigned kphase = 0;				/* bulk fill: number of barrier phases armed */
-	bool tail_fix = false;				/* bulk fill: [n, n4) holds row padding, not zeros */
-
-	const unsigned ring_s = rg.ring_s;
-	/* block fill: this lane's running source and destination (its first 16-byte chunk of
-	 * the block that starts at absolute index `filled`), carried instead of recomputed */
-	const unsigned dst0 = ring_s + 16u * g, dst_end = dst0 + R * 4u;
-	const unsigned mlim = ring_s + rg.pad * 4u;	/* chunks below this are mirrored behind the end */
-	unsigned fdst = dst0;
-	const float *fsrc = SRC ? x : x + filled + 4u * g;
-	/* request the ring content up to absolute index `to` (rounded up to whole blocks) */
-	auto request_at = [&](unsigned long long to, unsigned base) {
-	    /* FILL 0 only: whole blocks while they start below `to` and still fit in a ring
-	     * whose oldest live sample is `base` */
-	    const unsigned long long lim = min(to, (unsigned long long)(base & ~AL) + R - (RING_BLOCK - 1u));
-	    while (filled < lim) {
-		if (SRC) {				/* int16 rows: landing zone = upper half of the block */
-		    if (filled + RING_BLOCK <= n)
-			ring_block16<G>(ring_s, (fdst - dst0) >> 2, x16 + filled, g);
-		    else
-			ring_block16_tail<G>(ring_s, (fdst - dst0) >> 2, x16, n, filled, g);
-		} else if (filled + RING_BLOCK <= n)	/* the common case: all of it valid */
-		    ring_block_at<G>(fdst, fsrc, mlim, R);
-		else					/* end of the stream: zero fill */
-		    ring_block_tail<G>(rg, ring_s, (fdst - dst0) >> 2, x, n, filled, g);
-		filled += RING_BLOCK;
-		fsrc += RING_BLOCK;
-		fdst += RING_BLOCK * 4u;
-		if (fdst == dst_end)
-		    fdst = dst0;
-	    }
-	    cp_async_commit();
-	};
-	auto request = [&](unsigned long long to) {
-	    if (FILL == 0) {
-		request_at(to, pos);
-	    } else {
-		const unsigned to_b = (unsigned)min(to, (unsigned long long)n4);
-		const unsigned from_b = (unsigned)min(filled, (unsigned long long)to_b);
-		if (g == 0)
-		    ring_issue_bulk(rg, x, pos, pos_off, from_b, to_b, (kphase & 1u) ? bar1 : bar0);
-		if (n < n4 && from_b < n4 && to_b == n4 && to_b > from_b)
-		    tail_fix = true;
-		kphase++;
-		if (to > max(filled, (unsigned long long)n4))	/* past the end of the stream: zeros */
-		    ring_zero<G>(rg, pos, pos_off, max(filled, (unsigned long long)n4), to, g);
-		if (to > filled)
-		    filled = to;
-	    }
-	};
-	/* bulk fill: wait for everything requested before the latest request (all of it if `all`) */
-	auto settle = [&](bool all) {
-	    /* phase k (0-based) lives on barrier k&1 with parity (k>>1)&1 */
-	    if (kphase >= 2u) {
-		const unsigned k = kphase - 2u;
-		mbar_wait((k & 1u) ? bar1 : bar0, (k >> 1) & 1u);
-	    }
-	    if ((all || tail_fix) && kphase >= 1u) {
-		const unsigned k = kphase - 1u;
-		mbar_wait((k & 1u) ? bar1 : bar0, (k >> 1) & 1u);
-	    }
-	    if (tail_fix) {
-		__syncwarp(gmask);
-		if (n >= (pos & ~3u))
-		    ring_zero<G>(rg, pos, pos_off, n, n4, g);
-		tail_fix = false;
-	    }
-	    __syncwarp(gmask);
-	};
-	/* wait until nothing is in flight into this ring */
-	auto drain = [&]() {
-	    if (FILL == 0) {
-		cp_async_wait<0>();
-	    } else {
-		if (kphase >= 2u) {
-		    const unsigned k = kphase - 2u;
-		    mbar_wait((k & 1u) ? bar1 : bar0, (k >> 1) & 1u);
-		}
-		if (kphase >= 1u) {
-		    const unsigned k = kphase - 1u;
-		    mbar_wait((k & 1u) ? bar1 : bar0, (k >> 1) & 1u);
-		}
-	    }
-	    __syncwarp(gmask);
-	};
-	if (MODE != 1) {
-	    if (FILL == 1) {
-		if (g == 0) {
-		    mbar_init(bar0, 1);
-		    mbar_init(bar1, 1);
-		    mbar_fence_init();
-		}
-	    }
-	    __syncwarp(gmask);
-	    request(reach(pos, 0u));
-	}
+	/* MODE 0, 2, 3: the stream's ring and its fill (MODE 1 reads the row in global memory) */
+	StreamRing<G, FILL, SRC> ring(rg, smem_u32(sm.bars), x, n, pos, lc.try_max_nocarrier - 1u + geo.span,
+		geo.span, g, gmask);
+	if (MODE != 1)
+	    ring.open(pos);
 
 	for (;;) {
 	    if (pos >= n) { done = 1; break; }			/* :1176 */
@@ -547,10 +440,7 @@ k_rx(const __grid_constant__ fsk_b200_geom geo, const __grid_constant__ fsk_b200
 		    unsigned i = 0;
 		    int found = -1;
 		    for (; (float)i + sf <= (float)vring; i = (unsigned)((float)i + sf)) {
-			if (SRC)
-			    found = detect_group<G>(x16 + pos + i, sn, au, g, gmask);
-			else
-			    found = detect_group<G>(x + pos + i, sn, au, g, gmask);
+			found = detect_group<G>(x + pos + i, sn, au, g, gmask);
 			if (found >= 0)
 			    break;
 		    }
@@ -562,14 +452,7 @@ k_rx(const __grid_constant__ fsk_b200_geom geo, const __grid_constant__ fsk_b200
 			const unsigned adv = min((unsigned)((float)i + sf), vring);
 			pos += adv;
 			vring -= adv;
-			/* restart the ring at the new position, as a resumed stream starts it */
-			drain();
-			filled = pos & ~AL;
-			pos_off = pos & AL;
-			fdst = dst0;
-			fsrc = SRC ? x : x + filled + 4u * g;
-			conv = filled;
-			coff = 0;
+			ring.restart(pos);
 			__syncwarp(gmask);
 			continue;
 		    }
@@ -586,169 +469,126 @@ k_rx(const __grid_constant__ fsk_b200_geom geo, const __grid_constant__ fsk_b200
 	    const unsigned try_first = carrier ? lc.nsamples_overscan : 0u;	/* :1263 */
 	    const int sel = carrier ? 0 : 1;			/* :1270 data / sync string */
 
-	    bool pending = false;
-	    if (MODE != 1) {
-		/* The samples of this iteration were normally requested an iteration ago (FILL 0,
-		 * below); whatever is missing -- first iteration of a launch, a restarted ring, the
-		 * bulk fill -- is requested here together with what the next iteration can need
-		 * (it starts at most `lookahead` samples further) */
-		const unsigned long long need_now = ((unsigned long long)pos + try_max - 1u + geo.span + 3u) & ~3ull;
-		const bool late = filled < need_now;	/* part of this window is only now requested */
-		if (FILL != 0 || late)
-		    request(reach(pos, lookahead));
-		if (SRC) {
-		    /* int16 rows: everything requested so far has to land and be widened in place
-		     * before the search reads it (the float fill lets the search itself wait) */
-		    cp_async_wait<0>();
-		    __syncwarp(gmask);
-		    while (conv < filled) {
-			ring_widen16<G>(rg, coff, g, gmask);
-			conv += RING_BLOCK;
-			coff += RING_BLOCK;
-			if (coff == R)
-			    coff = 0;
-		    }
-		    pending = false;
-		} else if (FILL == 0) {
-		    /* the search waits for all copies itself, right before its first correlation */
-		    pending = true;
-		} else
-		    settle(late);
-	    }
-	    /* MODE 1 reads from `pos` on (pos < n here), so that its indices stay small */
-	    const GlobalSrc gsrc = { SRC ? x : x + pos, n - pos };
-	    const GlobalSrc16 gsrc16 = { SRC ? x16 + pos : x16, n - pos };
+	    bool pending = MODE != 1 && ring.ready(pos, try_max, lookahead);
 
-	    unsigned long long bits;
-	    float amplitude, confidence;
-	    unsigned frame_start;
-	    Found refined = { 0.f, 0.f, 0u, 0u, 0u };
-	    if (MODE != 1) {
-		/* one (inlined) search site, taken a second time for the refinement of :1357-1389: whether
-		 * that happens is a pure function of the first result and the loop state, so it is
-		 * decided here and the state machine below only merges the outcome */
-		Found first = { 0.f, 0.f, 0u, 0u, 0u };
-		unsigned step = try_step;
-		float limit = lc.confidence_search_limit;
-		int which = sel;
-		for (int pass = 0;; pass++) {
-		    nsearch++;
-		    Found f;
-		    if (MODE == 3) {
-			/* :1265, :1378 from the chunk-prefix table of this iteration's search span, built once
-			 * (before the coarse search) for both */
-			/* (shared-window addresses turned back into pointers here, so that the loads stay LDS/STS) */
-			const float *ringp = static_cast<const float *>(__cvta_shared_to_generic(rg.ring_s));
-			float4 *pre = static_cast<float4 *>(__cvta_shared_to_generic(pre_s));
-			float4 *tot = static_cast<float4 *>(__cvta_shared_to_generic(tot_s));
-			const float4 *twc = static_cast<const float4 *>(__cvta_shared_to_generic(tw_s));
-			const float4 *locp = static_cast<const float4 *>(__cvta_shared_to_generic(loc_s));
-			float4 *redp = static_cast<float4 *>(__cvta_shared_to_generic(red_s));
-			const unsigned base = pos_off & ~3u;
-			if (pass == 0) {
-			    if (pending) {
-				cp_async_wait<0>();
-				__syncwarp(gmask);
-				pending = false;
-			    }
-			    pfx_build(ringp, R, base, ((pos_off & 3u) + try_max - 1u + geo.span) / 4u + 1u, pre, tot,
-				    twc, locp, pg, pfl, lane);
+	    /* one (inlined) search site, taken a second time for the refinement of :1357-1389: whether that
+	     * happens is a pure function of the first result and the loop state, so it is decided here and the
+	     * state machine below only merges the outcome */
+	    Found first = { 0.f, 0.f, 0u, 0u, 0u }, refined = { 0.f, 0.f, 0u, 0u, 0u };
+	    unsigned step = try_step;
+	    float limit = lc.confidence_search_limit;
+	    int which = sel;
+	    for (int pass = 0;; pass++) {
+		nsearch += MODE != 1;		/* (the generic path counts nothing) */
+		Found f;
+		if (MODE == 3) {
+		    /* :1265, :1378 from the chunk-prefix table of this iteration's search span, built once
+		     * (before the coarse search) for both */
+		    /* (shared-window addresses turned back into pointers here, so that the loads stay LDS/STS) */
+		    const float *ringp = static_cast<const float *>(__cvta_shared_to_generic(rg.ring_s));
+		    float4 *pre = static_cast<float4 *>(__cvta_shared_to_generic(pre_s));
+		    float4 *tot = static_cast<float4 *>(__cvta_shared_to_generic(tot_s));
+		    const float4 *twc = static_cast<const float4 *>(__cvta_shared_to_generic(tw_s));
+		    const float4 *locp = static_cast<const float4 *>(__cvta_shared_to_generic(loc_s));
+		    float4 *redp = static_cast<float4 *>(__cvta_shared_to_generic(red_s));
+		    const unsigned base = ring.pos_off & ~3u;
+		    if (pass == 0) {
+			if (pending) {
+			    cp_async_wait<0>();
 			    __syncwarp(gmask);
+			    pending = false;
 			}
-			f = pfx_search<LB>(ringp, R, base, pos_off & 3u, pre, tot, twc, tw_sample, pg, geo, pfl, which,
-				try_first, pg.kind[(carrier ? 1 : 0) + (pass ? 2 : 0)], limit, lane, redp, ncand);
-		    } else if (MODE == 2) {
-			/* :1265, :1378 from shared segment sums.  Which plan: the window is the one chosen at the
-			 * top of the iteration (carrier then), coarse or fine.  A coarse search in the steady
-			 * state ends at its first candidate (:499), and one candidate alone is cheapest analysed
-			 * by itself: that is tried first unless the previous coarse search of this stream needed
-			 * more than one (mhint); the fine search visits all of its candidates anyway. */
-			const fsk_b200_mkind &kind = mp.kind[(carrier ? 1 : 0) + (pass ? 2 : 0)];
-			Found seed = { 0.f, 0.f, 0u, 0u, 0u };
-			unsigned skip = 0;
-			bool decided = false;
-			if (pass == 0 && !mhint && !mp.always) {
-			    unsigned lo, hi;
-			    float am;
-			    const float c = frame_analyze_fast<G, W, L, true, LaneWinM<W> >(rg,
-				    ring_wrap(pos_off + try_first, R), geo, lwm, which, tw_s, g, gmask, lo, hi, am,
-				    pending);
-			    ncand++;
-			    if (0.f < c) {					/* src/fsk.c:492 */
-				seed = Found{ c, am, try_first, lo, hi };
-				decided = c >= limit;			/* :499 */
-			    }
-			    skip = 1;
-			    mhint = !decided;
-			}
-			if (decided)
-			    f = seed;
-			else {
-			    const FoundN r = find_frame_multi<G, W, L>(rg, pos_off, geo, lwm, which, tw_s, g, gmask,
-				    kind, limit, pending, seed, skip);
-			    f = r.f;
-			    ncand += r.ncand;
-			    if (pass == 0 && !skip)
-				mhint = r.ncand > 1u;
-			}
-		    } else if (MODE == 0 && pass == 1 && lc.slide)
-			/* :1373, the fine search: its candidates in ascending order, each from the one before */
-			f = find_frame_slide<G, W, L>(rg, pos_off, geo, lw, which, tw_s, g, gmask, try_first, try_max,
-				step, ncand);
-		    else
-			f = find_frame_fast_body<G, W, L>(rg, pos_off, geo, lw, which, tw_s, g,
-				gmask, try_first, try_max, step, limit, pending, ncand);
-		    if (pass) {
-			refined = f;
-			break;
+			pfx_build(ringp, R, base, ((ring.pos_off & 3u) + try_max - 1u + geo.span) / 4u + 1u, pre, tot,
+				twc, locp, pg, pfl, lane);
+			__syncwarp(gmask);
 		    }
-		    first = f;
-		    float c = f.confidence;
-		    const bool below_peak = c < peak_confidence * 0.75f;	/* :1278 */
-		    if (f.amplitude < track_amplitude * 0.25f)		/* :1286 */
-			c = 0.f;
-		    if (!(c > lc.confidence_threshold) || !(below_peak || !carrier) || !(c < INFINITY)
-			    || try_step <= 1u)
-			break;
-		    step = try_max / 8u;
-		    if (step == 0)
-			step = 1;
-		    limit = INFINITY;
-		    which = 0;
-		    pending = false;
-		}
-		confidence = first.confidence;
-		amplitude = first.amplitude;
-		frame_start = first.start;
-		bits = ((unsigned long long)first.bits_hi << 32) | first.bits_lo;
-		if (FILL == 0) {
-		    /* The searches are over, so the samples before the next start are dead: ask for
-		     * the next iteration's samples now, ahead of the bookkeeping below, instead of
-		     * right before they are needed.  `adv` restates the advance of :1318/:1407;
-		     * should it ever be short, the top of the loop asks for the rest. */
-		    float c = first.confidence;
-		    if (first.amplitude < track_amplitude * 0.25f)
-			c = 0.f;
-		    const unsigned fs = refined.confidence > first.confidence ? refined.start : first.start;
-		    const unsigned adv = c <= lc.confidence_threshold ? try_max
-			    : fs + lc.frame_nsamples - lc.nsamples_overscan;
-		    const unsigned npos = pos + adv;
-		    if (adv <= remaining && filled >= (npos & ~AL)) {
-			__syncwarp(gmask);	/* every read of this window precedes the copies */
-			request_at(reach(npos, lookahead), npos);
+		    f = pfx_search<LB>(ringp, R, base, ring.pos_off & 3u, pre, tot, twc, tw_sample, pg, geo, pfl, which,
+			    try_first, pg.kind[(carrier ? 1 : 0) + (pass ? 2 : 0)], limit, lane, redp, ncand);
+		} else if (MODE == 2) {
+		    /* :1265, :1378 from shared segment sums.  Which plan: the window is the one chosen at the
+		     * top of the iteration (carrier then), coarse or fine.  A coarse search in the steady
+		     * state ends at its first candidate (:499), and one candidate alone is cheapest analysed
+		     * by itself: that is tried first unless the previous coarse search of this stream needed
+		     * more than one (mhint); the fine search visits all of its candidates anyway. */
+		    const fsk_b200_mkind &kind = mp.kind[(carrier ? 1 : 0) + (pass ? 2 : 0)];
+		    Found seed = { 0.f, 0.f, 0u, 0u, 0u };
+		    unsigned skip = 0;
+		    bool decided = false;
+		    if (pass == 0 && !mhint && !mp.always) {
+			unsigned lo, hi;
+			float am;
+			const float c = frame_analyze_fast<G, W, L, true, LaneWinM<W> >(rg,
+				ring_wrap(ring.pos_off + try_first, R), geo, lwm, which, tw_s, g, gmask, lo, hi, am,
+				pending);
+			ncand++;
+			if (0.f < c) {					/* src/fsk.c:492 */
+			    seed = Found{ c, am, try_first, lo, hi };
+			    decided = c >= limit;			/* :499 */
+			}
+			skip = 1;
+			mhint = !decided;
 		    }
-		    /* (The bulk fill of MODE 3 asks at the top of the next iteration.  Asking here as well
-		     * costs one more barrier phase per iteration, and the state machine below is too short
-		     * to hide a copy; the other warps of the SM do that already.) */
+		    if (decided)
+			f = seed;
+		    else {
+			const FoundN r = find_frame_multi<G, W, L>(rg, ring.pos_off, geo, lwm, which, tw_s, g, gmask,
+				kind, limit, pending, seed, skip);
+			f = r.f;
+			ncand += r.ncand;
+			if (pass == 0 && !skip)
+			    mhint = r.ncand > 1u;
+		    }
+		} else if (MODE == 1) {		/* global memory, indexed from `pos` (< n) so that indices stay small */
+		    const typename RowOf<SRC>::Src src = { x + pos, n - pos };
+		    unsigned long long b;
+		    f.confidence = find_frame<G, typename RowOf<SRC>::Src>(src, 0u, geo, which, sm.tw, sm.scr, g,
+			    gmask, try_first, try_max, step, limit, b, f.amplitude, f.start);
+		    f.bits_lo = (unsigned)b;
+		    f.bits_hi = (unsigned)(b >> 32);
+		} else if (MODE == 0 && pass == 1 && lc.slide)
+		    /* :1373, the fine search: its candidates in ascending order, each from the one before */
+		    f = find_frame_slide<G, W, L>(rg, ring.pos_off, geo, lw, which, tw_s, g, gmask, try_first, try_max,
+			    step, ncand);
+		else
+		    f = find_frame_fast_body<G, W, L>(rg, ring.pos_off, geo, lw, which, tw_s, g,
+			    gmask, try_first, try_max, step, limit, pending, ncand);
+		if (pass) {
+		    refined = f;
+		    break;
 		}
-	    } else if (SRC)
-		confidence = find_frame<G, GlobalSrc16>(gsrc16, 0u, geo, sel, sm.tw, sm.scr, g, gmask,
-			try_first, try_max, try_step, lc.confidence_search_limit,
-			bits, amplitude, frame_start);
-	    else
-		confidence = find_frame<G, GlobalSrc>(gsrc, 0u, geo, sel, sm.tw, sm.scr, g, gmask,
-			try_first, try_max, try_step, lc.confidence_search_limit,
-			bits, amplitude, frame_start);
+		first = f;
+		float c = f.confidence;
+		const bool below_peak = c < peak_confidence * 0.75f;	/* :1278 */
+		if (f.amplitude < track_amplitude * 0.25f)		/* :1286 */
+		    c = 0.f;
+		if (!(c > lc.confidence_threshold) || !(below_peak || !carrier) || !(c < INFINITY)
+			|| try_step <= 1u)
+		    break;
+		step = try_max / 8u;
+		if (step == 0)
+		    step = 1;
+		limit = INFINITY;
+		which = 0;
+		pending = false;
+	    }
+	    float confidence = first.confidence, amplitude = first.amplitude;
+	    unsigned frame_start = first.start;
+	    unsigned long long bits = ((unsigned long long)first.bits_hi << 32) | first.bits_lo;
+	    if (MODE != 1 && FILL == 0) {
+		/* ask for the next iteration's samples now, ahead of the bookkeeping below.  `adv` restates the
+		 * advance of :1318/:1407; should it ever be short, the top of the loop asks for the rest. */
+		float c = first.confidence;
+		if (first.amplitude < track_amplitude * 0.25f)
+		    c = 0.f;
+		const unsigned fs = refined.confidence > first.confidence ? refined.start : first.start;
+		const unsigned adv = c <= lc.confidence_threshold ? try_max
+			: fs + lc.frame_nsamples - lc.nsamples_overscan;
+		const unsigned npos = pos + adv;
+		if (adv <= remaining && ring.filled >= (npos & ~ring.AL))
+		    ring.request_next(npos, lookahead);
+		/* (The bulk fill of MODE 3 asks at the loop top.  Asking here as well costs one more barrier phase per
+		 * iteration, and the state machine is too short to hide a copy; the SM's other warps do that.) */
+	    }
 
 	    bool want_refine = false;
 	    if (confidence < peak_confidence * 0.75f) {		/* :1278-1282 */
@@ -791,31 +631,13 @@ k_rx(const __grid_constant__ fsk_b200_geom geo, const __grid_constant__ fsk_b200
 		    acquired = FSK_B200_FRAME_ACQUIRED;
 		    want_refine = true;
 		}
-		if (want_refine && confidence < INFINITY && try_step > 1u) {	/* :1357-1389 */
-		    try_step = try_max / 8u;
-		    if (try_step == 0)
-			try_step = 1;
-		    unsigned long long bits2;
-		    float amplitude2, confidence2;
-		    unsigned frame_start2;
-		    /* `carrier` is 1 by now, so the data string is searched (:1378) */
-		    if (MODE != 1) {
-			confidence2 = refined.confidence;	/* searched above */
-			amplitude2 = refined.amplitude;
-			frame_start2 = refined.start;
-			bits2 = ((unsigned long long)refined.bits_hi << 32) | refined.bits_lo;
-		    } else if (SRC)
-			confidence2 = find_frame<G, GlobalSrc16>(gsrc16, 0u, geo, 0, sm.tw, sm.scr, g,
-				gmask, try_first, try_max, try_step, INFINITY,
-				bits2, amplitude2, frame_start2);
-		    else
-			confidence2 = find_frame<G, GlobalSrc>(gsrc, 0u, geo, 0, sm.tw, sm.scr, g,
-				gmask, try_first, try_max, try_step, INFINITY,
-				bits2, amplitude2, frame_start2);
-		    if (confidence2 > confidence) {
+		/* :1357-1389, searched above (`carrier` is 1 by now, so the data string was searched, :1378) */
+		if (want_refine && confidence < INFINITY && try_step > 1u) {
+		    const unsigned long long bits2 = ((unsigned long long)refined.bits_hi << 32) | refined.bits_lo;
+		    if (refined.confidence > confidence) {
 			bits = bits2;
-			amplitude = amplitude2;
-			frame_start = frame_start2;
+			amplitude = refined.amplitude;
+			frame_start = refined.start;
 		    }
 		}
 		track_amplitude = (track_amplitude + amplitude) / 2.f;	/* :1391 */
@@ -836,23 +658,11 @@ k_rx(const __grid_constant__ fsk_b200_geom geo, const __grid_constant__ fsk_b200
 	    pos += advance;
 	    if (AUTO == 1)
 		vring = advance >= vring ? 0u : vring - advance;
-	    if (MODE != 1) {
-		pos_off = ring_wrap(pos_off + advance, R);	/* advance < R by construction */
-		if (filled < (pos & ~AL)) {
-		    /* skipped past everything requested so far: restart the ring here */
-		    drain();
-		    filled = pos & ~AL;
-		    pos_off = pos & AL;
-		    fdst = dst0;
-		    fsrc = SRC ? x : x + filled + 4u * g;
-		    conv = filled;
-		    coff = 0;
-		}
-		__syncwarp(gmask);	/* every read of this window precedes the next copies */
-	    }
+	    if (MODE != 1)
+		ring.advance(pos, advance);
 	}
 	if (MODE != 1)
-	    drain();	/* before the slot is reused or the block exits */
+	    ring.drain();	/* before the slot is reused or the block exits */
 
 	if (g == 0) {
 	    st.pos = pos;
